@@ -3,22 +3,25 @@
 //   forward  Y[n x d]  = X[n x k] W[d x k]^T + b          (nn.Linear, Models.py:145-150)
 //   wgrad    dW[d x k] = dY[n x d]^T X[n x k], db = colsum(dY)   (its autograd; X is a constant feature table)
 //
-// Both are HBM-bound (32-64 flop/B at d = 64-128): the job of the kernel is to stream X once at HBM speed.  All 8
-// projections of a step run as ONE grouped launch (one CTA per 128-row tile / work item, looked up in a problem table)
-// -- a single projection has only ~136 row tiles.
+// Both are HBM-bound at d = 64 (the job of the kernel is to stream X once at HBM speed) with the tensor work not far behind.
+// All 8 projections of a step run as ONE grouped launch: a persistent grid (one CTA per SM) walks the work units -- 256-row
+// tiles (fwd) / (256-feature tile x row chunk) items (wgrad), 128 above d = 128 or when 256 would leave SMs idle -- looked up in
+// a problem table, long-K problems first.
 //
-// Precision: fp32 operands are split  x = hi + lo  (hi = top 19 bits, exactly TF32-representable) while the tile sits in
-// shared memory, and three tf32 wgmmas accumulate lo*hi + hi*lo + hi*hi in fp32 registers ("3xTF32", error ~2^-21
-// relative per product, i.e. fp32-class).  mode 1 skips the split (plain TF32, ~2^-11).
+// Precision: fp32 operands are split  x = hi + lo  (hi = top 19 bits, exactly TF32-representable) and three tf32 wgmmas
+// accumulate lo*hi + hi*lo + hi*hi in fp32 registers ("3xTF32", error ~2^-21 relative per product, i.e. fp32-class).  mode 1
+// skips the split (plain TF32, ~2^-11).
 //
-// CTA = two warpgroups (256 threads), each owning 64 rows (fwd) / 64 features (wgrad) of the 128-wide tile; thread 0
-// keeps a ring of TMA loads in flight (one mbarrier per stage) while the CTA transforms and multiplies the oldest stage.
-// wgmma takes tf32 operands K-major only:
-//   forward  X tile [128 rows][32 k] and W tile [d rows][32 k] arrive K-major with the 128-byte swizzle straight from TMA;
-//            the split is elementwise (hi in place, lo in a twin buffer at the same swizzled positions).
-//   wgrad    the contraction runs over ROWS, so the X tile [32 rows][128 features] and dY tile [32 rows][d] arrive row-major
-//            (no swizzle) and the transform pass writes them transposed -- [128 features][32 rows], [d][32 rows], 128-byte
-//            swizzled -- splitting as it goes; no transposed copy of X or dY ever exists in global memory.
+// CTA = 3 warpgroups.  Warpgroup 0 is the producer: one thread keeps a ring of TMA stages in flight (a full and an empty
+// mbarrier per stage), running ahead across work units; it hands most of its registers to the two consumer warpgroups
+// (setmaxnreg).  Each consumer owns MB blocks of 64 rows (fwd) / features (wgrad) of the tile.  X goes into wgmma A-fragment
+// REGISTERS straight from the stage and is split there; B (W or dY^T, hi and lo) is consumed from shared memory as it arrived
+// from TMA, ready-made: W is split once per step by `wsplit`, dY^T is transposed and split once per step by `dyt_split`.  One
+// wgmma group (one k8 step) stays in flight while the next A fragment is loaded; no CTA-wide barrier in the main loop.
+//   forward  A = X[rows][k]: the X tile [TM rows][32 k] arrives K-major with the 128-byte swizzle, exactly the A layout.
+//   wgrad    A = X^T (M = features, K = rows): the fragment is read transposed out of the raw X tile, which arrives as TM/32
+//            boxes [32 rows][32 features] with the 128-byte swizzle; features are permuted inside the tile so that the reads
+//            are bank-conflict free (arithmetic at ld_frag_wgrad), and the epilogue undoes the permutation.
 #include <mutex>
 #include <stdlib.h>
 #include <vector>
@@ -82,265 +85,268 @@ __device__ __forceinline__ uint8_t* align1024(uint8_t* p) {
 }
 
 // ------------------------------------------------------------------------------------------------
-// forward
+// one main loop for both directions
 // ------------------------------------------------------------------------------------------------
-template <int D, bool SPLIT>
-__global__ void __launch_bounds__(256, D <= 128 ? 2 : 1) proj_fwd_tc_kernel(const __grid_constant__ FwdParams P) {
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = align1024(smem_raw);
-  constexpr int NC = D / 32;
-  constexpr uint32_t kB = D * 128u;
-  constexpr uint32_t stage_bytes = (kTileA + kB) * (SPLIT ? 2u : 1u);
-  const int stages = P.stages;
-  uint64_t* full = reinterpret_cast<uint64_t*>(smem + (size_t)stages * stage_bytes);
-  auto sA = [&](int s) { return smem + (size_t)s * stage_bytes; };
-  auto sAlo = [&](int s) { return sA(s) + kTileA; };
-  auto sB = [&](int s) { return sA(s) + kTileA * (SPLIT ? 2u : 1u); };
-  auto sBlo = [&](int s) { return sB(s) + kB; };
+constexpr uint32_t kSmemMax = 227u * 1024u;   // dynamic shared memory per block on sm_90
+constexpr int kProducerRegs = 40, kConsumerRegs = 232;   // 128 * 40 + 256 * 232 <= 65536 (launched at 384 x 168)
 
-  const int tid = threadIdx.x, wg = tid >> 7, warp = (tid >> 5) & 3, lane = tid & 31;
-  int p = 0;
-  while (p + 1 < P.n_prob && (int)blockIdx.x >= P.prob[p + 1].tile_start) ++p;
-  const FwdProblem pr = P.prob[p];
-  const int mblk = blockIdx.x - pr.tile_start, kb_n = pr.kblocks;
-  const CUtensorMap* tmA = &P.tmA[p];
-  const CUtensorMap* tmW = &P.tmW[p];
-  auto issue = [&](int kb) {
-    const int s = kb % stages;
-    mbar_arrive_expect_tx(&full[s], stage_bytes - (SPLIT ? kTileA : 0u));
-    tma_load_2d(sA(s), tmA, &full[s], kb * BK, mblk * BM);
-    tma_load_2d(sB(s), tmW, &full[s], kb * BK, 0);
-    if (SPLIT) tma_load_2d(sBlo(s), tmW, &full[s], kb * BK, D);
-  };
-  if (tid == 0) {
-    prefetch_tmap(tmA); prefetch_tmap(tmW);
-    for (int s = 0; s < stages; ++s) mbar_init(&full[s], 1);
-    fence_barrier_init();
-    for (int kb = 0; kb < stages && kb < kb_n; ++kb) issue(kb);
+template <int D, bool SPLIT, int MB>
+struct ProjCfg {
+  static constexpr int TM = tile_m(MB);
+  static constexpr uint32_t kX = TM * BK * 4u;                 // X tile of one stage
+  static constexpr uint32_t kB = D * BK * 4u;                  // one B operand tile [D][32], hi or lo
+  static constexpr uint32_t kStage = kX + kB * (SPLIT ? 2u : 1u);
+  static constexpr int kFit = (int)((kSmemMax - 1024u - 256u) / kStage);
+  static constexpr int kStages = kFit > 4 ? 4 : kFit;          // 4 at d = 64, 3 at d = 128, 2 at d = 256
+  static constexpr uint32_t kSmem = 1024u /*align slack*/ + kStages * kStage + 2u * kStages * 8u;
+  static_assert(kStages >= 2, "projection ring needs two stages");
+};
+
+// A fragment (4 registers, layout at WgmmaRS) of k8 step kk for m64 block `blk` (0 .. 2MB-1 over the CTA), read from the stage's X
+// tile.  Forward: A(m, k) = X tile row m, column k; element (r, c) sits at r*128 + ((c/4) ^ (r%8))*16 + (c%4)*4.  A warp's 32
+// lanes read rows 16w + g (r%8 = g), chunk (2kk) ^ g or (2kk+1) ^ g, word t: 8 chunks x 4 words = 32 banks, conflict free.
+__device__ __forceinline__ void ld_frag_fwd(uint32_t (&a)[4], uint32_t sx, int blk, int kk, int warp, int lane) {
+  const int g = lane >> 2, t = lane & 3;
+  const uint32_t row = sx + (blk * 64 + warp * 16 + g) * 128 + t * 4;
+  const uint32_t c0 = ((2 * kk) ^ g) << 4, c1 = c0 ^ 16;
+  a[0] = lds_u32(row + c0);
+  a[1] = lds_u32(row + 1024 + c0);
+  a[2] = lds_u32(row + c1);
+  a[3] = lds_u32(row + 1024 + c1);
+}
+// Wgrad: A(m, k) = X[row k][feature phi(m)] out of boxes [32 rows][32 features] (4 KiB, same swizzle, r%8 = row%8).
+// Fragment row m = 16w + 8h + g (h = 0 for a0/a2, 1 for a1/a3), k = t (a0/a1) or t + 4 (a2/a3) within k8 step kk (rows 8kk..).
+// Feature map inside the block's 64 features:  phi(m) = 32(w/2) + 8(w%2) + 4h + (g%4) + 16(g/4), a bijection onto 0..63
+// (bits: g%4 -> 0-1, h -> 2, w%2 -> 3, g/4 -> 4, w/2 -> 5).  In box w/2 the element sits in chunk q = 2(w%2) + h + 4(g/4), word g%4.
+// Banks of one load (fixed w, h, kk; lanes vary g, t): chunk q ^ (row % 8) = (2(w%2) + h + 4(g/4)) ^ t [^ 4 for k = t + 4];
+// t < 4 only touches bits 0-1, so (g/4, t) -> 8 distinct chunks, times word g%4 -> 32 distinct banks: conflict free.
+__device__ __forceinline__ int wgrad_feature(int blk, int warp, int h, int g) {
+  return blk * 64 + 32 * (warp >> 1) + 8 * (warp & 1) + 4 * h + (g & 3) + 16 * (g >> 2);
+}
+__device__ __forceinline__ void ld_frag_wgrad(uint32_t (&a)[4], uint32_t sx, int blk, int kk, int warp, int lane) {
+  const int g = lane >> 2, t = lane & 3;
+  const uint32_t base = sx + (blk * 2 + (warp >> 1)) * 4096 + kk * 1024 + t * 128 + (g & 3) * 4;
+  const uint32_t q = (2 * (warp & 1) + 4 * (g >> 2)) ^ t;
+  a[0] = lds_u32(base + (q << 4));
+  a[1] = lds_u32(base + ((q ^ 1) << 4));
+  a[2] = lds_u32(base + 512 + ((q ^ 4) << 4));
+  a[3] = lds_u32(base + 512 + ((q ^ 5) << 4));
+}
+
+// work unit -> (problem, number of k-blocks, what the producer loads for k-block kb, where the epilogue writes)
+template <int D, bool SPLIT, int MB>
+struct FwdUnit {
+  using Cfg = ProjCfg<D, SPLIT, MB>;
+  const FwdParams& P; int p, mblk, kb_n;
+  __device__ FwdUnit(const FwdParams& P_, int u) : P(P_) {
+    p = 0;
+    while (p + 1 < P.n_prob && u >= P.prob[p + 1].tile_start) ++p;
+    mblk = u - P.prob[p].tile_start;
+    kb_n = P.prob[p].kblocks;
   }
-  __syncthreads();
-
-  float acc[NC][16];
+  __device__ void issue(uint8_t* st, uint64_t* bar, int kb, uint64_t pol) const {
+    tma_load_2d_hint(st, &P.tmA[p], bar, kb * BK, mblk * Cfg::TM, pol);
+    tma_load_2d(st + Cfg::kX, &P.tmW[p], bar, kb * BK, 0);
+    if (SPLIT) tma_load_2d(st + Cfg::kX + Cfg::kB, &P.tmW[p], bar, kb * BK, D);
+  }
+  static __device__ void ld_frag(uint32_t (&a)[4], uint32_t sx, int blk, int kk, int warp, int lane) { ld_frag_fwd(a, sx, blk, kk, warp, lane); }
+  __device__ void store(float (&acc)[MB][D / 2], int cw, int warp, int lane) const {   // registers (+bias) -> Y
+    const FwdProblem& pr = P.prob[p];
+    const int g = lane >> 2, t = lane & 3;
 #pragma unroll
-  for (int c = 0; c < NC; ++c)
+    for (int j = 0; j < MB; ++j) {
+      const int row0 = mblk * Cfg::TM + (cw * MB + j) * 64 + warp * 16 + g;
 #pragma unroll
-    for (int i = 0; i < 16; ++i) acc[c][i] = 0.f;
-
-  for (int kb = 0; kb < kb_n; ++kb) {
-    const int s = kb % stages;
-    mbar_wait(&full[s], (uint32_t)(kb / stages) & 1u);
-    if (SPLIT) {
-      split_tile_inplace(reinterpret_cast<float4*>(sA(s)), reinterpret_cast<float4*>(sAlo(s)), kTileA / 16, tid, 256);
-      fence_proxy_async_smem();
-      __syncthreads();
-    }
-    const uint32_t a0 = smem_u32(sA(s)) + wg * 8192u, al0 = smem_u32(sAlo(s)) + wg * 8192u;
-    const uint32_t b0 = smem_u32(sB(s)), bl0 = smem_u32(sBlo(s));
-    wgmma_fence();
+      for (int c = 0; c < D / 8; ++c) {
+        const int col = c * 8 + 2 * t;
+        const float2 b = pr.bias ? __ldg(reinterpret_cast<const float2*>(pr.bias + col)) : make_float2(0.f, 0.f);
 #pragma unroll
-    for (int kk = 0; kk < 4; ++kk) {  // k8 = 32 bytes inside the 128-byte swizzle row
-#pragma unroll
-      for (int c = 0; c < NC; ++c) {  // 32 output columns = 32 rows of W = 4 KiB
-        const uint64_t bd = gmma_desc_sw128(b0 + c * 4096u + kk * 32u);
-        if (SPLIT) {
-          wgmma_m64n32k8_tf32(acc[c], gmma_desc_sw128(al0 + kk * 32u), bd, 1);                                 // lo * hi
-          wgmma_m64n32k8_tf32(acc[c], gmma_desc_sw128(a0 + kk * 32u), gmma_desc_sw128(bl0 + c * 4096u + kk * 32u), 1);  // hi * lo
-          wgmma_m64n32k8_tf32(acc[c], gmma_desc_sw128(a0 + kk * 32u), bd, 1);                                  // hi * hi
-        } else {
-          wgmma_m64n32k8_tf32(acc[c], gmma_desc_sw128(a0 + kk * 32u), bd, 1);
+        for (int h = 0; h < 2; ++h) {
+          const int row = row0 + 8 * h;
+          if (row < pr.n)
+            *reinterpret_cast<float2*>(pr.Y + (long long)row * pr.ldy + col) = make_float2(acc[j][4 * c + 2 * h] + b.x, acc[j][4 * c + 2 * h + 1] + b.y);
         }
       }
     }
-    wgmma_commit();
-    wgmma_wait<0>();
-    __syncthreads();   // every warpgroup is done with stage s
-    if (tid == 0 && kb + stages < kb_n) issue(kb + stages);
   }
+};
 
-  // epilogue: registers (+bias) -> global
-  const int row0 = mblk * BM + wg * 64 + warp * 16 + (lane >> 2);
+template <int D, bool SPLIT, int MB>
+struct WgUnit {
+  using Cfg = ProjCfg<D, SPLIT, MB>;
+  const WgParams& P; int p, u, ft, r0, kb_n;
+  __device__ WgUnit(const WgParams& P_, int u_) : P(P_), u(u_) {
+    p = 0;
+    while (p + 1 < P.n_prob && u >= P.prob[p + 1].item_start) ++p;
+    const WgProblem& pr = P.prob[p];
+    const int local = u - pr.item_start, chunk = local / pr.ft_tiles;
+    ft = local - chunk * pr.ft_tiles;
+    r0 = chunk * pr.rows_per_chunk;
+    kb_n = (min(pr.n, r0 + pr.rows_per_chunk) - r0 + BK - 1) / BK;   // chunks are BK-aligned; rows past n load as zeros
+  }
+  __device__ void issue(uint8_t* st, uint64_t* bar, int kb, uint64_t pol) const {
+    const int r = r0 + kb * BK;
 #pragma unroll
-  for (int c = 0; c < NC; ++c) {
+    for (int b = 0; b < Cfg::TM / 32; ++b) tma_load_2d_hint(st + b * 4096, &P.tmX[p], bar, ft * Cfg::TM + 32 * b, r, pol);
+    tma_load_2d(st + Cfg::kX, &P.tmG[p], bar, r, 0);
+    if (SPLIT) tma_load_2d(st + Cfg::kX + Cfg::kB, &P.tmG[p], bar, r, D);
+  }
+  static __device__ void ld_frag(uint32_t (&a)[4], uint32_t sx, int blk, int kk, int warp, int lane) { ld_frag_wgrad(a, sx, blk, kk, warp, lane); }
+  __device__ void store(float (&acc)[MB][D / 2], int cw, int warp, int lane) const {   // registers -> partial[item][feature][d]
+    const int g = lane >> 2, t = lane & 3;
+    float* out = P.partial + (long long)u * Cfg::TM * D;
 #pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      const int col = c * 32 + j * 8 + (lane & 3) * 2;
-      const float2 b = pr.bias ? __ldg(reinterpret_cast<const float2*>(pr.bias + col)) : make_float2(0.f, 0.f);
+    for (int j = 0; j < MB; ++j)
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
-        const int row = row0 + 8 * h;
-        if (row < pr.n)
-          *reinterpret_cast<float2*>(pr.Y + (long long)row * pr.ldy + col) = make_float2(acc[c][4 * j + 2 * h] + b.x, acc[c][4 * j + 2 * h + 1] + b.y);
+        float* o = out + (long long)wgrad_feature(cw * MB + j, warp, h, g) * D + 2 * t;
+#pragma unroll
+        for (int c = 0; c < D / 8; ++c) *reinterpret_cast<float2*>(o + c * 8) = make_float2(acc[j][4 * c + 2 * h], acc[j][4 * c + 2 * h + 1]);
       }
-    }
   }
-}
+};
 
-// ------------------------------------------------------------------------------------------------
-// wgrad
-// ------------------------------------------------------------------------------------------------
-template <int D, bool SPLIT>
-__global__ void __launch_bounds__(256, D <= 128 ? 2 : 1) proj_wgrad_tc_kernel(const __grid_constant__ WgParams P) {
+template <int D, bool SPLIT, int MB, class Unit, class Params>
+__device__ __forceinline__ void proj_pipeline(const Params& P, int total) {
+  using Cfg = ProjCfg<D, SPLIT, MB>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = align1024(smem_raw);
-  constexpr int NC = D / 32;
-  constexpr uint32_t kB = D * 128u;               // [D][32 rows] operand tile == raw [32 rows][D] tile
-  constexpr uint32_t raw_bytes = kTileA + kB;     // raw X [32][128] | raw dY [32][D]
-  const int stages = P.stages;
-  uint8_t* opA = smem + (size_t)stages * raw_bytes;   // A_hi | A_lo | B_hi | B_lo (K-major, swizzled)
-  uint8_t* opAlo = opA + kTileA;
-  uint8_t* opB = opA + kTileA * (SPLIT ? 2u : 1u);
-  uint8_t* opBlo = opB + kB;
-  uint64_t* full = reinterpret_cast<uint64_t*>(opB + kB * (SPLIT ? 2u : 1u));
-  auto rawX = [&](int s) { return reinterpret_cast<const float*>(smem + (size_t)s * raw_bytes); };
-  auto rawG = [&](int s) { return reinterpret_cast<const float*>(smem + (size_t)s * raw_bytes + kTileA); };
-
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem + Cfg::kStages * Cfg::kStage);
+  uint64_t* empty = full + Cfg::kStages;
   const int tid = threadIdx.x, wg = tid >> 7, warp = (tid >> 5) & 3, lane = tid & 31;
-  // item -> (problem, feature tile, row range)
-  const int item = blockIdx.x;
-  int p = 0;
-  while (p + 1 < P.n_prob && item >= P.prob[p + 1].item_start) ++p;
-  const WgProblem pr = P.prob[p];
-  const int local = item - pr.item_start;
-  const int chunk = local / pr.ft_tiles;
-  const int ft = local - chunk * pr.ft_tiles;
-  const int r0 = chunk * pr.rows_per_chunk;
-  const int kb_n = (min(pr.n, r0 + pr.rows_per_chunk) - r0 + BK - 1) / BK;   // chunks are BK-aligned; rows past n load as zeros
-  const CUtensorMap* tmX = &P.tmX[p];
-  const CUtensorMap* tmG = &P.tmG[p];
-  auto issue = [&](int kb) {
-    const int s = kb % stages;
-    uint8_t* dst = smem + (size_t)s * raw_bytes;
-    mbar_arrive_expect_tx(&full[s], raw_bytes);
-    tma_load_2d(dst, tmX, &full[s], ft * BM, r0 + kb * BK);
-    tma_load_2d(dst + kTileA, tmG, &full[s], 0, r0 + kb * BK);
-  };
   if (tid == 0) {
-    prefetch_tmap(tmX); prefetch_tmap(tmG);
-    for (int s = 0; s < stages; ++s) mbar_init(&full[s], 1);
+    for (int s = 0; s < Cfg::kStages; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 8); }   // empty: one arrival per consumer warp
     fence_barrier_init();
-    for (int kb = 0; kb < stages && kb < kb_n; ++kb) issue(kb);
   }
   __syncthreads();
 
-  float acc[NC][16];
-#pragma unroll
-  for (int c = 0; c < NC; ++c)
-#pragma unroll
-    for (int i = 0; i < 16; ++i) acc[c][i] = 0.f;
+  if (wg == 0) {   // producer warpgroup: one thread issues every load, across work units
+    setmaxnreg_dec<kProducerRegs>();
+    if (tid == 0) {
+      const uint64_t pol = l2_policy_evict_first();
+      int s = 0; uint32_t ph = 0;
+      for (int u = blockIdx.x; u < total; u += gridDim.x) {
+        const Unit w(P, u);
+        for (int kb = 0; kb < w.kb_n; ++kb) {
+          mbar_wait(&empty[s], ph ^ 1u);
+          mbar_arrive_expect_tx(&full[s], Cfg::kStage);
+          w.issue(smem + s * Cfg::kStage, &full[s], kb, pol);
+          if (++s == Cfg::kStages) { s = 0; ph ^= 1u; }
+        }
+      }
+    }
+    return;
+  }
 
-  for (int kb = 0; kb < kb_n; ++kb) {
-    const int s = kb % stages;
-    mbar_wait(&full[s], (uint32_t)(kb / stages) & 1u);
-    // transpose + split: A[f][r] = X[r][f] (thread: one feature, 16 rows), B[e][r] = dY[r][e]; 4 rows -> one 16-byte chunk
-    {
-      const float* x = rawX(s);
-      const int f = tid & 127, rh = tid >> 7;
+  setmaxnreg_inc<kConsumerRegs>();
+  const int cw = wg - 1;   // consumer warpgroup 0 / 1
+  int s = 0; uint32_t ph = 0;
+  float acc[MB][D / 2];
+  for (int u = blockIdx.x; u < total; u += gridDim.x) {
+    const Unit w(P, u);
 #pragma unroll
-      for (int q = rh * 4; q < rh * 4 + 4; ++q) {
-        const float4 v = make_float4(x[(4 * q) * BM + f], x[(4 * q + 1) * BM + f], x[(4 * q + 2) * BM + f], x[(4 * q + 3) * BM + f]);
-        const uint32_t off = sw128_off(f, q);
-        if (SPLIT) {
-          float4 h, l;
-          split4(v, h, l);
-          *reinterpret_cast<float4*>(opA + off) = h;
-          *reinterpret_cast<float4*>(opAlo + off) = l;
-        } else {
-          *reinterpret_cast<float4*>(opA + off) = v;
-        }
-      }
-      const float* g = rawG(s);
+    for (int j = 0; j < MB; ++j)
 #pragma unroll
-      for (int i = tid; i < D * 8; i += 256) {
-        const int e = i % D, q = i / D;
-        const float4 v = make_float4(g[(4 * q) * D + e], g[(4 * q + 1) * D + e], g[(4 * q + 2) * D + e], g[(4 * q + 3) * D + e]);
-        const uint32_t off = sw128_off(e, q);
-        if (SPLIT) {
-          float4 h, l;
-          split4(v, h, l);
-          *reinterpret_cast<float4*>(opB + off) = h;
-          *reinterpret_cast<float4*>(opBlo + off) = l;
-        } else {
-          *reinterpret_cast<float4*>(opB + off) = v;
+      for (int i = 0; i < D / 2; ++i) acc[j][i] = 0.f;
+    int prev = -1;
+    for (int kb = 0; kb < w.kb_n; ++kb) {
+      mbar_wait(&full[s], ph);
+      const uint32_t st = smem_u32(smem + s * Cfg::kStage), bh = st + Cfg::kX, bl = bh + Cfg::kB;
+#pragma unroll
+      for (int kk = 0; kk < 4; ++kk) {   // one k8 step = one wgmma group; the previous group runs while this one is loaded
+        uint32_t ah[MB][4], al[MB][4];
+#pragma unroll
+        for (int j = 0; j < MB; ++j) {
+          Unit::ld_frag(ah[j], st, cw * MB + j, kk, warp, lane);
+          if (SPLIT)
+#pragma unroll
+            for (int i = 0; i < 4; ++i) {
+              const float x = __uint_as_float(ah[j][i]), hi = tf32_hi(x);
+              ah[j][i] = __float_as_uint(hi);
+              al[j][i] = __float_as_uint(x - hi);
+            }
         }
+        wgmma_fence();
+        const uint64_t dh = gmma_desc_sw128(bh + kk * 32u);
+#pragma unroll
+        for (int j = 0; j < MB; ++j) {
+          if (SPLIT) {
+            WgmmaRS<D>::mma(acc[j], al[j], dh);                               // lo * hi
+            WgmmaRS<D>::mma(acc[j], ah[j], gmma_desc_sw128(bl + kk * 32u));   // hi * lo
+          }
+          WgmmaRS<D>::mma(acc[j], ah[j], dh);                                 // hi * hi
+        }
+        wgmma_commit();
+        wgmma_wait<1>();
+        if (kk == 0 && prev >= 0 && lane == 0) mbar_arrive(&empty[prev]);   // the previous stage's last group is done
       }
+      prev = s;
+      if (++s == Cfg::kStages) { s = 0; ph ^= 1u; }
     }
-    fence_proxy_async_smem();
-    __syncthreads();   // raw stage s consumed, operands visible to wgmma
-    if (tid == 0 && kb + stages < kb_n) issue(kb + stages);
-    const uint32_t a0 = smem_u32(opA) + wg * 8192u, al0 = smem_u32(opAlo) + wg * 8192u;
-    const uint32_t b0 = smem_u32(opB), bl0 = smem_u32(opBlo);
-    wgmma_fence();
-#pragma unroll
-    for (int kk = 0; kk < 4; ++kk) {
-#pragma unroll
-      for (int c = 0; c < NC; ++c) {
-        const uint64_t bd = gmma_desc_sw128(b0 + c * 4096u + kk * 32u);
-        if (SPLIT) {
-          wgmma_m64n32k8_tf32(acc[c], gmma_desc_sw128(al0 + kk * 32u), bd, 1);
-          wgmma_m64n32k8_tf32(acc[c], gmma_desc_sw128(a0 + kk * 32u), gmma_desc_sw128(bl0 + c * 4096u + kk * 32u), 1);
-          wgmma_m64n32k8_tf32(acc[c], gmma_desc_sw128(a0 + kk * 32u), bd, 1);
-        } else {
-          wgmma_m64n32k8_tf32(acc[c], gmma_desc_sw128(a0 + kk * 32u), bd, 1);
-        }
-      }
-    }
-    wgmma_commit();
     wgmma_wait<0>();
-    __syncthreads();   // operand buffers free for the next transform
-  }
-
-  // epilogue: partial[item][feature][d]
-  const int f0 = wg * 64 + warp * 16 + (lane >> 2);
-  float* out = P.partial + (long long)item * BM * D;
-#pragma unroll
-  for (int c = 0; c < NC; ++c) {
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      const int col = c * 32 + j * 8 + (lane & 3) * 2;
-#pragma unroll
-      for (int h = 0; h < 2; ++h)
-        *reinterpret_cast<float2*>(out + (long long)(f0 + 8 * h) * D + col) = make_float2(acc[c][4 * j + 2 * h], acc[c][4 * j + 2 * h + 1]);
-    }
+    if (prev >= 0 && lane == 0) mbar_arrive(&empty[prev]);
+    w.store(acc, cw, warp, lane);
   }
 }
 
-// Ring depth: enough TMA stages in flight to cover HBM latency, and at most ~110 KiB of shared memory where that allows
-// two CTAs per SM (one CTA transforms / multiplies while the other's loads land).
-static int ring_stages(uint32_t stage_bytes, uint32_t fixed_bytes) {
-  int s = (int)((110u * 1024u - fixed_bytes) / stage_bytes);
-  if (s < 2) s = 2;
-  if (s > 4) s = 4;
-  return s;
+template <int D, bool SPLIT, int MB>
+__global__ void __launch_bounds__(384, 1) proj_fwd_tc_kernel(const __grid_constant__ FwdParams P) {
+  proj_pipeline<D, SPLIT, MB, FwdUnit<D, SPLIT, MB>>(P, P.total_tiles);
 }
 
-template <int D, bool SPLIT>
-static int launch_fwd(FwdParams P, cudaStream_t st) {
-  constexpr uint32_t stage = (kTileA + D * 128u) * (SPLIT ? 2u : 1u);
-  P.stages = ring_stages(stage, 0);
-  const uint32_t smem = (uint32_t)P.stages * stage + 1024 /*align slack*/ + 64 /*barriers*/;
-  LLMREC_CHECK_CUDA(cudaFuncSetAttribute(proj_fwd_tc_kernel<D, SPLIT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  proj_fwd_tc_kernel<D, SPLIT><<<P.total_tiles, 256, smem, st>>>(P);
+template <int D, bool SPLIT, int MB>
+__global__ void __launch_bounds__(384, 1) proj_wgrad_tc_kernel(const __grid_constant__ WgParams P) {
+  proj_pipeline<D, SPLIT, MB, WgUnit<D, SPLIT, MB>>(P, P.total_items);
+}
+
+static int num_sms() {
+  static int n[64] = {};
+  int dev = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 132;
+  if (!n[dev] && cudaDeviceGetAttribute(&n[dev], cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) n[dev] = 132;
+  return n[dev];
+}
+
+// MB = 2 (256-wide tiles: half the W / dY^T re-reads from L2) where the accumulators fit (d <= 128) and the tiles still fill every SM
+static int pick_mb(int d, long long units_at_256) { return d <= 128 && units_at_256 >= num_sms() ? 2 : 1; }
+
+template <int D, bool SPLIT, int MB>
+static int launch_fwd(const FwdParams& P, cudaStream_t st) {
+  using Cfg = ProjCfg<D, SPLIT, MB>;
+  LLMREC_CHECK_CUDA(cudaFuncSetAttribute(proj_fwd_tc_kernel<D, SPLIT, MB>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Cfg::kSmem));
+  const int grid = P.total_tiles < num_sms() ? P.total_tiles : num_sms();
+  proj_fwd_tc_kernel<D, SPLIT, MB><<<grid, 384, Cfg::kSmem, st>>>(P);
   LLMREC_CHECK_LAUNCH("proj_fwd_tc");
   return 0;
 }
 
-template <int D, bool SPLIT>
-static int launch_wgrad(WgParams P, cudaStream_t st) {
-  constexpr uint32_t raw = kTileA + D * 128u;
-  constexpr uint32_t ops = (kTileA + D * 128u) * (SPLIT ? 2u : 1u);
-  P.stages = ring_stages(raw, ops);
-  const uint32_t smem = (uint32_t)P.stages * raw + ops + 1024 + 64;
-  LLMREC_CHECK_CUDA(cudaFuncSetAttribute(proj_wgrad_tc_kernel<D, SPLIT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  proj_wgrad_tc_kernel<D, SPLIT><<<P.total_items, 256, smem, st>>>(P);
+template <int D, bool SPLIT, int MB>
+static int launch_wgrad(const WgParams& P, cudaStream_t st) {
+  using Cfg = ProjCfg<D, SPLIT, MB>;
+  LLMREC_CHECK_CUDA(cudaFuncSetAttribute(proj_wgrad_tc_kernel<D, SPLIT, MB>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Cfg::kSmem));
+  const int grid = P.total_items < num_sms() ? P.total_items : num_sms();
+  proj_wgrad_tc_kernel<D, SPLIT, MB><<<grid, 384, Cfg::kSmem, st>>>(P);
   LLMREC_CHECK_LAUNCH("proj_wgrad_tc");
   return 0;
 }
 
+// MB = 2 exists for d <= 128 only (its accumulators at d > 128 would not fit next to the fragments)
+template <int D, bool SPLIT>
+static int launch_fwd_mb(const FwdParams& P, int mb, cudaStream_t st) {
+  if constexpr (D <= 128) { if (mb == 2) return launch_fwd<D, SPLIT, 2>(P, st); }
+  return launch_fwd<D, SPLIT, 1>(P, st);
+}
+template <int D, bool SPLIT>
+static int launch_wgrad_mb(const WgParams& P, int mb, cudaStream_t st) {
+  if constexpr (D <= 128) { if (mb == 2) return launch_wgrad<D, SPLIT, 2>(P, st); }
+  return launch_wgrad<D, SPLIT, 1>(P, st);
+}
+
 #define LLMREC_PROJ_WIDTHS(X) X(32) X(64) X(96) X(128) X(160) X(192) X(224) X(256)
 
-static int fwd_launch(const FwdParams& P, bool split, cudaStream_t st) {
+static int fwd_launch(const FwdParams& P, bool split, int mb, cudaStream_t st) {
   switch (P.d) {
-#define LLMREC_CASE(W) case W: return split ? launch_fwd<W, true>(P, st) : launch_fwd<W, false>(P, st);
+#define LLMREC_CASE(W) case W: return split ? launch_fwd_mb<W, true>(P, mb, st) : launch_fwd_mb<W, false>(P, mb, st);
     LLMREC_PROJ_WIDTHS(LLMREC_CASE)
 #undef LLMREC_CASE
   }
@@ -348,14 +354,38 @@ static int fwd_launch(const FwdParams& P, bool split, cudaStream_t st) {
   return 1;
 }
 
-static int wgrad_launch(const WgParams& P, bool split, cudaStream_t st) {
+static int wgrad_launch(const WgParams& P, bool split, int mb, cudaStream_t st) {
   switch (P.d) {
-#define LLMREC_CASE(W) case W: return split ? launch_wgrad<W, true>(P, st) : launch_wgrad<W, false>(P, st);
+#define LLMREC_CASE(W) case W: return split ? launch_wgrad_mb<W, true>(P, mb, st) : launch_wgrad_mb<W, false>(P, mb, st);
     LLMREC_PROJ_WIDTHS(LLMREC_CASE)
 #undef LLMREC_CASE
   }
   set_error("proj_wgrad: no tensor-core kernel for d=%d", P.d);
   return 1;
+}
+
+// dY -> dY^T [hi ; lo] ([2d x ldt], hi exactly TF32-representable; [d x ldt] unsplit in mode 1) for every problem of a grouped
+// weight gradient in ONE launch (blockIdx.z): the B operand of the wgrad kernel, K-major (rows of dY contiguous), from strided views.
+struct DytParams { const float* dY[kMaxProb]; long long ld[kMaxProb]; int n[kMaxProb]; float* out[kMaxProb]; long long ldt[kMaxProb]; int d, split; };
+__global__ void __launch_bounds__(256) dyt_split_kernel(const DytParams P) {
+  __shared__ float tile[32][33];
+  const int p = blockIdx.z, n = P.n[p], r0 = blockIdx.x * 32, e0 = blockIdx.y * 32;
+  if (r0 >= n) return;
+  const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
+  const float* __restrict__ src = P.dY[p];
+#pragma unroll
+  for (int i = ty; i < 32; i += 8) tile[i][tx] = r0 + i < n ? __ldg(src + (long long)(r0 + i) * P.ld[p] + e0 + tx) : 0.f;
+  __syncthreads();
+  if (r0 + tx >= n) return;
+  float* __restrict__ dst = P.out[p];
+  const long long ldt = P.ldt[p], lo = (long long)P.d * ldt;
+#pragma unroll
+  for (int i = ty; i < 32; i += 8) {
+    const float v = tile[tx][i];
+    float* o = dst + (long long)(e0 + i) * ldt + r0 + tx;
+    if (P.split) { const float h = tf32_hi(v); o[0] = h; o[lo] = v - h; }
+    else o[0] = v;
+  }
 }
 
 // W -> [hi ; lo]  ([2d x k], hi exactly TF32-representable); every distinct weight matrix of a grouped launch in ONE launch (blockIdx.y)
@@ -369,12 +399,12 @@ __global__ void wsplit_kernel(const WsplitParams P) {
   }
 }
 
-// dW[dc][f] = sum over (problems sharing this dW, in list order) x (row chunks, in order) of partial[item][f % 128][dc]
+// dW[dc][f] = sum over (problems sharing this dW, in list order) x (row chunks, in order) of partial[item][f % tm][dc]
 // One launch for every output.  Block = (output feature tile, group of 4 features): 64 float4 elements x 4 source
 // slices; each thread sums every 4th (problem, chunk) source with independent loads in flight, the 4 slices are
 // combined in a fixed order -> deterministic and latency-tolerant (the naive per-element loop was latency-bound).
 struct ReduceOut { float* dW; int k, n_src, accumulate, blk_start; int src[kMaxProb]; };
-struct ReduceParams { ReduceOut out[kMaxProb]; int n_out; int d; const float* partial; WgProblem prob[kMaxProb]; };
+struct ReduceParams { ReduceOut out[kMaxProb]; int n_out; int d, tm; const float* partial; WgProblem prob[kMaxProb]; };
 __global__ void __launch_bounds__(256) wgrad_reduce_kernel(const ReduceParams R) {
   __shared__ float4 part[4][64];
   int o = 0;
@@ -383,10 +413,10 @@ __global__ void __launch_bounds__(256) wgrad_reduce_kernel(const ReduceParams R)
   const int d = R.d, f4_per_feat = d >> 2;                 // d % 32 == 0 on this path
   const int feats_per_blk = 64 / f4_per_feat;              // 4 at d = 64, 2 at d = 128, 1 at d = 256
   const int local = blockIdx.x - ro.blk_start;
-  const int groups_per_ft = BM / feats_per_blk;
+  const int tm = R.tm, groups_per_ft = tm / feats_per_blk;
   const int ft = local / groups_per_ft, fg = local - ft * groups_per_ft;
   const int e = threadIdx.x & 63, sl = threadIdx.x >> 6;
-  const int f = fg * feats_per_blk + e / f4_per_feat;      // feature inside the 128-feature tile
+  const int f = fg * feats_per_blk + e / f4_per_feat;      // feature inside the tm-feature tile
   const int dc4 = e - (e / f4_per_feat) * f4_per_feat;     // float4 column
   float4 s = make_float4(0.f, 0.f, 0.f, 0.f);
   int idx = 0;
@@ -395,7 +425,7 @@ __global__ void __launch_bounds__(256) wgrad_reduce_kernel(const ReduceParams R)
 #pragma unroll 4
     for (int c = 0; c < pr.chunks; ++c, ++idx) {
       if ((idx & 3) != sl) continue;
-      const float4 v = __ldg(reinterpret_cast<const float4*>(R.partial + ((long long)(pr.item_start + c * pr.ft_tiles + ft) * BM + f) * d) + dc4);
+      const float4 v = __ldg(reinterpret_cast<const float4*>(R.partial + ((long long)(pr.item_start + c * pr.ft_tiles + ft) * tm + f) * d) + dc4);
       s.x += v.x; s.y += v.y; s.z += v.z; s.w += v.w;
     }
   }
@@ -404,7 +434,7 @@ __global__ void __launch_bounds__(256) wgrad_reduce_kernel(const ReduceParams R)
   if (sl == 0) {
     float4 a = part[0][e], b = part[1][e], c = part[2][e], g = part[3][e];
     float4 t = make_float4((a.x + b.x) + (c.x + g.x), (a.y + b.y) + (c.y + g.y), (a.z + b.z) + (c.z + g.z), (a.w + b.w) + (c.w + g.w));
-    const int gf = ft * BM + f;
+    const int gf = ft * tm + f;
     if (gf < ro.k) {
       float* p = ro.dW + (long long)(dc4 * 4) * ro.k + gf;
       if (ro.accumulate) { t.x += p[0]; t.y += p[ro.k]; t.z += p[2LL * ro.k]; t.w += p[3LL * ro.k]; }
@@ -463,7 +493,7 @@ __global__ void __launch_bounds__(256) colsum_kernel(const ColsumParams P) {
 // host API (grouped)
 // ------------------------------------------------------------------------------------------------
 bool proj_tc_supported(int d, int64_t ldx, const void* X, int k, bool wgrad) {
-  (void)wgrad;   // both directions take d in multiples of 32 (wgmma n32 column blocks)
+  (void)wgrad;   // both directions take d in multiples of 32 (wgmma N = d)
   return d % 32 == 0 && d >= 32 && d <= 256 && ldx % 4 == 0 && aligned16(X) && k >= 1 && k % 4 == 0;
 }
 
@@ -472,11 +502,13 @@ int proj_fwd_tc_group(const llmrec_proj_fwd_problem* pr, int n_prob, int d, int 
   FwdParams P;
   memset(&P, 0, sizeof(P));
   P.n_prob = n_prob; P.d = d;
-  int tiles = 0;
   WsplitParams WS;
   memset(&WS, 0, sizeof(WS));
   int n_ws = 0;
-  long long ws_max = 0;
+  long long ws_max = 0, tiles256 = 0;
+  for (int p = 0; p < n_prob; ++p) tiles256 += (pr[p].n + tile_m(2) - 1) / tile_m(2);
+  const int mb = pick_mb(d, tiles256), tm = tile_m(mb);
+  int tiles = 0;
   for (int p = 0; p < n_prob; ++p) {
     const float* wsrc = split ? pr[p].wsplit : pr[p].W;
     LLMREC_CHECK_ARG(!split || pr[p].wsplit, "proj_fwd: 3xTF32 mode needs a wsplit buffer of 2*d*k floats");
@@ -487,11 +519,11 @@ int proj_fwd_tc_group(const llmrec_proj_fwd_problem* pr, int n_prob, int d, int 
       ws_max = WS.n[n_ws] > ws_max ? WS.n[n_ws] : ws_max;
       ++n_ws;
     }
-    if (!make_tmap_2d_f32(&P.tmA[p], pr[p].X, (uint64_t)pr[p].k, (uint64_t)pr[p].n, (uint64_t)pr[p].ldx * 4, BK, BM)) return 4;
+    if (!make_tmap_2d_f32(&P.tmA[p], pr[p].X, (uint64_t)pr[p].k, (uint64_t)pr[p].n, (uint64_t)pr[p].ldx * 4, BK, (uint32_t)tm)) return 4;
     if (!make_tmap_2d_f32(&P.tmW[p], wsrc, (uint64_t)pr[p].k, (uint64_t)(split ? 2 * d : d), (uint64_t)pr[p].k * 4, BK, (uint32_t)d)) return 4;
     P.prob[p].n = (int)pr[p].n; P.prob[p].k = pr[p].k; P.prob[p].kblocks = (pr[p].k + BK - 1) / BK;
     P.prob[p].tile_start = tiles; P.prob[p].ldy = pr[p].ldy; P.prob[p].Y = pr[p].Y; P.prob[p].bias = pr[p].bias;
-    tiles += (int)((pr[p].n + BM - 1) / BM);
+    tiles += (int)((pr[p].n + tm - 1) / tm);
   }
   P.total_tiles = tiles;
   if (n_ws > 0) {
@@ -499,7 +531,7 @@ int proj_fwd_tc_group(const llmrec_proj_fwd_problem* pr, int n_prob, int d, int 
     LLMREC_CHECK_LAUNCH("wsplit");
   }
   if (tiles <= 0) return 0;
-  return fwd_launch(P, split, st);
+  return fwd_launch(P, split, mb, st);
 }
 
 static int wg_rows_per_chunk(int64_t n) {
@@ -508,42 +540,68 @@ static int wg_rows_per_chunk(int64_t n) {
   return r;
 }
 
-int64_t proj_wgrad_tc_scratch(const llmrec_proj_wgrad_problem* pr, int n_prob, int d) {
-  int64_t items = 0;
+// Work plan of a grouped weight gradient, shared by the scratch query and the launch.  Scratch layout (floats):
+//   [colsum ticket: 4] [partials: items x tm x d] [colsum partials: n_prob x kColsumSlices x d] [per problem dY^T hi, lo: 2 x d x ldt]
+struct WgPlan { WgProblem prob[kMaxProb]; int items, mb, tm; int64_t ldt[kMaxProb], dyt[kMaxProb], colsum, total; };
+static void wg_plan(const llmrec_proj_wgrad_problem* pr, int n_prob, int d, WgPlan& W) {
+  long long items256 = 0;
   for (int p = 0; p < n_prob; ++p) {
-    int rpc = wg_rows_per_chunk(pr[p].n);
-    items += (int64_t)((pr[p].k + BM - 1) / BM) * ((pr[p].n + rpc - 1) / rpc);
+    const int rpc = wg_rows_per_chunk(pr[p].n);
+    items256 += (long long)((pr[p].k + tile_m(2) - 1) / tile_m(2)) * ((pr[p].n + rpc - 1) / rpc);
   }
-  return items * BM * d + (int64_t)n_prob * kColsumSlices * d + 4;   // + the colsum ticket (must start at zero; the kernel re-zeroes it)
+  W.mb = pick_mb(d, items256); W.tm = tile_m(W.mb);
+  W.items = 0;
+  for (int p = 0; p < n_prob; ++p) {
+    WgProblem& w = W.prob[p];
+    w.n = (int)pr[p].n; w.k = pr[p].k; w.ft_tiles = (pr[p].k + W.tm - 1) / W.tm;
+    w.rows_per_chunk = wg_rows_per_chunk(pr[p].n);
+    w.chunks = (int)((pr[p].n + w.rows_per_chunk - 1) / w.rows_per_chunk);
+    w.item_start = W.items;
+    W.items += w.ft_tiles * w.chunks;
+  }
+  W.colsum = 4 + (int64_t)W.items * W.tm * d;
+  int64_t off = W.colsum + (int64_t)n_prob * kColsumSlices * d;
+  for (int p = 0; p < n_prob; ++p) {
+    W.ldt[p] = (pr[p].n + 3) & ~int64_t(3);   // TMA row pitch: a multiple of 16 bytes
+    W.dyt[p] = off;
+    off += 2 * (int64_t)d * W.ldt[p];
+  }
+  W.total = off;
+}
+
+int64_t proj_wgrad_tc_scratch(const llmrec_proj_wgrad_problem* pr, int n_prob, int d) {
+  WgPlan W;
+  wg_plan(pr, n_prob, d, W);
+  return W.total;   // the colsum ticket must start at zero; the kernel re-zeroes it
 }
 
 int proj_wgrad_tc_group(const llmrec_proj_wgrad_problem* pr, int n_prob, int d, int mode, float* scratch, int64_t scratch_elems, cudaStream_t st) {
   const bool split = (mode == 0);
+  WgPlan W;
+  wg_plan(pr, n_prob, d, W);
+  LLMREC_CHECK_ARG(scratch && scratch_elems >= W.total, "proj_wgrad: scratch too small (%lld < %lld)", (long long)scratch_elems, (long long)W.total);
   WgParams P;
   memset(&P, 0, sizeof(P));
-  P.n_prob = n_prob; P.d = d;
-  int items = 0;
+  P.n_prob = n_prob; P.d = d; P.total_items = W.items;
+  P.partial = scratch + 4;                                   // word 0 of the scratch is the colsum ticket (fixed position for every problem set)
   ColsumParams C;
   memset(&C, 0, sizeof(C));
-  C.d = d;
+  C.d = d; C.n_prob = n_prob; C.partial = scratch + W.colsum;
+  C.ticket = reinterpret_cast<unsigned*>(scratch);
+  DytParams T;
+  memset(&T, 0, sizeof(T));
+  T.d = d; T.split = split ? 1 : 0;
+  int64_t n_max = 0;
   for (int p = 0; p < n_prob; ++p) {
-    if (!make_tmap_2d_f32(&P.tmX[p], pr[p].X, (uint64_t)pr[p].k, (uint64_t)pr[p].n, (uint64_t)pr[p].ldx * 4, BM, BK, false)) return 4;
-    if (!make_tmap_2d_f32(&P.tmG[p], pr[p].dY, (uint64_t)d, (uint64_t)pr[p].n, (uint64_t)pr[p].lddy * 4, (uint32_t)d, BK, false)) return 4;
-    WgProblem& w = P.prob[p];
-    w.n = (int)pr[p].n; w.k = pr[p].k; w.ft_tiles = (pr[p].k + BM - 1) / BM;
-    w.rows_per_chunk = wg_rows_per_chunk(pr[p].n);
-    w.chunks = (int)((pr[p].n + w.rows_per_chunk - 1) / w.rows_per_chunk);
-    w.item_start = items;
-    items += w.ft_tiles * w.chunks;
+    P.prob[p] = W.prob[p];
+    float* dyt = scratch + W.dyt[p];
+    if (!make_tmap_2d_f32(&P.tmX[p], pr[p].X, (uint64_t)pr[p].k, (uint64_t)pr[p].n, (uint64_t)pr[p].ldx * 4, BK, BK)) return 4;
+    if (!make_tmap_2d_f32(&P.tmG[p], dyt, (uint64_t)pr[p].n, (uint64_t)(split ? 2 * d : d), (uint64_t)W.ldt[p] * 4, BK, (uint32_t)d)) return 4;
+    T.dY[p] = pr[p].dY; T.ld[p] = pr[p].lddy; T.n[p] = (int)pr[p].n; T.out[p] = dyt; T.ldt[p] = W.ldt[p];
+    n_max = pr[p].n > n_max ? pr[p].n : n_max;
     C.dY[p] = pr[p].dY; C.ld[p] = pr[p].lddy; C.n[p] = pr[p].n; C.db[p] = pr[p].db; C.acc[p] = pr[p].accumulate & LLMREC_WGRAD_ACCUMULATE;
   }
-  P.total_items = items;
-  const int64_t need = (int64_t)items * BM * d + (int64_t)n_prob * kColsumSlices * d + 4;
-  LLMREC_CHECK_ARG(scratch && scratch_elems >= need, "proj_wgrad: scratch too small (%lld < %lld)", (long long)scratch_elems, (long long)need);
-  P.partial = scratch + 4;                                   // word 0 of the scratch is the colsum ticket (fixed position for every problem set)
-  C.n_prob = n_prob; C.partial = scratch + 4 + (int64_t)items * BM * d;
-  C.ticket = reinterpret_cast<unsigned*>(scratch);
-  if (items <= 0) return 0;
+  if (W.items <= 0) return 0;
   // The bias gradients depend on dY only: colsum runs as a BRANCH beside the weight-gradient kernel -- fork/join through events, so inside a stream capture it becomes a parallel graph branch.
   // The side stream and the two events are per device, created on first use (never during the call that is being captured in practice:
   // callers run one eager step first); LLMREC_BRANCHES=0 keeps everything on `st`.
@@ -575,13 +633,15 @@ int proj_wgrad_tc_group(const llmrec_proj_wgrad_problem* pr, int n_prob, int d, 
     LLMREC_CHECK_LAUNCH("colsum");
     if (forked) LLMREC_CHECK_CUDA(cudaEventRecord(ev_join, side));
   }
+  dyt_split_kernel<<<dim3((unsigned)((n_max + 31) / 32), (unsigned)(d / 32), (unsigned)n_prob), 256, 0, st>>>(T);
+  LLMREC_CHECK_LAUNCH("dyt_split");
   {
-    int rc = wgrad_launch(P, split, st);
+    int rc = wgrad_launch(P, split, W.mb, st);
     if (rc) return rc;
   }
   ReduceParams R;
   memset(&R, 0, sizeof(R));
-  R.d = d; R.partial = scratch + 4;
+  R.d = d; R.tm = W.tm; R.partial = scratch + 4;
   int blocks = 0;
   for (int p = 0; p < n_prob; ++p) {
     R.prob[p] = P.prob[p];
@@ -595,7 +655,7 @@ int proj_wgrad_tc_group(const llmrec_proj_wgrad_problem* pr, int n_prob, int d, 
     R.out[o].src[R.out[o].n_src++] = p;
   }
   const int feats_per_blk = 64 / (d / 4);
-  for (int o = 0; o < R.n_out; ++o) { R.out[o].blk_start = blocks; blocks += ((R.out[o].k + BM - 1) / BM) * (BM / feats_per_blk); }
+  for (int o = 0; o < R.n_out; ++o) { R.out[o].blk_start = blocks; blocks += ((R.out[o].k + W.tm - 1) / W.tm) * (W.tm / feats_per_blk); }
   wgrad_reduce_kernel<<<blocks, 256, 0, st>>>(R);
   LLMREC_CHECK_LAUNCH("wgrad_reduce");
   if (forked) LLMREC_CHECK_CUDA(cudaStreamWaitEvent(st, ev_join, 0));

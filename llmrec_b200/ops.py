@@ -255,7 +255,7 @@ def proj_wgrad_group(problems, d, mode=0):
     need = int(N.lib().llmrec_proj_wgrad_group_scratch(arr, len(problems), d, mode))
     scratch = _get_scratch(("wgrad", problems[0][0].device.index), need, problems[0][0].device, zero=True) if need else None     # holds a ticket word
     N.check(N.lib().llmrec_proj_wgrad_group_f32(arr, len(problems), d, mode, _p(scratch), need, _stream()), "proj_wgrad_group")
-    _count(3 if need else len(problems))
+    _count(4 if need else len(problems))
 
 
 def proj_wgrad(X, dY, dW, db, accumulate=False, mode=0):
