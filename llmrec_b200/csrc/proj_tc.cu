@@ -400,9 +400,12 @@ __global__ void wsplit_kernel(const WsplitParams P) {
 }
 
 // dW[dc][f] = sum over (problems sharing this dW, in list order) x (row chunks, in order) of partial[item][f % tm][dc]
-// One launch for every output.  Block = (output feature tile, group of 4 features): 64 float4 elements x 4 source
-// slices; each thread sums every 4th (problem, chunk) source with independent loads in flight, the 4 slices are
-// combined in a fixed order -> deterministic and latency-tolerant (the naive per-element loop was latency-bound).
+// One launch for every output.  Block = (output feature tile, group of feats_per_blk = 64 / (d/4) features): 64 float4
+// lanes x 4 source slices; each thread sums every 4th (problem, chunk) source with independent loads in flight, the 4
+// slices are combined in a fixed order -> deterministic and latency-tolerant (the naive per-element loop was latency-bound).
+// When d/4 does not divide 64 (d = 96, 160, 192, 224) the last 64 - feats_per_blk * d/4 lanes would land on the next
+// group's first feature, which that group's block owns: they load and store nothing (a second read-modify-write of the
+// same element races under accumulate).
 struct ReduceOut { float* dW; int k, n_src, accumulate, blk_start; int src[kMaxProb]; };
 struct ReduceParams { ReduceOut out[kMaxProb]; int n_out; int d, tm; const float* partial; WgProblem prob[kMaxProb]; };
 __global__ void __launch_bounds__(256) wgrad_reduce_kernel(const ReduceParams R) {
@@ -411,16 +414,17 @@ __global__ void __launch_bounds__(256) wgrad_reduce_kernel(const ReduceParams R)
   while (o + 1 < R.n_out && (int)blockIdx.x >= R.out[o + 1].blk_start) ++o;
   const ReduceOut ro = R.out[o];
   const int d = R.d, f4_per_feat = d >> 2;                 // d % 32 == 0 on this path
-  const int feats_per_blk = 64 / f4_per_feat;              // 4 at d = 64, 2 at d = 128, 1 at d = 256
+  const int feats_per_blk = 64 / f4_per_feat;              // 8 at d = 32, 4 at d = 64, 2 at d = 96 / 128, 1 above
   const int local = blockIdx.x - ro.blk_start;
   const int tm = R.tm, groups_per_ft = tm / feats_per_blk;
   const int ft = local / groups_per_ft, fg = local - ft * groups_per_ft;
   const int e = threadIdx.x & 63, sl = threadIdx.x >> 6;
+  const bool owned = e < feats_per_blk * f4_per_feat;      // every lane at d = 32, 64, 128, 256
   const int f = fg * feats_per_blk + e / f4_per_feat;      // feature inside the tm-feature tile
   const int dc4 = e - (e / f4_per_feat) * f4_per_feat;     // float4 column
   float4 s = make_float4(0.f, 0.f, 0.f, 0.f);
   int idx = 0;
-  for (int j = 0; j < ro.n_src; ++j) {
+  for (int j = 0; owned && j < ro.n_src; ++j) {
     const WgProblem pr = R.prob[ro.src[j]];
 #pragma unroll 4
     for (int c = 0; c < pr.chunks; ++c, ++idx) {
@@ -431,7 +435,7 @@ __global__ void __launch_bounds__(256) wgrad_reduce_kernel(const ReduceParams R)
   }
   part[sl][e] = s;
   __syncthreads();
-  if (sl == 0) {
+  if (sl == 0 && owned) {
     float4 a = part[0][e], b = part[1][e], c = part[2][e], g = part[3][e];
     float4 t = make_float4((a.x + b.x) + (c.x + g.x), (a.y + b.y) + (c.y + g.y), (a.z + b.z) + (c.z + g.z), (a.w + b.w) + (c.w + g.w));
     const int gf = ft * tm + f;
@@ -519,8 +523,11 @@ int proj_fwd_tc_group(const llmrec_proj_fwd_problem* pr, int n_prob, int d, int 
       ws_max = WS.n[n_ws] > ws_max ? WS.n[n_ws] : ws_max;
       ++n_ws;
     }
-    if (!make_tmap_2d_f32(&P.tmA[p], pr[p].X, (uint64_t)pr[p].k, (uint64_t)pr[p].n, (uint64_t)pr[p].ldx * 4, BK, (uint32_t)tm)) return 4;
-    if (!make_tmap_2d_f32(&P.tmW[p], wsrc, (uint64_t)pr[p].k, (uint64_t)(split ? 2 * d : d), (uint64_t)pr[p].k * 4, BK, (uint32_t)d)) return 4;
+    // an empty problem has no tiles (and a tensor map cannot have an empty dimension); its W is still split when a later problem shares it
+    if (pr[p].n > 0) {
+      if (!make_tmap_2d_f32(&P.tmA[p], pr[p].X, (uint64_t)pr[p].k, (uint64_t)pr[p].n, (uint64_t)pr[p].ldx * 4, BK, (uint32_t)tm)) return 4;
+      if (!make_tmap_2d_f32(&P.tmW[p], wsrc, (uint64_t)pr[p].k, (uint64_t)(split ? 2 * d : d), (uint64_t)pr[p].k * 4, BK, (uint32_t)d)) return 4;
+    }
     P.prob[p].n = (int)pr[p].n; P.prob[p].k = pr[p].k; P.prob[p].kblocks = (pr[p].k + BK - 1) / BK;
     P.prob[p].tile_start = tiles; P.prob[p].ldy = pr[p].ldy; P.prob[p].Y = pr[p].Y; P.prob[p].bias = pr[p].bias;
     tiles += (int)((pr[p].n + tm - 1) / tm);
@@ -595,13 +602,16 @@ int proj_wgrad_tc_group(const llmrec_proj_wgrad_problem* pr, int n_prob, int d, 
   for (int p = 0; p < n_prob; ++p) {
     P.prob[p] = W.prob[p];
     float* dyt = scratch + W.dyt[p];
-    if (!make_tmap_2d_f32(&P.tmX[p], pr[p].X, (uint64_t)pr[p].k, (uint64_t)pr[p].n, (uint64_t)pr[p].ldx * 4, BK, BK)) return 4;
-    if (!make_tmap_2d_f32(&P.tmG[p], dyt, (uint64_t)pr[p].n, (uint64_t)(split ? 2 * d : d), (uint64_t)W.ldt[p] * 4, BK, (uint32_t)d)) return 4;
+    // an empty problem has no work items (and a tensor map cannot have an empty dimension); colsum and the reduce still
+    // write its dW / db: zeros, or the prior under accumulate
+    if (pr[p].n > 0) {
+      if (!make_tmap_2d_f32(&P.tmX[p], pr[p].X, (uint64_t)pr[p].k, (uint64_t)pr[p].n, (uint64_t)pr[p].ldx * 4, BK, BK)) return 4;
+      if (!make_tmap_2d_f32(&P.tmG[p], dyt, (uint64_t)pr[p].n, (uint64_t)(split ? 2 * d : d), (uint64_t)W.ldt[p] * 4, BK, (uint32_t)d)) return 4;
+    }
     T.dY[p] = pr[p].dY; T.ld[p] = pr[p].lddy; T.n[p] = (int)pr[p].n; T.out[p] = dyt; T.ldt[p] = W.ldt[p];
     n_max = pr[p].n > n_max ? pr[p].n : n_max;
     C.dY[p] = pr[p].dY; C.ld[p] = pr[p].lddy; C.n[p] = pr[p].n; C.db[p] = pr[p].db; C.acc[p] = pr[p].accumulate & LLMREC_WGRAD_ACCUMULATE;
   }
-  if (W.items <= 0) return 0;
   // The bias gradients depend on dY only: colsum runs as a BRANCH beside the weight-gradient kernel -- fork/join through events, so inside a stream capture it becomes a parallel graph branch.
   // The side stream and the two events are per device, created on first use (never during the call that is being captured in practice:
   // callers run one eager step first); LLMREC_BRANCHES=0 keeps everything on `st`.
@@ -633,9 +643,9 @@ int proj_wgrad_tc_group(const llmrec_proj_wgrad_problem* pr, int n_prob, int d, 
     LLMREC_CHECK_LAUNCH("colsum");
     if (forked) LLMREC_CHECK_CUDA(cudaEventRecord(ev_join, side));
   }
-  dyt_split_kernel<<<dim3((unsigned)((n_max + 31) / 32), (unsigned)(d / 32), (unsigned)n_prob), 256, 0, st>>>(T);
-  LLMREC_CHECK_LAUNCH("dyt_split");
-  {
+  if (W.items > 0) {   // no items: every problem is empty, and only colsum and the reduce run
+    dyt_split_kernel<<<dim3((unsigned)((n_max + 31) / 32), (unsigned)(d / 32), (unsigned)n_prob), 256, 0, st>>>(T);
+    LLMREC_CHECK_LAUNCH("dyt_split");
     int rc = wgrad_launch(P, split, W.mb, st);
     if (rc) return rc;
   }
