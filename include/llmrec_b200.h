@@ -6,7 +6,8 @@
  * points are what a ctypes/cffi binding of that API binds: plain device pointers, sizes and a
  * cudaStream_t.  No torch types.  Conventions:
  *   - every pointer is a DEVICE pointer unless the name ends in _host;
- *   - all matrices are row-major fp32 with an explicit leading dimension (elements);
+ *   - all matrices are row-major fp32 with an explicit leading dimension (elements), except the side-feature table X of the
+ *     _bf16 projection entry points: raw bfloat16 bits (uint16_t), row-major, leading dimension in elements;
  *   - index arrays are int32 (CSR rowptr/col; nnz < 2^31) unless stated;
  *   - nothing is allocated, nothing synchronises the host; work is enqueued on `stream`;
  *   - return 0 on success, non-zero on error; llmrec_last_error() gives the message
@@ -151,6 +152,34 @@ int llmrec_proj_wgrad_group_f32(const llmrec_proj_wgrad_problem* probs_host, int
  * weight-gradient kernel; inside a stream capture this becomes a parallel graph branch.  One side stream + two events per device,
  * created on first use (the only objects the library ever creates); LLMREC_BRANCHES=0 keeps everything on `stream`. */
 int64_t llmrec_proj_wgrad_group_scratch(const llmrec_proj_wgrad_problem* probs_host, int32_t n_prob, int32_t d, int32_t mode);
+
+/* bf16 feature tables (--feat_dtype bf16): the same grouped projections with X as raw bfloat16 bits (row-major, leading dimension
+ * ldx in ELEMENTS); W, bias, Y, dY, dW, db stay fp32.  The result is what the fp32 entry points compute on the upcast table:
+ *   mode 0: W (forward) / dY (weight gradient) split EXACTLY into three bf16 terms t0 + t1 + t2 (t0 = trunc_bf16(v), t1 =
+ *           trunc_bf16(v - t0), t2 = the rest, bf16-exact); a bf16 X needs no split, every bf16 x bf16 product is exact in fp32,
+ *           so only the accumulation rounds (fp32-class, no product term dropped);
+ *   mode 1: one bf16 wgmma, W / dY truncated to bf16;
+ *   mode 2: the exact SIMT kernels with X widened on load (forward bit-identical to mode 2 on the upcast table; the weight
+ *           gradient too, up to the order of its atomics across 1024-row chunks).
+ * The tensor-core path takes d = 32..256 in steps of 32, k % 8 == 0, ldx % 8 == 0 and a 16-byte aligned X; other shapes run
+ * the SIMT kernels.  `wsplit` (2*d*k floats, holding the 3*d*k bf16 terms) is needed in modes 0 AND 1.  Scratch, accumulate,
+ * grouping and the side-stream bias sums are as for the _f32 forms. */
+typedef struct {
+  const uint16_t* X; const float* W; const float* bias; float* Y; float* wsplit;
+  int64_t ldx, ldy, n;
+  int32_t k, _reserved;       /* 0 */
+} llmrec_proj_fwd_problem_bf16;
+typedef struct {
+  const uint16_t* X; const float* dY; float* dW; float* db;
+  int64_t ldx, lddy, n;
+  int32_t k, accumulate;      /* LLMREC_WGRAD_ACCUMULATE */
+} llmrec_proj_wgrad_problem_bf16;
+int llmrec_proj_fwd_group_bf16(const llmrec_proj_fwd_problem_bf16* probs_host, int32_t n_prob, int32_t d, int32_t mode,
+                               llmrec_stream_t stream);
+int llmrec_proj_wgrad_group_bf16(const llmrec_proj_wgrad_problem_bf16* probs_host, int32_t n_prob, int32_t d, int32_t mode,
+                                 float* scratch /* zero-initialised ONCE, as for llmrec_proj_wgrad_group_f32 */,
+                                 int64_t scratch_elems, llmrec_stream_t stream);
+int64_t llmrec_proj_wgrad_group_bf16_scratch(const llmrec_proj_wgrad_problem_bf16* probs_host, int32_t n_prob, int32_t d, int32_t mode);
 
 /* ---------------------------------------------------------------------------------------------
  * Fusion (Models.py:185-197):  out = mean(layer_0..layer_{L}) + sum_t coef[t] * x_t / max(||x_t||_2, 1e-12)

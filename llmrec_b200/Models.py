@@ -82,13 +82,16 @@ class MM_Model(nn.Module):
         self.item_id_embedding = nn.Embedding(n_items, embedding_dim)
         nn.init.xavier_uniform_(self.user_id_embedding.weight)
         nn.init.xavier_uniform_(self.item_id_embedding.weight)
-        as_f32 = lambda a: torch.as_tensor(a).float().contiguous()
-        self.register_buffer("image_feats", as_f32(image_feats), persistent=False)
-        self.register_buffer("text_feats", as_f32(text_feats), persistent=False)
-        self.register_buffer("user_feats", as_f32(user_init_embedding), persistent=False)
+        # --feat_dtype bf16: the constant feature tables are rounded once (torch's round-to-nearest-even cast; no RNG is drawn, so the
+        # seeded parameter init above is unchanged) and stay bf16; the projection kernels read them as they are
+        feat_dtype = torch.bfloat16 if getattr(args, "feat_dtype", "fp32") == "bf16" else torch.float32
+        as_feat = lambda a: torch.as_tensor(a).float().to(feat_dtype).contiguous()
+        self.register_buffer("image_feats", as_feat(image_feats), persistent=False)
+        self.register_buffer("text_feats", as_feat(text_feats), persistent=False)
+        self.register_buffer("user_feats", as_feat(user_init_embedding), persistent=False)
         self._item_keys = list(item_attribute_dict.keys())
         for k in self._item_keys:
-            self.register_buffer("item_feat__" + k, as_f32(item_attribute_dict[k]), persistent=False)
+            self.register_buffer("item_feat__" + k, as_feat(item_attribute_dict[k]), persistent=False)
         self.batch_norm = nn.BatchNorm1d(d)      # present (unused) in the reference; kept for state_dict parity
         self.tau = 0.5
         self._hp = None

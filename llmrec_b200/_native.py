@@ -39,6 +39,14 @@ class ProjWgradProblem(C.Structure):
                 ("ldx", C.c_int64), ("lddy", C.c_int64), ("n", C.c_int64), ("k", C.c_int32), ("accumulate", C.c_int32)]
 
 
+class ProjFwdProblemBf16(C.Structure):      # X: raw bfloat16 bits
+    _fields_ = ProjFwdProblem._fields_
+
+
+class ProjWgradProblemBf16(C.Structure):    # X: raw bfloat16 bits
+    _fields_ = ProjWgradProblem._fields_
+
+
 class BprHead(C.Structure):
     _fields_ = [("XU", C.c_void_p), ("XI", C.c_void_p), ("GU", C.c_void_p), ("GI", C.c_void_p),
                 ("ldxu", C.c_int64), ("ldxi", C.c_int64), ("ldgu", C.c_int64), ("ldgi", C.c_int64),
@@ -81,6 +89,9 @@ SIGNATURES = {
     "llmrec_proj_fwd_group_f32": (C.c_int, [C.POINTER(ProjFwdProblem), C.c_int32, C.c_int32, C.c_int32, c_stream]),
     "llmrec_proj_wgrad_group_f32": (C.c_int, [C.POINTER(ProjWgradProblem), C.c_int32, C.c_int32, C.c_int32, c_f32p, C.c_int64, c_stream]),
     "llmrec_proj_wgrad_group_scratch": (C.c_int64, [C.POINTER(ProjWgradProblem), C.c_int32, C.c_int32, C.c_int32]),
+    "llmrec_proj_fwd_group_bf16": (C.c_int, [C.POINTER(ProjFwdProblemBf16), C.c_int32, C.c_int32, C.c_int32, c_stream]),
+    "llmrec_proj_wgrad_group_bf16": (C.c_int, [C.POINTER(ProjWgradProblemBf16), C.c_int32, C.c_int32, C.c_int32, c_f32p, C.c_int64, c_stream]),
+    "llmrec_proj_wgrad_group_bf16_scratch": (C.c_int64, [C.POINTER(ProjWgradProblemBf16), C.c_int32, C.c_int32, C.c_int32]),
     "llmrec_proj_wgrad_f32": (C.c_int, [c_f32p, C.c_int64, c_f32p, C.c_int64, c_f32p, c_f32p, C.c_int64, C.c_int32, C.c_int32,
                                         C.c_int32, C.c_int32, c_f32p, C.c_int64, c_stream]),
     "llmrec_proj_wgrad_scratch": (C.c_int64, [C.c_int64, C.c_int32, C.c_int32, C.c_int32]),

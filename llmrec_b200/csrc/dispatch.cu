@@ -1,54 +1,70 @@
 // C-ABI entry points that pick between the wgmma kernels and the exact SIMT kernels by `mode`
 // (0 = wgmma 3xTF32, 1 = wgmma TF32, 2 = fp32 SIMT) and by shape support.
+#include <vector>
 #include "common.cuh"
 
 namespace llmrec {
 int proj_fwd_simt(const float*, int64_t, const float*, const float*, float*, int64_t, int64_t, int, int, cudaStream_t);
+int proj_fwd_simt(const uint16_t*, int64_t, const float*, const float*, float*, int64_t, int64_t, int, int, cudaStream_t);
 int proj_wgrad_simt(const float*, int64_t, const float*, int64_t, float*, float*, int64_t, int, int, int, cudaStream_t);
+int proj_wgrad_simt(const uint16_t*, int64_t, const float*, int64_t, float*, float*, int64_t, int, int, int, cudaStream_t);
 int score_topk_simt(const float*, int64_t, const float*, int64_t, const int*, int, int, int, const int*, const int*, int, int*, float*, float*, int64_t, cudaStream_t);
-bool proj_tc_supported(int d, int64_t ldx, const void* X, int k, bool wgrad);
-int proj_fwd_tc_group(const llmrec_proj_fwd_problem*, int, int, int, cudaStream_t);
-int proj_wgrad_tc_group(const llmrec_proj_wgrad_problem*, int, int, int, float*, int64_t, cudaStream_t);
-int64_t proj_wgrad_tc_scratch(const llmrec_proj_wgrad_problem*, int, int);
+bool proj_tc_supported(int d, int64_t ldx, const void* X, int k, bool wgrad, bool bf16);
+int proj_fwd_tc_group(const llmrec_proj_fwd_problem*, int, int, int, bool, cudaStream_t);
+int proj_wgrad_tc_group(const llmrec_proj_wgrad_problem*, int, int, int, bool, float*, int64_t, cudaStream_t);
+int64_t proj_wgrad_tc_scratch(const llmrec_proj_wgrad_problem*, int, int, bool);
 bool score_tc_supported(int d, int K, long long ldu, long long ldi, const void* U, const void* I);
 long long score_tc_scratch(int n_batch, int n_items, int d, int K);
 int score_topk_tc(const float*, long long, const float*, long long, const int*, int, int, int, const int*, const int*, int, int*, float*, float*, long long, cudaStream_t);
 }  // namespace llmrec
 using namespace llmrec;
 
-static bool fwd_tc_ok(const llmrec_proj_fwd_problem* pr, int n, int d, int mode) {
+// bf16 X: the bf16 problems travel in the fp32 structs (same layout; X then holds a bf16 table's address), the tensor-core path
+// reads W as bf16 terms in modes 0 and 1 (wsplit needed in both)
+static bool fwd_tc_ok(const llmrec_proj_fwd_problem* pr, int n, int d, int mode, bool bf16) {
   if (mode == 2 || n > 8) return false;
   for (int p = 0; p < n; ++p)
-    if (!proj_tc_supported(d, pr[p].ldx, pr[p].X, pr[p].k, false) || pr[p].ldy % 4 != 0 || !aligned16(pr[p].Y) || !aligned16(pr[p].W) ||
-        (pr[p].bias && !aligned16(pr[p].bias)) || (mode == 0 && !pr[p].wsplit))
+    if (!proj_tc_supported(d, pr[p].ldx, pr[p].X, pr[p].k, false, bf16) || pr[p].ldy % 4 != 0 || !aligned16(pr[p].Y) || !aligned16(pr[p].W) ||
+        (pr[p].bias && !aligned16(pr[p].bias)) || ((mode == 0 || bf16) && !pr[p].wsplit))
       return false;
   return true;
 }
-static bool wg_tc_ok(const llmrec_proj_wgrad_problem* pr, int n, int d, int mode) {
+static bool wg_tc_ok(const llmrec_proj_wgrad_problem* pr, int n, int d, int mode, bool bf16) {
   if (mode == 2 || n > 8) return false;
   for (int p = 0; p < n; ++p)
-    if (!proj_tc_supported(d, pr[p].ldx, pr[p].X, pr[p].k, true) || pr[p].lddy % 4 != 0 || !aligned16(pr[p].dY)) return false;
+    if (!proj_tc_supported(d, pr[p].ldx, pr[p].X, pr[p].k, true, bf16) || pr[p].lddy % 4 != 0 || !aligned16(pr[p].dY)) return false;
   return true;
 }
 
-extern "C" int llmrec_proj_fwd_group_f32(const llmrec_proj_fwd_problem* pr, int32_t n_prob, int32_t d, int32_t mode, llmrec_stream_t stream) {
+static int proj_fwd_group(const llmrec_proj_fwd_problem* pr, int32_t n_prob, int32_t d, int32_t mode, bool bf16, llmrec_stream_t stream) {
   LLMREC_REQUIRE_DEVICE();
   LLMREC_CHECK_ARG(n_prob >= 1 && d >= 1, "proj_fwd_group: bad sizes");
   cudaStream_t st = as_stream(stream);
   for (int p0 = 0; p0 < n_prob; p0 += 8) {
     int np = n_prob - p0 < 8 ? n_prob - p0 : 8;
-    if (fwd_tc_ok(pr + p0, np, d, mode)) {
-      int rc = proj_fwd_tc_group(pr + p0, np, d, mode, st);
+    if (fwd_tc_ok(pr + p0, np, d, mode, bf16)) {
+      int rc = proj_fwd_tc_group(pr + p0, np, d, mode, bf16, st);
       if (rc) return rc;
     } else {
       for (int p = p0; p < p0 + np; ++p) {
         if (pr[p].n <= 0) continue;
-        int rc = proj_fwd_simt(pr[p].X, pr[p].ldx, pr[p].W, pr[p].bias, pr[p].Y, pr[p].ldy, pr[p].n, pr[p].k, d, st);
+        int rc = bf16 ? proj_fwd_simt(reinterpret_cast<const uint16_t*>(pr[p].X), pr[p].ldx, pr[p].W, pr[p].bias, pr[p].Y, pr[p].ldy, pr[p].n, pr[p].k, d, st)
+                      : proj_fwd_simt(pr[p].X, pr[p].ldx, pr[p].W, pr[p].bias, pr[p].Y, pr[p].ldy, pr[p].n, pr[p].k, d, st);
         if (rc) return rc;
       }
     }
   }
   return 0;
+}
+extern "C" int llmrec_proj_fwd_group_f32(const llmrec_proj_fwd_problem* pr, int32_t n_prob, int32_t d, int32_t mode, llmrec_stream_t stream) {
+  return proj_fwd_group(pr, n_prob, d, mode, false, stream);
+}
+extern "C" int llmrec_proj_fwd_group_bf16(const llmrec_proj_fwd_problem_bf16* pr, int32_t n_prob, int32_t d, int32_t mode, llmrec_stream_t stream) {
+  LLMREC_CHECK_ARG(pr && n_prob >= 1, "proj_fwd_group: bad sizes");
+  std::vector<llmrec_proj_fwd_problem> q(n_prob);
+  for (int p = 0; p < n_prob; ++p)
+    q[p] = {reinterpret_cast<const float*>(pr[p].X), pr[p].W, pr[p].bias, pr[p].Y, pr[p].wsplit, pr[p].ldx, pr[p].ldy, pr[p].n, pr[p].k, 0};
+  return proj_fwd_group(q.data(), n_prob, d, mode, true, stream);
 }
 extern "C" int llmrec_proj_fwd_f32(const float* X, int64_t ldx, const float* W, const float* bias, float* Y, int64_t ldy,
                                    int64_t n, int32_t k, int32_t d, int32_t mode, float* wsplit, llmrec_stream_t stream) {
@@ -57,38 +73,61 @@ extern "C" int llmrec_proj_fwd_f32(const float* X, int64_t ldx, const float* W, 
   return llmrec_proj_fwd_group_f32(&p, 1, d, mode, stream);
 }
 
-extern "C" int64_t llmrec_proj_wgrad_group_scratch(const llmrec_proj_wgrad_problem* pr, int32_t n_prob, int32_t d, int32_t mode) {
+static int64_t proj_wgrad_scratch(const llmrec_proj_wgrad_problem* pr, int32_t n_prob, int32_t d, int32_t mode, bool bf16) {
   int64_t need = 0;
   for (int p0 = 0; p0 < n_prob; p0 += 8) {
     int np = n_prob - p0 < 8 ? n_prob - p0 : 8;
-    if (wg_tc_ok(pr + p0, np, d, mode)) { int64_t s = proj_wgrad_tc_scratch(pr + p0, np, d); need = s > need ? s : need; }
+    if (wg_tc_ok(pr + p0, np, d, mode, bf16)) { int64_t s = proj_wgrad_tc_scratch(pr + p0, np, d, bf16); need = s > need ? s : need; }
   }
   return need;
 }
-extern "C" int llmrec_proj_wgrad_group_f32(const llmrec_proj_wgrad_problem* pr, int32_t n_prob, int32_t d, int32_t mode,
-                                           float* scratch, int64_t scratch_elems, llmrec_stream_t stream) {
+static int proj_wgrad_group(const llmrec_proj_wgrad_problem* pr, int32_t n_prob, int32_t d, int32_t mode, bool bf16,
+                            float* scratch, int64_t scratch_elems, llmrec_stream_t stream) {
   LLMREC_REQUIRE_DEVICE();
   LLMREC_CHECK_ARG(n_prob >= 1 && d >= 1, "proj_wgrad_group: bad sizes");
   cudaStream_t st = as_stream(stream);
   for (int p0 = 0; p0 < n_prob; p0 += 8) {
     int np = n_prob - p0 < 8 ? n_prob - p0 : 8;
-    if (wg_tc_ok(pr + p0, np, d, mode)) {
-      int rc = proj_wgrad_tc_group(pr + p0, np, d, mode, scratch, scratch_elems, st);
+    if (wg_tc_ok(pr + p0, np, d, mode, bf16)) {
+      int rc = proj_wgrad_tc_group(pr + p0, np, d, mode, bf16, scratch, scratch_elems, st);
       if (rc) return rc;
     } else {
       for (int p = p0; p < p0 + np; ++p) {
-        int rc = proj_wgrad_simt(pr[p].X, pr[p].ldx, pr[p].dY, pr[p].lddy, pr[p].dW, pr[p].db, pr[p].n, pr[p].k, d, pr[p].accumulate & LLMREC_WGRAD_ACCUMULATE, st);
+        const int acc = pr[p].accumulate & LLMREC_WGRAD_ACCUMULATE;
+        int rc = bf16 ? proj_wgrad_simt(reinterpret_cast<const uint16_t*>(pr[p].X), pr[p].ldx, pr[p].dY, pr[p].lddy, pr[p].dW, pr[p].db, pr[p].n, pr[p].k, d, acc, st)
+                      : proj_wgrad_simt(pr[p].X, pr[p].ldx, pr[p].dY, pr[p].lddy, pr[p].dW, pr[p].db, pr[p].n, pr[p].k, d, acc, st);
         if (rc) return rc;
       }
     }
   }
   return 0;
 }
+static std::vector<llmrec_proj_wgrad_problem> as_f32_layout(const llmrec_proj_wgrad_problem_bf16* pr, int32_t n_prob) {
+  std::vector<llmrec_proj_wgrad_problem> q(n_prob > 0 ? n_prob : 0);
+  for (int p = 0; p < n_prob; ++p)
+    q[p] = {reinterpret_cast<const float*>(pr[p].X), pr[p].dY, pr[p].dW, pr[p].db, pr[p].ldx, pr[p].lddy, pr[p].n, pr[p].k, pr[p].accumulate};
+  return q;
+}
+extern "C" int64_t llmrec_proj_wgrad_group_scratch(const llmrec_proj_wgrad_problem* pr, int32_t n_prob, int32_t d, int32_t mode) {
+  return proj_wgrad_scratch(pr, n_prob, d, mode, false);
+}
+extern "C" int64_t llmrec_proj_wgrad_group_bf16_scratch(const llmrec_proj_wgrad_problem_bf16* pr, int32_t n_prob, int32_t d, int32_t mode) {
+  return proj_wgrad_scratch(as_f32_layout(pr, n_prob).data(), n_prob, d, mode, true);
+}
+extern "C" int llmrec_proj_wgrad_group_f32(const llmrec_proj_wgrad_problem* pr, int32_t n_prob, int32_t d, int32_t mode,
+                                           float* scratch, int64_t scratch_elems, llmrec_stream_t stream) {
+  return proj_wgrad_group(pr, n_prob, d, mode, false, scratch, scratch_elems, stream);
+}
+extern "C" int llmrec_proj_wgrad_group_bf16(const llmrec_proj_wgrad_problem_bf16* pr, int32_t n_prob, int32_t d, int32_t mode,
+                                            float* scratch, int64_t scratch_elems, llmrec_stream_t stream) {
+  LLMREC_CHECK_ARG(pr && n_prob >= 1, "proj_wgrad_group: bad sizes");
+  return proj_wgrad_group(as_f32_layout(pr, n_prob).data(), n_prob, d, mode, true, scratch, scratch_elems, stream);
+}
 extern "C" int64_t llmrec_proj_wgrad_scratch(int64_t n, int32_t k, int32_t d, int32_t mode) {
   llmrec_proj_wgrad_problem p{nullptr, nullptr, nullptr, nullptr, 4, 4, n, k, 0};
   // alignment of real pointers is checked at call time; size the scratch for the tensor-core path
   if (mode == 2 || d % 32 != 0 || d > 256 || k % 4 != 0) return 0;
-  return proj_wgrad_tc_scratch(&p, 1, d);
+  return proj_wgrad_tc_scratch(&p, 1, d, false);
 }
 extern "C" int llmrec_proj_wgrad_f32(const float* X, int64_t ldx, const float* dY, int64_t lddy, float* dW, float* db,
                                      int64_t n, int32_t k, int32_t d, int32_t accumulate, int32_t mode,

@@ -1,12 +1,18 @@
 // Exact-fp32 SIMT version of the side-feature projection and its weight gradient
 // (nn.Linear at Models.py:145-150).  mode 2 of llmrec_proj_*: the bit-conservative path used as the
 // on-device checker for the wgmma kernels (proj_tc.cu) and for shapes those do not cover.
+// Templated on the element type of X: fp32, or bf16 (raw uint16_t bits) widened to fp32 on load -- the same FMA order, so a bf16
+// table gives the bits of the fp32 kernel on its upcast copy.
 #include "common.cuh"
 
 namespace llmrec {
 
+__device__ __forceinline__ float x_f32(float x) { return x; }
+__device__ __forceinline__ float x_f32(uint16_t x) { return __uint_as_float((uint32_t)x << 16); }
+
 // Y[n x d] = X[n x k] W^T[k x d] + b ; 64x64 tile, K step 16, 4x4 per thread
-__global__ void __launch_bounds__(256) proj_fwd_simt_kernel(const float* __restrict__ X, int64_t ldx, const float* __restrict__ W,
+template <class T>
+__global__ void __launch_bounds__(256) proj_fwd_simt_kernel(const T* __restrict__ X, int64_t ldx, const float* __restrict__ W,
                                                             const float* __restrict__ bias, float* __restrict__ Y, int64_t ldy,
                                                             int64_t n, int k, int d) {
   __shared__ float Xs[16][64 + 4];
@@ -19,7 +25,7 @@ __global__ void __launch_bounds__(256) proj_fwd_simt_kernel(const float* __restr
     for (int i = threadIdx.x; i < 64 * 16; i += 256) {
       int r = i >> 4, kk = i & 15;
       int64_t gr = row0 + r;
-      Xs[kk][r] = (gr < n && k0 + kk < k) ? X[gr * ldx + k0 + kk] : 0.f;
+      Xs[kk][r] = (gr < n && k0 + kk < k) ? x_f32(X[gr * ldx + k0 + kk]) : 0.f;
       int gc = col0 + r;
       Ws[kk][r] = (gc < d && k0 + kk < k) ? W[(int64_t)gc * k + k0 + kk] : 0.f;
     }
@@ -49,7 +55,8 @@ __global__ void __launch_bounds__(256) proj_fwd_simt_kernel(const float* __restr
 }
 
 // dW[d x k] += sum_r dY[r,:]^T X[r,:] over a row chunk ; db[d] += colsum(dY) (k-tile 0 only)
-__global__ void __launch_bounds__(256) proj_wgrad_simt_kernel(const float* __restrict__ X, int64_t ldx, const float* __restrict__ dY, int64_t lddy,
+template <class T>
+__global__ void __launch_bounds__(256) proj_wgrad_simt_kernel(const T* __restrict__ X, int64_t ldx, const float* __restrict__ dY, int64_t lddy,
                                                               float* __restrict__ dW, float* __restrict__ db, int64_t n, int k, int d, int rows_per_chunk) {
   __shared__ float Gs[16][64 + 4];  // dY tile  [r][dcol]
   __shared__ float Xs[16][64 + 4];  // X tile   [r][kcol]
@@ -64,7 +71,7 @@ __global__ void __launch_bounds__(256) proj_wgrad_simt_kernel(const float* __res
       int r = i >> 6, c = i & 63;
       int64_t gr = r0 + r;
       Gs[r][c] = (gr < r_end && d0 + c < d) ? dY[gr * lddy + d0 + c] : 0.f;
-      Xs[r][c] = (gr < r_end && k0 + c < k) ? X[gr * ldx + k0 + c] : 0.f;
+      Xs[r][c] = (gr < r_end && k0 + c < k) ? x_f32(X[gr * ldx + k0 + c]) : 0.f;
     }
     __syncthreads();
 #pragma unroll
@@ -94,21 +101,35 @@ __global__ void __launch_bounds__(256) proj_wgrad_simt_kernel(const float* __res
   }
 }
 
-int proj_fwd_simt(const float* X, int64_t ldx, const float* W, const float* bias, float* Y, int64_t ldy, int64_t n, int k, int d, cudaStream_t st) {
+template <class T>
+static int fwd_simt(const T* X, int64_t ldx, const float* W, const float* bias, float* Y, int64_t ldy, int64_t n, int k, int d, cudaStream_t st) {
   dim3 grid((unsigned)((n + 63) / 64), (d + 63) / 64);
-  proj_fwd_simt_kernel<<<grid, 256, 0, st>>>(X, ldx, W, bias, Y, ldy, n, k, d);
+  proj_fwd_simt_kernel<T><<<grid, 256, 0, st>>>(X, ldx, W, bias, Y, ldy, n, k, d);
   LLMREC_CHECK_LAUNCH("proj_fwd_simt");
   return 0;
 }
-int proj_wgrad_simt(const float* X, int64_t ldx, const float* dY, int64_t lddy, float* dW, float* db, int64_t n, int k, int d, int accumulate, cudaStream_t st) {
+template <class T>
+static int wgrad_simt(const T* X, int64_t ldx, const float* dY, int64_t lddy, float* dW, float* db, int64_t n, int k, int d, int accumulate, cudaStream_t st) {
   if (!accumulate) {
     cudaMemsetAsync(dW, 0, sizeof(float) * (size_t)d * k, st);
     if (db) cudaMemsetAsync(db, 0, sizeof(float) * d, st);
   }
   const int rows_per_chunk = 1024;
   dim3 grid((k + 63) / 64, (d + 63) / 64, (unsigned)((n + rows_per_chunk - 1) / rows_per_chunk));
-  proj_wgrad_simt_kernel<<<grid, 256, 0, st>>>(X, ldx, dY, lddy, dW, db, n, k, d, rows_per_chunk);
+  proj_wgrad_simt_kernel<T><<<grid, 256, 0, st>>>(X, ldx, dY, lddy, dW, db, n, k, d, rows_per_chunk);
   LLMREC_CHECK_LAUNCH("proj_wgrad_simt");
   return 0;
+}
+int proj_fwd_simt(const float* X, int64_t ldx, const float* W, const float* bias, float* Y, int64_t ldy, int64_t n, int k, int d, cudaStream_t st) {
+  return fwd_simt(X, ldx, W, bias, Y, ldy, n, k, d, st);
+}
+int proj_fwd_simt(const uint16_t* X, int64_t ldx, const float* W, const float* bias, float* Y, int64_t ldy, int64_t n, int k, int d, cudaStream_t st) {
+  return fwd_simt(X, ldx, W, bias, Y, ldy, n, k, d, st);
+}
+int proj_wgrad_simt(const float* X, int64_t ldx, const float* dY, int64_t lddy, float* dW, float* db, int64_t n, int k, int d, int accumulate, cudaStream_t st) {
+  return wgrad_simt(X, ldx, dY, lddy, dW, db, n, k, d, accumulate, st);
+}
+int proj_wgrad_simt(const uint16_t* X, int64_t ldx, const float* dY, int64_t lddy, float* dW, float* db, int64_t n, int k, int d, int accumulate, cudaStream_t st) {
+  return wgrad_simt(X, ldx, dY, lddy, dW, db, n, k, d, accumulate, st);
 }
 }  // namespace llmrec

@@ -22,6 +22,9 @@
 //   wgrad    A = X^T (M = features, K = rows): the fragment is read transposed out of the raw X tile, which arrives as TM/32
 //            boxes [32 rows][32 features] with the 128-byte swizzle; features are permuted inside the tile so that the reads
 //            are bank-conflict free (arithmetic at ld_frag_wgrad), and the epilogue undoes the permutation.
+// bf16 X (--feat_dtype bf16, BF16 = true): the same pipeline with 64 k / rows per stage.  X is exact in bf16, so it is not split and
+// A is read by descriptor straight from the stage (wgrad: MN-major, no permutation); W / dY^T arrive as three exact bf16 terms
+// (wsplit_bf16, dyt_split<true>) and each k16 step issues X*w2 + X*w1 + X*w0: no product term is dropped (mode 1: X*w0 only).
 #include <mutex>
 #include <stdlib.h>
 #include <vector>
@@ -55,12 +58,12 @@ static EncodeFn get_encode() {
   return fn;
 }
 
-bool make_tmap_2d_f32(CUtensorMap* out, const void* base, uint64_t inner, uint64_t outer, uint64_t row_stride_bytes,
-                      uint32_t box_inner, uint32_t box_outer, bool swizzle128) {
+bool make_tmap_2d(CUtensorMap* out, CUtensorMapDataType dtype, const void* base, uint64_t inner, uint64_t outer, uint64_t row_stride_bytes,
+                  uint32_t box_inner, uint32_t box_outer, bool swizzle128) {
   struct Entry { TmapKey k; CUtensorMap m; };
   static std::vector<Entry> cache;
   static std::mutex mu;
-  TmapKey key{base, inner, outer, row_stride_bytes, box_inner, box_outer, swizzle128 ? 1u : 0u, 0u};
+  TmapKey key{base, inner, outer, row_stride_bytes, box_inner, box_outer, swizzle128 ? 1u : 0u, (uint32_t)dtype};
   std::lock_guard<std::mutex> lock(mu);
   for (auto& e : cache)
     if (memcmp(&e.k, &key, sizeof(key)) == 0) { *out = e.m; return true; }
@@ -70,7 +73,7 @@ bool make_tmap_2d_f32(CUtensorMap* out, const void* base, uint64_t inner, uint64
   cuuint64_t strides[1] = {row_stride_bytes};
   cuuint32_t box[2] = {box_inner, box_outer};
   cuuint32_t estr[2] = {1, 1};
-  CUresult r = enc(out, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<void*>(base), dims, strides, box, estr,
+  CUresult r = enc(out, dtype, 2, const_cast<void*>(base), dims, strides, box, estr,
                    CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle128 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled failed (%d) inner=%llu outer=%llu stride=%llu box=%ux%u", (int)r,
@@ -90,12 +93,15 @@ __device__ __forceinline__ uint8_t* align1024(uint8_t* p) {
 constexpr uint32_t kSmemMax = 227u * 1024u;   // dynamic shared memory per block on sm_90
 constexpr int kProducerRegs = 40, kConsumerRegs = 232;   // 128 * 40 + 256 * 232 <= 65536 (launched at 384 x 168)
 
-template <int D, bool SPLIT, int MB>
+// BF16: X is a bf16 table.  A stage then covers 64 k (fwd) / rows (wgrad) in the same bytes, and a 3-way split of the fp32
+// operand (W or dY^T) gives three B tiles instead of two.
+template <int D, bool SPLIT, int MB, bool BF16 = false>
 struct ProjCfg {
   static constexpr int TM = tile_m(MB);
-  static constexpr uint32_t kX = TM * BK * 4u;                 // X tile of one stage
-  static constexpr uint32_t kB = D * BK * 4u;                  // one B operand tile [D][32], hi or lo
-  static constexpr uint32_t kStage = kX + kB * (SPLIT ? 2u : 1u);
+  static constexpr int NB = SPLIT ? (BF16 ? 3 : 2) : 1;        // B tiles per stage
+  static constexpr uint32_t kX = TM * 128u;                    // X tile of one stage: 128 bytes per row / feature
+  static constexpr uint32_t kB = D * 128u;                     // one B operand tile [D][32 fp32 | 64 bf16]
+  static constexpr uint32_t kStage = kX + kB * NB;
   static constexpr int kFit = (int)((kSmemMax - 1024u - 256u) / kStage);
   static constexpr int kStages = kFit > 4 ? 4 : kFit;          // 4 at d = 64, 3 at d = 128, 2 at d = 256
   static constexpr uint32_t kSmem = 1024u /*align slack*/ + kStages * kStage + 2u * kStages * 8u;
@@ -134,9 +140,10 @@ __device__ __forceinline__ void ld_frag_wgrad(uint32_t (&a)[4], uint32_t sx, int
 }
 
 // work unit -> (problem, number of k-blocks, what the producer loads for k-block kb, where the epilogue writes)
-template <int D, bool SPLIT, int MB>
+template <int D, bool SPLIT, int MB, bool BF16 = false>
 struct FwdUnit {
-  using Cfg = ProjCfg<D, SPLIT, MB>;
+  using Cfg = ProjCfg<D, SPLIT, MB, BF16>;
+  static constexpr int kTransA = 0;   // bf16: A = the X tile as it arrived, K-major
   const FwdParams& P; int p, mblk, kb_n;
   __device__ FwdUnit(const FwdParams& P_, int u) : P(P_) {
     p = 0;
@@ -145,11 +152,14 @@ struct FwdUnit {
     kb_n = P.prob[p].kblocks;
   }
   __device__ void issue(uint8_t* st, uint64_t* bar, int kb, uint64_t pol) const {
-    tma_load_2d_hint(st, &P.tmA[p], bar, kb * BK, mblk * Cfg::TM, pol);
-    tma_load_2d(st + Cfg::kX, &P.tmW[p], bar, kb * BK, 0);
-    if (SPLIT) tma_load_2d(st + Cfg::kX + Cfg::kB, &P.tmW[p], bar, kb * BK, D);
+    constexpr int bk = stage_k(BF16);
+    tma_load_2d_hint(st, &P.tmA[p], bar, kb * bk, mblk * Cfg::TM, pol);
+#pragma unroll
+    for (int i = 0; i < Cfg::NB; ++i) tma_load_2d(st + Cfg::kX + i * Cfg::kB, &P.tmW[p], bar, kb * bk, i * D);
   }
   static __device__ void ld_frag(uint32_t (&a)[4], uint32_t sx, int blk, int kk, int warp, int lane) { ld_frag_fwd(a, sx, blk, kk, warp, lane); }
+  // bf16: descriptor of m64 block `blk` (64 rows x 128 bytes), k16 step kk (+32 bytes inside the swizzled rows)
+  static __device__ uint64_t a_desc(uint32_t sx, int blk, int kk) { return gmma_desc_sw128(sx + blk * 8192u + kk * 32u); }
   __device__ void store(float (&acc)[MB][D / 2], int cw, int warp, int lane) const {   // registers (+bias) -> Y
     const FwdProblem& pr = P.prob[p];
     const int g = lane >> 2, t = lane & 3;
@@ -171,9 +181,11 @@ struct FwdUnit {
   }
 };
 
-template <int D, bool SPLIT, int MB>
+template <int D, bool SPLIT, int MB, bool BF16 = false>
 struct WgUnit {
-  using Cfg = ProjCfg<D, SPLIT, MB>;
+  using Cfg = ProjCfg<D, SPLIT, MB, BF16>;
+  static constexpr int kBk = stage_k(BF16);
+  static constexpr int kTransA = 1;   // bf16: A = X^T, read MN-major out of the raw X tile (no feature permutation)
   const WgParams& P; int p, u, ft, r0, kb_n;
   __device__ WgUnit(const WgParams& P_, int u_) : P(P_), u(u_) {
     p = 0;
@@ -182,16 +194,23 @@ struct WgUnit {
     const int local = u - pr.item_start, chunk = local / pr.ft_tiles;
     ft = local - chunk * pr.ft_tiles;
     r0 = chunk * pr.rows_per_chunk;
-    kb_n = (min(pr.n, r0 + pr.rows_per_chunk) - r0 + BK - 1) / BK;   // chunks are BK-aligned; rows past n load as zeros
+    kb_n = (min(pr.n, r0 + pr.rows_per_chunk) - r0 + kBk - 1) / kBk;   // chunks are stage-aligned; rows past n load as zeros
   }
   __device__ void issue(uint8_t* st, uint64_t* bar, int kb, uint64_t pol) const {
-    const int r = r0 + kb * BK;
+    const int r = r0 + kb * kBk;
+    if constexpr (BF16) {   // TM/64 boxes [64 rows][64 features], 8 KiB each: one per m64 block
 #pragma unroll
-    for (int b = 0; b < Cfg::TM / 32; ++b) tma_load_2d_hint(st + b * 4096, &P.tmX[p], bar, ft * Cfg::TM + 32 * b, r, pol);
-    tma_load_2d(st + Cfg::kX, &P.tmG[p], bar, r, 0);
-    if (SPLIT) tma_load_2d(st + Cfg::kX + Cfg::kB, &P.tmG[p], bar, r, D);
+      for (int b = 0; b < Cfg::TM / 64; ++b) tma_load_2d_hint(st + b * 8192, &P.tmX[p], bar, ft * Cfg::TM + 64 * b, r, pol);
+    } else {
+#pragma unroll
+      for (int b = 0; b < Cfg::TM / 32; ++b) tma_load_2d_hint(st + b * 4096, &P.tmX[p], bar, ft * Cfg::TM + 32 * b, r, pol);
+    }
+#pragma unroll
+    for (int i = 0; i < Cfg::NB; ++i) tma_load_2d(st + Cfg::kX + i * Cfg::kB, &P.tmG[p], bar, r, i * D);
   }
   static __device__ void ld_frag(uint32_t (&a)[4], uint32_t sx, int blk, int kk, int warp, int lane) { ld_frag_wgrad(a, sx, blk, kk, warp, lane); }
+  // bf16: descriptor of m64 block `blk` (its own box), k16 step kk = rows 16kk .. 16kk + 15 (+2048 bytes)
+  static __device__ uint64_t a_desc(uint32_t sx, int blk, int kk) { return gmma_desc_sw128_mn(sx + blk * 8192u + kk * 2048u); }
   __device__ void store(float (&acc)[MB][D / 2], int cw, int warp, int lane) const {   // registers -> partial[item][feature][d]
     const int g = lane >> 2, t = lane & 3;
     float* out = P.partial + (long long)u * Cfg::TM * D;
@@ -199,16 +218,17 @@ struct WgUnit {
     for (int j = 0; j < MB; ++j)
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
-        float* o = out + (long long)wgrad_feature(cw * MB + j, warp, h, g) * D + 2 * t;
+        const int f = BF16 ? (cw * MB + j) * 64 + warp * 16 + 8 * h + g : wgrad_feature(cw * MB + j, warp, h, g);
+        float* o = out + (long long)f * D + 2 * t;
 #pragma unroll
         for (int c = 0; c < D / 8; ++c) *reinterpret_cast<float2*>(o + c * 8) = make_float2(acc[j][4 * c + 2 * h], acc[j][4 * c + 2 * h + 1]);
       }
   }
 };
 
-template <int D, bool SPLIT, int MB, class Unit, class Params>
+template <int D, bool SPLIT, int MB, bool BF16, class Unit, class Params>
 __device__ __forceinline__ void proj_pipeline(const Params& P, int total) {
-  using Cfg = ProjCfg<D, SPLIT, MB>;
+  using Cfg = ProjCfg<D, SPLIT, MB, BF16>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = align1024(smem_raw);
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + Cfg::kStages * Cfg::kStage);
@@ -252,33 +272,54 @@ __device__ __forceinline__ void proj_pipeline(const Params& P, int total) {
     for (int kb = 0; kb < w.kb_n; ++kb) {
       mbar_wait(&full[s], ph);
       const uint32_t st = smem_u32(smem + s * Cfg::kStage), bh = st + Cfg::kX, bl = bh + Cfg::kB;
+      if constexpr (BF16) {
+        // X is exact in bf16: A comes straight from the stage by descriptor, B = w0 (or dY^T's first term) [+ w1 + w2], the
+        // smallest term first.  One k16 step = one wgmma group; the previous group runs while this one is issued.
 #pragma unroll
-      for (int kk = 0; kk < 4; ++kk) {   // one k8 step = one wgmma group; the previous group runs while this one is loaded
-        uint32_t ah[MB][4], al[MB][4];
+        for (int kk = 0; kk < 4; ++kk) {
+          wgmma_fence();
 #pragma unroll
-        for (int j = 0; j < MB; ++j) {
-          Unit::ld_frag(ah[j], st, cw * MB + j, kk, warp, lane);
-          if (SPLIT)
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-              const float x = __uint_as_float(ah[j][i]), hi = tf32_hi(x);
-              ah[j][i] = __float_as_uint(hi);
-              al[j][i] = __float_as_uint(x - hi);
+          for (int j = 0; j < MB; ++j) {
+            const uint64_t a = Unit::a_desc(st, cw * MB + j, kk);
+            if (SPLIT) {
+              WgmmaSSbf16<D, Unit::kTransA>::mma(acc[j], a, gmma_desc_sw128(bl + Cfg::kB + kk * 32u));   // X * w2
+              WgmmaSSbf16<D, Unit::kTransA>::mma(acc[j], a, gmma_desc_sw128(bl + kk * 32u));             // X * w1
             }
-        }
-        wgmma_fence();
-        const uint64_t dh = gmma_desc_sw128(bh + kk * 32u);
-#pragma unroll
-        for (int j = 0; j < MB; ++j) {
-          if (SPLIT) {
-            WgmmaRS<D>::mma(acc[j], al[j], dh);                               // lo * hi
-            WgmmaRS<D>::mma(acc[j], ah[j], gmma_desc_sw128(bl + kk * 32u));   // hi * lo
+            WgmmaSSbf16<D, Unit::kTransA>::mma(acc[j], a, gmma_desc_sw128(bh + kk * 32u));               // X * w0
           }
-          WgmmaRS<D>::mma(acc[j], ah[j], dh);                                 // hi * hi
+          wgmma_commit();
+          wgmma_wait<1>();
+          if (kk == 0 && prev >= 0 && lane == 0) mbar_arrive(&empty[prev]);   // the previous stage's last group is done
         }
-        wgmma_commit();
-        wgmma_wait<1>();
-        if (kk == 0 && prev >= 0 && lane == 0) mbar_arrive(&empty[prev]);   // the previous stage's last group is done
+      } else {
+#pragma unroll
+        for (int kk = 0; kk < 4; ++kk) {   // one k8 step = one wgmma group; the previous group runs while this one is loaded
+          uint32_t ah[MB][4], al[MB][4];
+#pragma unroll
+          for (int j = 0; j < MB; ++j) {
+            Unit::ld_frag(ah[j], st, cw * MB + j, kk, warp, lane);
+            if (SPLIT)
+#pragma unroll
+              for (int i = 0; i < 4; ++i) {
+                const float x = __uint_as_float(ah[j][i]), hi = tf32_hi(x);
+                ah[j][i] = __float_as_uint(hi);
+                al[j][i] = __float_as_uint(x - hi);
+              }
+          }
+          wgmma_fence();
+          const uint64_t dh = gmma_desc_sw128(bh + kk * 32u);
+#pragma unroll
+          for (int j = 0; j < MB; ++j) {
+            if (SPLIT) {
+              WgmmaRS<D>::mma(acc[j], al[j], dh);                               // lo * hi
+              WgmmaRS<D>::mma(acc[j], ah[j], gmma_desc_sw128(bl + kk * 32u));   // hi * lo
+            }
+            WgmmaRS<D>::mma(acc[j], ah[j], dh);                                 // hi * hi
+          }
+          wgmma_commit();
+          wgmma_wait<1>();
+          if (kk == 0 && prev >= 0 && lane == 0) mbar_arrive(&empty[prev]);   // the previous stage's last group is done
+        }
       }
       prev = s;
       if (++s == Cfg::kStages) { s = 0; ph ^= 1u; }
@@ -289,14 +330,14 @@ __device__ __forceinline__ void proj_pipeline(const Params& P, int total) {
   }
 }
 
-template <int D, bool SPLIT, int MB>
+template <int D, bool SPLIT, int MB, bool BF16>
 __global__ void __launch_bounds__(384, 1) proj_fwd_tc_kernel(const __grid_constant__ FwdParams P) {
-  proj_pipeline<D, SPLIT, MB, FwdUnit<D, SPLIT, MB>>(P, P.total_tiles);
+  proj_pipeline<D, SPLIT, MB, BF16, FwdUnit<D, SPLIT, MB, BF16>>(P, P.total_tiles);
 }
 
-template <int D, bool SPLIT, int MB>
+template <int D, bool SPLIT, int MB, bool BF16>
 __global__ void __launch_bounds__(384, 1) proj_wgrad_tc_kernel(const __grid_constant__ WgParams P) {
-  proj_pipeline<D, SPLIT, MB, WgUnit<D, SPLIT, MB>>(P, P.total_items);
+  proj_pipeline<D, SPLIT, MB, BF16, WgUnit<D, SPLIT, MB, BF16>>(P, P.total_items);
 }
 
 static int num_sms() {
@@ -310,43 +351,45 @@ static int num_sms() {
 // MB = 2 (256-wide tiles: half the W / dY^T re-reads from L2) where the accumulators fit (d <= 128) and the tiles still fill every SM
 static int pick_mb(int d, long long units_at_256) { return d <= 128 && units_at_256 >= num_sms() ? 2 : 1; }
 
-template <int D, bool SPLIT, int MB>
+template <int D, bool SPLIT, int MB, bool BF16>
 static int launch_fwd(const FwdParams& P, cudaStream_t st) {
-  using Cfg = ProjCfg<D, SPLIT, MB>;
-  LLMREC_CHECK_CUDA(cudaFuncSetAttribute(proj_fwd_tc_kernel<D, SPLIT, MB>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Cfg::kSmem));
+  using Cfg = ProjCfg<D, SPLIT, MB, BF16>;
+  LLMREC_CHECK_CUDA(cudaFuncSetAttribute(proj_fwd_tc_kernel<D, SPLIT, MB, BF16>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Cfg::kSmem));
   const int grid = P.total_tiles < num_sms() ? P.total_tiles : num_sms();
-  proj_fwd_tc_kernel<D, SPLIT, MB><<<grid, 384, Cfg::kSmem, st>>>(P);
+  proj_fwd_tc_kernel<D, SPLIT, MB, BF16><<<grid, 384, Cfg::kSmem, st>>>(P);
   LLMREC_CHECK_LAUNCH("proj_fwd_tc");
   return 0;
 }
 
-template <int D, bool SPLIT, int MB>
+template <int D, bool SPLIT, int MB, bool BF16>
 static int launch_wgrad(const WgParams& P, cudaStream_t st) {
-  using Cfg = ProjCfg<D, SPLIT, MB>;
-  LLMREC_CHECK_CUDA(cudaFuncSetAttribute(proj_wgrad_tc_kernel<D, SPLIT, MB>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Cfg::kSmem));
+  using Cfg = ProjCfg<D, SPLIT, MB, BF16>;
+  LLMREC_CHECK_CUDA(cudaFuncSetAttribute(proj_wgrad_tc_kernel<D, SPLIT, MB, BF16>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Cfg::kSmem));
   const int grid = P.total_items < num_sms() ? P.total_items : num_sms();
-  proj_wgrad_tc_kernel<D, SPLIT, MB><<<grid, 384, Cfg::kSmem, st>>>(P);
+  proj_wgrad_tc_kernel<D, SPLIT, MB, BF16><<<grid, 384, Cfg::kSmem, st>>>(P);
   LLMREC_CHECK_LAUNCH("proj_wgrad_tc");
   return 0;
 }
 
 // MB = 2 exists for d <= 128 only (its accumulators at d > 128 would not fit next to the fragments)
-template <int D, bool SPLIT>
+template <int D, bool SPLIT, bool BF16>
 static int launch_fwd_mb(const FwdParams& P, int mb, cudaStream_t st) {
-  if constexpr (D <= 128) { if (mb == 2) return launch_fwd<D, SPLIT, 2>(P, st); }
-  return launch_fwd<D, SPLIT, 1>(P, st);
+  if constexpr (D <= 128) { if (mb == 2) return launch_fwd<D, SPLIT, 2, BF16>(P, st); }
+  return launch_fwd<D, SPLIT, 1, BF16>(P, st);
 }
-template <int D, bool SPLIT>
+template <int D, bool SPLIT, bool BF16>
 static int launch_wgrad_mb(const WgParams& P, int mb, cudaStream_t st) {
-  if constexpr (D <= 128) { if (mb == 2) return launch_wgrad<D, SPLIT, 2>(P, st); }
-  return launch_wgrad<D, SPLIT, 1>(P, st);
+  if constexpr (D <= 128) { if (mb == 2) return launch_wgrad<D, SPLIT, 2, BF16>(P, st); }
+  return launch_wgrad<D, SPLIT, 1, BF16>(P, st);
 }
 
 #define LLMREC_PROJ_WIDTHS(X) X(32) X(64) X(96) X(128) X(160) X(192) X(224) X(256)
 
-static int fwd_launch(const FwdParams& P, bool split, int mb, cudaStream_t st) {
+static int fwd_launch(const FwdParams& P, bool split, int mb, bool bf16, cudaStream_t st) {
   switch (P.d) {
-#define LLMREC_CASE(W) case W: return split ? launch_fwd_mb<W, true>(P, mb, st) : launch_fwd_mb<W, false>(P, mb, st);
+#define LLMREC_CASE(W) case W: \
+    if (bf16) return split ? launch_fwd_mb<W, true, true>(P, mb, st) : launch_fwd_mb<W, false, true>(P, mb, st); \
+    return split ? launch_fwd_mb<W, true, false>(P, mb, st) : launch_fwd_mb<W, false, false>(P, mb, st);
     LLMREC_PROJ_WIDTHS(LLMREC_CASE)
 #undef LLMREC_CASE
   }
@@ -354,9 +397,11 @@ static int fwd_launch(const FwdParams& P, bool split, int mb, cudaStream_t st) {
   return 1;
 }
 
-static int wgrad_launch(const WgParams& P, bool split, int mb, cudaStream_t st) {
+static int wgrad_launch(const WgParams& P, bool split, int mb, bool bf16, cudaStream_t st) {
   switch (P.d) {
-#define LLMREC_CASE(W) case W: return split ? launch_wgrad_mb<W, true>(P, mb, st) : launch_wgrad_mb<W, false>(P, mb, st);
+#define LLMREC_CASE(W) case W: \
+    if (bf16) return split ? launch_wgrad_mb<W, true, true>(P, mb, st) : launch_wgrad_mb<W, false, true>(P, mb, st); \
+    return split ? launch_wgrad_mb<W, true, false>(P, mb, st) : launch_wgrad_mb<W, false, false>(P, mb, st);
     LLMREC_PROJ_WIDTHS(LLMREC_CASE)
 #undef LLMREC_CASE
   }
@@ -366,7 +411,9 @@ static int wgrad_launch(const WgParams& P, bool split, int mb, cudaStream_t st) 
 
 // dY -> dY^T [hi ; lo] ([2d x ldt], hi exactly TF32-representable; [d x ldt] unsplit in mode 1) for every problem of a grouped
 // weight gradient in ONE launch (blockIdx.z): the B operand of the wgrad kernel, K-major (rows of dY contiguous), from strided views.
+// BF16 (the bf16-X kernels): dY^T as bf16 terms [w0 ; w1 ; w2] ([3d x ldt], bf16_split3) or [d x ldt] truncated in mode 1.
 struct DytParams { const float* dY[kMaxProb]; long long ld[kMaxProb]; int n[kMaxProb]; float* out[kMaxProb]; long long ldt[kMaxProb]; int d, split; };
+template <bool BF16>
 __global__ void __launch_bounds__(256) dyt_split_kernel(const DytParams P) {
   __shared__ float tile[32][33];
   const int p = blockIdx.z, n = P.n[p], r0 = blockIdx.x * 32, e0 = blockIdx.y * 32;
@@ -377,14 +424,20 @@ __global__ void __launch_bounds__(256) dyt_split_kernel(const DytParams P) {
   for (int i = ty; i < 32; i += 8) tile[i][tx] = r0 + i < n ? __ldg(src + (long long)(r0 + i) * P.ld[p] + e0 + tx) : 0.f;
   __syncthreads();
   if (r0 + tx >= n) return;
-  float* __restrict__ dst = P.out[p];
   const long long ldt = P.ldt[p], lo = (long long)P.d * ldt;
 #pragma unroll
   for (int i = ty; i < 32; i += 8) {
     const float v = tile[tx][i];
-    float* o = dst + (long long)(e0 + i) * ldt + r0 + tx;
-    if (P.split) { const float h = tf32_hi(v); o[0] = h; o[lo] = v - h; }
-    else o[0] = v;
+    const long long at = (long long)(e0 + i) * ldt + r0 + tx;
+    if constexpr (BF16) {
+      uint16_t* o = reinterpret_cast<uint16_t*>(P.out[p]) + at;
+      if (P.split) bf16_split3(v, o[0], o[lo], o[2 * lo]);
+      else o[0] = bf16_bits(bf16_trunc(v));
+    } else {
+      float* o = P.out[p] + at;
+      if (P.split) { const float h = tf32_hi(v); o[0] = h; o[lo] = v - h; }
+      else o[0] = v;
+    }
   }
 }
 
@@ -396,6 +449,17 @@ __global__ void wsplit_kernel(const WsplitParams P) {
   const long long n = P.n[blockIdx.y];
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
     const float v = W[i]; const float h = tf32_hi(v); out[i] = h; out[n + i] = v - h;
+  }
+}
+// The bf16-X kernels' B operand: W -> bf16 [w0 ; w1 ; w2] ([3d x k], W = w0 + w1 + w2 exactly) when split, else [d x k] = w0
+// (W truncated to bf16).  6dk bytes: fits the 2dk-float wsplit buffer of the fp32 path.
+__global__ void wsplit_bf16_kernel(const WsplitParams P, int split) {
+  const float* __restrict__ W = P.W[blockIdx.y];
+  uint16_t* __restrict__ out = reinterpret_cast<uint16_t*>(P.out[blockIdx.y]);
+  const long long n = P.n[blockIdx.y];
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    if (split) bf16_split3(W[i], out[i], out[n + i], out[2 * n + i]);
+    else out[i] = bf16_bits(bf16_trunc(W[i]));
   }
 }
 
@@ -496,13 +560,20 @@ __global__ void __launch_bounds__(256) colsum_kernel(const ColsumParams P) {
 // ------------------------------------------------------------------------------------------------
 // host API (grouped)
 // ------------------------------------------------------------------------------------------------
-bool proj_tc_supported(int d, int64_t ldx, const void* X, int k, bool wgrad) {
+// bf16 X: a 16-byte TMA row pitch needs ldx % 8 == 0, and the bf16 W terms [3d x k] need k % 8 == 0
+bool proj_tc_supported(int d, int64_t ldx, const void* X, int k, bool wgrad, bool bf16) {
   (void)wgrad;   // both directions take d in multiples of 32 (wgmma N = d)
-  return d % 32 == 0 && d >= 32 && d <= 256 && ldx % 4 == 0 && aligned16(X) && k >= 1 && k % 4 == 0;
+  const int q = bf16 ? 8 : 4;
+  return d % 32 == 0 && d >= 32 && d <= 256 && ldx % q == 0 && aligned16(X) && k >= 1 && k % q == 0;
 }
 
-int proj_fwd_tc_group(const llmrec_proj_fwd_problem* pr, int n_prob, int d, int mode, cudaStream_t st) {
+static CUtensorMapDataType x_type(bool bf16) { return bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32; }
+
+// bf16: pr[p].X holds the address of a bf16 table (llmrec_proj_fwd_problem_bf16 carried in the fp32 struct's layout)
+int proj_fwd_tc_group(const llmrec_proj_fwd_problem* pr, int n_prob, int d, int mode, bool bf16, cudaStream_t st) {
   const bool split = (mode == 0);
+  const bool need_ws = split || bf16;          // bf16 kernels read W as bf16 terms in both modes
+  const int es = bf16 ? 2 : 4, bk = stage_k(bf16);
   FwdParams P;
   memset(&P, 0, sizeof(P));
   P.n_prob = n_prob; P.d = d;
@@ -514,31 +585,33 @@ int proj_fwd_tc_group(const llmrec_proj_fwd_problem* pr, int n_prob, int d, int 
   const int mb = pick_mb(d, tiles256), tm = tile_m(mb);
   int tiles = 0;
   for (int p = 0; p < n_prob; ++p) {
-    const float* wsrc = split ? pr[p].wsplit : pr[p].W;
-    LLMREC_CHECK_ARG(!split || pr[p].wsplit, "proj_fwd: 3xTF32 mode needs a wsplit buffer of 2*d*k floats");
+    const float* wsrc = need_ws ? pr[p].wsplit : pr[p].W;
+    LLMREC_CHECK_ARG(!need_ws || pr[p].wsplit, "proj_fwd: 3xTF32 mode and bf16 X need a wsplit buffer of 2*d*k floats");
     bool fresh = true;
     for (int q = 0; q < p; ++q) fresh = fresh && !(pr[q].W == pr[p].W && pr[q].wsplit == pr[p].wsplit);
-    if (split && fresh) {
+    if (need_ws && fresh) {
       WS.W[n_ws] = pr[p].W; WS.out[n_ws] = pr[p].wsplit; WS.n[n_ws] = (long long)d * pr[p].k;
       ws_max = WS.n[n_ws] > ws_max ? WS.n[n_ws] : ws_max;
       ++n_ws;
     }
     // an empty problem has no tiles (and a tensor map cannot have an empty dimension); its W is still split when a later problem shares it
     if (pr[p].n > 0) {
-      if (!make_tmap_2d_f32(&P.tmA[p], pr[p].X, (uint64_t)pr[p].k, (uint64_t)pr[p].n, (uint64_t)pr[p].ldx * 4, BK, (uint32_t)tm)) return 4;
-      if (!make_tmap_2d_f32(&P.tmW[p], wsrc, (uint64_t)pr[p].k, (uint64_t)(split ? 2 * d : d), (uint64_t)pr[p].k * 4, BK, (uint32_t)d)) return 4;
+      const int pieces = split ? (bf16 ? 3 : 2) : 1;
+      if (!make_tmap_2d(&P.tmA[p], x_type(bf16), pr[p].X, (uint64_t)pr[p].k, (uint64_t)pr[p].n, (uint64_t)pr[p].ldx * es, bk, (uint32_t)tm)) return 4;
+      if (!make_tmap_2d(&P.tmW[p], x_type(bf16), wsrc, (uint64_t)pr[p].k, (uint64_t)(pieces * d), (uint64_t)pr[p].k * es, bk, (uint32_t)d)) return 4;
     }
-    P.prob[p].n = (int)pr[p].n; P.prob[p].k = pr[p].k; P.prob[p].kblocks = (pr[p].k + BK - 1) / BK;
+    P.prob[p].n = (int)pr[p].n; P.prob[p].k = pr[p].k; P.prob[p].kblocks = (pr[p].k + bk - 1) / bk;
     P.prob[p].tile_start = tiles; P.prob[p].ldy = pr[p].ldy; P.prob[p].Y = pr[p].Y; P.prob[p].bias = pr[p].bias;
     tiles += (int)((pr[p].n + tm - 1) / tm);
   }
   P.total_tiles = tiles;
   if (n_ws > 0) {
-    wsplit_kernel<<<dim3((unsigned)((ws_max + 255) / 256), n_ws), 256, 0, st>>>(WS);
+    if (bf16) wsplit_bf16_kernel<<<dim3((unsigned)((ws_max + 255) / 256), n_ws), 256, 0, st>>>(WS, split ? 1 : 0);
+    else wsplit_kernel<<<dim3((unsigned)((ws_max + 255) / 256), n_ws), 256, 0, st>>>(WS);
     LLMREC_CHECK_LAUNCH("wsplit");
   }
   if (tiles <= 0) return 0;
-  return fwd_launch(P, split, mb, st);
+  return fwd_launch(P, split, mb, bf16, st);
 }
 
 static int wg_rows_per_chunk(int64_t n) {
@@ -549,8 +622,9 @@ static int wg_rows_per_chunk(int64_t n) {
 
 // Work plan of a grouped weight gradient, shared by the scratch query and the launch.  Scratch layout (floats):
 //   [colsum ticket: 4] [partials: items x tm x d] [colsum partials: n_prob x kColsumSlices x d] [per problem dY^T hi, lo: 2 x d x ldt]
+// (bf16 X: the three bf16 terms of dY^T, 3 x d x ldt bf16, in the same 2 x d x ldt floats)
 struct WgPlan { WgProblem prob[kMaxProb]; int items, mb, tm; int64_t ldt[kMaxProb], dyt[kMaxProb], colsum, total; };
-static void wg_plan(const llmrec_proj_wgrad_problem* pr, int n_prob, int d, WgPlan& W) {
+static void wg_plan(const llmrec_proj_wgrad_problem* pr, int n_prob, int d, bool bf16, WgPlan& W) {
   long long items256 = 0;
   for (int p = 0; p < n_prob; ++p) {
     const int rpc = wg_rows_per_chunk(pr[p].n);
@@ -569,23 +643,26 @@ static void wg_plan(const llmrec_proj_wgrad_problem* pr, int n_prob, int d, WgPl
   W.colsum = 4 + (int64_t)W.items * W.tm * d;
   int64_t off = W.colsum + (int64_t)n_prob * kColsumSlices * d;
   for (int p = 0; p < n_prob; ++p) {
-    W.ldt[p] = (pr[p].n + 3) & ~int64_t(3);   // TMA row pitch: a multiple of 16 bytes
+    W.ldt[p] = bf16 ? (pr[p].n + 7) & ~int64_t(7) : (pr[p].n + 3) & ~int64_t(3);   // TMA row pitch: a multiple of 16 bytes
     W.dyt[p] = off;
     off += 2 * (int64_t)d * W.ldt[p];
   }
   W.total = off;
 }
 
-int64_t proj_wgrad_tc_scratch(const llmrec_proj_wgrad_problem* pr, int n_prob, int d) {
+int64_t proj_wgrad_tc_scratch(const llmrec_proj_wgrad_problem* pr, int n_prob, int d, bool bf16) {
   WgPlan W;
-  wg_plan(pr, n_prob, d, W);
+  wg_plan(pr, n_prob, d, bf16, W);
   return W.total;   // the colsum ticket must start at zero; the kernel re-zeroes it
 }
 
-int proj_wgrad_tc_group(const llmrec_proj_wgrad_problem* pr, int n_prob, int d, int mode, float* scratch, int64_t scratch_elems, cudaStream_t st) {
+// bf16: pr[p].X holds the address of a bf16 table (llmrec_proj_wgrad_problem_bf16 carried in the fp32 struct's layout)
+int proj_wgrad_tc_group(const llmrec_proj_wgrad_problem* pr, int n_prob, int d, int mode, bool bf16, float* scratch, int64_t scratch_elems,
+                        cudaStream_t st) {
   const bool split = (mode == 0);
+  const int es = bf16 ? 2 : 4, bk = stage_k(bf16), pieces = split ? (bf16 ? 3 : 2) : 1;
   WgPlan W;
-  wg_plan(pr, n_prob, d, W);
+  wg_plan(pr, n_prob, d, bf16, W);
   LLMREC_CHECK_ARG(scratch && scratch_elems >= W.total, "proj_wgrad: scratch too small (%lld < %lld)", (long long)scratch_elems, (long long)W.total);
   WgParams P;
   memset(&P, 0, sizeof(P));
@@ -605,8 +682,8 @@ int proj_wgrad_tc_group(const llmrec_proj_wgrad_problem* pr, int n_prob, int d, 
     // an empty problem has no work items (and a tensor map cannot have an empty dimension); colsum and the reduce still
     // write its dW / db: zeros, or the prior under accumulate
     if (pr[p].n > 0) {
-      if (!make_tmap_2d_f32(&P.tmX[p], pr[p].X, (uint64_t)pr[p].k, (uint64_t)pr[p].n, (uint64_t)pr[p].ldx * 4, BK, BK)) return 4;
-      if (!make_tmap_2d_f32(&P.tmG[p], dyt, (uint64_t)pr[p].n, (uint64_t)(split ? 2 * d : d), (uint64_t)W.ldt[p] * 4, BK, (uint32_t)d)) return 4;
+      if (!make_tmap_2d(&P.tmX[p], x_type(bf16), pr[p].X, (uint64_t)pr[p].k, (uint64_t)pr[p].n, (uint64_t)pr[p].ldx * es, bk, bk)) return 4;
+      if (!make_tmap_2d(&P.tmG[p], x_type(bf16), dyt, (uint64_t)pr[p].n, (uint64_t)(pieces * d), (uint64_t)W.ldt[p] * es, bk, (uint32_t)d)) return 4;
     }
     T.dY[p] = pr[p].dY; T.ld[p] = pr[p].lddy; T.n[p] = (int)pr[p].n; T.out[p] = dyt; T.ldt[p] = W.ldt[p];
     n_max = pr[p].n > n_max ? pr[p].n : n_max;
@@ -644,9 +721,11 @@ int proj_wgrad_tc_group(const llmrec_proj_wgrad_problem* pr, int n_prob, int d, 
     if (forked) LLMREC_CHECK_CUDA(cudaEventRecord(ev_join, side));
   }
   if (W.items > 0) {   // no items: every problem is empty, and only colsum and the reduce run
-    dyt_split_kernel<<<dim3((unsigned)((n_max + 31) / 32), (unsigned)(d / 32), (unsigned)n_prob), 256, 0, st>>>(T);
+    const dim3 grid((unsigned)((n_max + 31) / 32), (unsigned)(d / 32), (unsigned)n_prob);
+    if (bf16) dyt_split_kernel<true><<<grid, 256, 0, st>>>(T);
+    else dyt_split_kernel<false><<<grid, 256, 0, st>>>(T);
     LLMREC_CHECK_LAUNCH("dyt_split");
-    int rc = wgrad_launch(P, split, W.mb, st);
+    int rc = wgrad_launch(P, split, W.mb, bf16, st);
     if (rc) return rc;
   }
   ReduceParams R;

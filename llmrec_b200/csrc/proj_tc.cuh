@@ -5,22 +5,26 @@
 namespace llmrec {
 
 constexpr int kMaxProb = 8;
-constexpr int BK = 32;  // k (fwd) / rows (wgrad) per pipeline stage: fp32 per 128-byte swizzle row
+constexpr int BK = 32;    // k (fwd) / rows (wgrad) per pipeline stage: fp32 per 128-byte swizzle row
+constexpr int BK16 = 64;  // the same for bf16 X: 64 elements per 128-byte swizzle row
+constexpr int stage_k(bool bf16) { return bf16 ? BK16 : BK; }
 // Tile = 2 consumer warpgroups x MB blocks of wgmma M = 64: 256 rows (fwd) / features (wgrad) when MB = 2, 128 when MB = 1.
 constexpr int tile_m(int mb) { return 128 * mb; }
 
 struct FwdProblem { int n, k, kblocks, tile_start; long long ldy; float* Y; const float* bias; };
 struct FwdParams {
-  CUtensorMap tmA[kMaxProb];  // X [n x k], boxes [TM rows][32 k], 128-byte swizzle
-  CUtensorMap tmW[kMaxProb];  // [2d x k] (hi rows then lo rows) when SPLIT, [d x k] otherwise; boxes [d][32 k]
+  CUtensorMap tmA[kMaxProb];  // X [n x k], boxes [TM rows][32 k] (bf16: [TM rows][64 k]), 128-byte swizzle
+  CUtensorMap tmW[kMaxProb];  // fp32: [2d x k] (hi rows then lo rows) when SPLIT, [d x k] otherwise; boxes [d][32 k]
+                              // bf16: [3d x k] (w0, w1, w2 rows) when SPLIT, [d x k] (w0) otherwise; boxes [d][64 k]
   FwdProblem prob[kMaxProb];
   int n_prob, total_tiles, d;
 };
 
 struct WgProblem { int n, k, ft_tiles, chunks, rows_per_chunk, item_start; };
 struct WgParams {
-  CUtensorMap tmX[kMaxProb];  // X [n x k], boxes [32 rows][32 features], 128-byte swizzle
+  CUtensorMap tmX[kMaxProb];  // X [n x k], boxes [32 rows][32 features] (bf16: [64 rows][64 features]), 128-byte swizzle
   CUtensorMap tmG[kMaxProb];  // dY^T [2d x n] (hi rows then lo rows) when SPLIT, [d x n] otherwise; boxes [d][32 rows]
+                              // bf16: [3d x n] (three bf16 terms) when SPLIT, [d x n] otherwise; boxes [d][64 rows]
   WgProblem prob[kMaxProb];
   int n_prob, total_items, d;
   float* partial;  // [total_items][TM][d]

@@ -55,12 +55,13 @@ class HoistedHotPath(HotPath):
         self.Kc = Kc
         TU = torch.zeros(self.nu, Kc, dtype=torch.float32, device=dev)
         TI = torch.zeros(self.ni, Kc, dtype=torch.float32, device=dev)
+        # bf16 feature tables (--feat_dtype bf16) are widened to fp32 one table at a time for these one-time products; TU / TI stay fp32
         for j, X in enumerate(raw[:-1]):                          # item-side raw tables: TU_s = ui.X, TI_s = iu.TU_s
             c0, w = self.col0[j], widths[j]
-            self.ui.apply([(X, TU[:, c0:c0 + w], None, False)])
+            self.ui.apply([(X.float(), TU[:, c0:c0 + w], None, False)])
             self.iu.apply([(TU[:, c0:c0 + w], TI[:, c0:c0 + w], None, False)])
         c0, w = self.col0[-2], widths[-1]                          # user table: TI_usr = iu.X_usr (prof_i), TU_usr = ui.TI_usr (prof_u)
-        self.iu.apply([(raw[-1], TI[:, c0:c0 + w], None, False)])
+        self.iu.apply([(raw[-1].float(), TI[:, c0:c0 + w], None, False)])
         self.ui.apply([(TI[:, c0:c0 + w], TU[:, c0:c0 + w], None, False)])
         sc = self.col0[-1]
         TU[:, sc] = gs["cu"]; TU[:, sc + 1] = gs["ru"]             # Fu bias scale, prof_u bias scale

@@ -68,6 +68,9 @@ class Trainer(object):
         args = self.args = get_args()
         if not torch.cuda.is_available():
             raise RuntimeError("llmrec_b200.Trainer needs a CUDA (H100) device: there is no CPU fallback")
+        if getattr(args, "feat_dtype", "fp32") == "bf16" and (args.mask or args.mask_rate > 0):
+            raise ValueError("--feat_dtype bf16 cannot be combined with --mask / --mask_rate > 0: the mask branch overwrites rows of the "
+                             "feature tables with fp32 column means in place (Trainer._mask_features); use --feat_dtype fp32")
         self.device = torch.device(device)
         self.task_name = "%s_%s_%s" % (datetime.now().strftime("%Y-%m-%d %H:%M:%S"), args.dataset, args.cf_model)
         self.logger = Logger(filename=self.task_name, is_debug=args.debug)

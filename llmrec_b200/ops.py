@@ -222,19 +222,49 @@ def _get_scratch(key, n, device, zero=False):
     return t
 
 
+FEAT_DTYPES = (torch.float32, torch.bfloat16)     # element types of the side-feature table X the projections accept
+
+
+def _feat(X, name="X"):
+    """X of a projection: a CUDA fp32 or bf16 row-major 2-D tensor (column slices fine)."""
+    if X.dim() != 2 or X.dtype not in FEAT_DTYPES or not X.is_cuda or (X.shape[1] > 1 and X.stride(1) != 1):
+        raise ValueError(f"{name}: need a CUDA fp32 or bf16 row-major 2-D tensor, got {tuple(X.shape)} {X.dtype} {X.device} strides {X.stride()}")
+    return X
+
+
+def _group_dtype(Xs, what):
+    """The one X dtype of a grouped call: a bf16 group runs the _bf16 entry points, and one call never mixes the two."""
+    dt = {X.dtype for X in Xs}
+    if len(dt) != 1:
+        raise ValueError(f"{what}: every problem of one call must share the X dtype, got {sorted(str(t) for t in dt)}")
+    return dt.pop()
+
+
+def _f32(t, name):
+    if t is not None and t.dtype != torch.float32:
+        raise ValueError(f"{name}: must be fp32 (only the feature table X may be bf16), got {t.dtype}")
+    return t
+
+
 def proj_fwd_group(problems, d, mode=0):
     """problems: list of (X[n x k], W[d x k], bias[d]|None, out[n x d]).  One grouped launch (wgmma) --
-    the 8 nn.Linear calls of Models.py:145-150.  Problems sharing W share the hi/lo split buffer."""
-    arr = (N.ProjFwdProblem * len(problems))()
+    the 8 nn.Linear calls of Models.py:145-150.  Problems sharing W share the split buffer.  X is fp32 or bf16 (all problems
+    alike); W, bias and out are fp32."""
+    bf16 = _group_dtype([_feat(X) for X, _, _, _ in problems], "proj_fwd") == torch.bfloat16
+    arr = ((N.ProjFwdProblemBf16 if bf16 else N.ProjFwdProblem) * len(problems))()
     for i, (X, W, b, out) in enumerate(problems):
-        _mat(out)
-        n, k = _mat(X).shape
+        _mat(out); _f32(W, "proj_fwd W"); _f32(b, "proj_fwd bias")
+        n, k = X.shape
         if not W.is_contiguous() or tuple(W.shape) != (d, k) or tuple(out.shape) != (n, d):
             raise ValueError("proj_fwd: bad shapes")
-        ws = _get_scratch(("wsplit", W.data_ptr()), 2 * d * k, X.device) if mode == 0 else None
-        arr[i] = N.ProjFwdProblem(_p(X), _p(W), _p(b), _p(out), _p(ws), _ld(X), _ld(out), n, k, 0)
-    N.check(N.lib().llmrec_proj_fwd_group_f32(arr, len(problems), d, mode, _stream()), "proj_fwd_group")
-    _count((2 if mode == 0 else 1) * -(-len(problems) // 8))
+        # the bf16 kernels read W as bf16 terms in modes 0 and 1: 3dk (or dk) bf16 in the 2dk floats of the fp32 hi/lo split
+        ws = _get_scratch(("wsplit", W.data_ptr()), 2 * d * k, X.device) if mode == 0 or (bf16 and mode == 1) else None
+        arr[i] = (N.ProjFwdProblemBf16 if bf16 else N.ProjFwdProblem)(_p(X), _p(W), _p(b), _p(out), _p(ws), _ld(X), _ld(out), n, k, 0)
+    if bf16:
+        N.check(N.lib().llmrec_proj_fwd_group_bf16(arr, len(problems), d, mode, _stream()), "proj_fwd_group_bf16")
+    else:
+        N.check(N.lib().llmrec_proj_fwd_group_f32(arr, len(problems), d, mode, _stream()), "proj_fwd_group")
+    _count((2 if mode == 0 or (bf16 and mode == 1) else 1) * -(-len(problems) // 8))
 
 
 def proj_fwd(X, W, b, out, mode=0):
@@ -244,17 +274,23 @@ def proj_fwd(X, W, b, out, mode=0):
 
 
 def proj_wgrad_group(problems, d, mode=0):
-    """problems: list of (X[n x k], dY[n x d], dW[d x k], db[d]|None, accumulate).  dW (+)= dY^T X ; db (+)= colsum(dY)."""
-    arr = (N.ProjWgradProblem * len(problems))()
+    """problems: list of (X[n x k], dY[n x d], dW[d x k], db[d]|None, accumulate).  dW (+)= dY^T X ; db (+)= colsum(dY).
+    X is fp32 or bf16 (all problems alike); dY, dW and db are fp32."""
+    bf16 = _group_dtype([_feat(X) for X, _, _, _, _ in problems], "proj_wgrad") == torch.bfloat16
+    arr = ((N.ProjWgradProblemBf16 if bf16 else N.ProjWgradProblem) * len(problems))()
     for i, (X, dY, dW, db, acc) in enumerate(problems):
-        _mat(dY)
-        n, k = _mat(X).shape
+        _mat(dY); _f32(dW, "proj_wgrad dW"); _f32(db, "proj_wgrad db")
+        n, k = X.shape
         if not dW.is_contiguous() or tuple(dW.shape) != (d, k) or tuple(dY.shape) != (n, d):
             raise ValueError("proj_wgrad: bad shapes")
-        arr[i] = N.ProjWgradProblem(_p(X), _p(dY), _p(dW), _p(db), _ld(X), _ld(dY), n, k, 1 if acc else 0)
-    need = int(N.lib().llmrec_proj_wgrad_group_scratch(arr, len(problems), d, mode))
+        arr[i] = (N.ProjWgradProblemBf16 if bf16 else N.ProjWgradProblem)(_p(X), _p(dY), _p(dW), _p(db), _ld(X), _ld(dY), n, k, 1 if acc else 0)
+    lib = N.lib()
+    need = int((lib.llmrec_proj_wgrad_group_bf16_scratch if bf16 else lib.llmrec_proj_wgrad_group_scratch)(arr, len(problems), d, mode))
     scratch = _get_scratch(("wgrad", problems[0][0].device.index), need, problems[0][0].device, zero=True) if need else None     # holds a ticket word
-    N.check(N.lib().llmrec_proj_wgrad_group_f32(arr, len(problems), d, mode, _p(scratch), need, _stream()), "proj_wgrad_group")
+    if bf16:
+        N.check(lib.llmrec_proj_wgrad_group_bf16(arr, len(problems), d, mode, _p(scratch), need, _stream()), "proj_wgrad_group_bf16")
+    else:
+        N.check(lib.llmrec_proj_wgrad_group_f32(arr, len(problems), d, mode, _p(scratch), need, _stream()), "proj_wgrad_group")
     _count(4 if need else len(problems))
 
 

@@ -21,8 +21,9 @@ def spmm_bytes(nnz, M, N, d, segs=1):
     return 4 * nnz + 4 * (M + 1) + 4 * M + segs * (4 * d * N + 4 * d * M)
 
 
-def proj_bytes(n, k, d):
-    return 4 * n * k + 4 * k * d + 4 * n * d
+def proj_bytes(n, k, d, x_bytes=4):
+    """Y[n x d] = X[n x k] W^T (or its weight gradient): X read once at x_bytes per element (4 fp32, 2 bf16), fp32 W and Y."""
+    return x_bytes * n * k + 4 * k * d + 4 * n * d
 
 
 def step_bytes(hp, nnz):
@@ -32,7 +33,8 @@ def step_bytes(hp, nnz):
     if hp.has_feats:
         f = hp.feats
         gemms = [(ni, f["image"].shape[1]), (ni, f["text"].shape[1])] + [(ni, v.shape[1]) for v in f["item"].values()] + [(nu, f["user"].shape[1])]
-        out["proj_fwd"] = out["proj_wgrad"] = sum(proj_bytes(n, k, d) for n, k in gemms)
+        xb = f["image"].element_size()
+        out["proj_fwd"] = out["proj_wgrad"] = sum(proj_bytes(n, k, d, xb) for n, k in gemms)
     sp = lambda M, N, segs: spmm_bytes(nnz, M, N, d, segs)
     out["spmm_fwd"] = sp(nu, ni, S + 1) + sp(ni, nu, S + 2) + sp(nu, ni, 2) + (sp(ni, nu, 1) if L >= 2 else 0)
     out["spmm_bwd"] = sp(ni, nu, 1) + sp(nu, ni, S + 2) + sp(ni, nu, S + 1) + (sp(nu, ni, 1) + sp(ni, nu, 1) if L >= 2 else 0)

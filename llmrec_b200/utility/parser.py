@@ -79,6 +79,10 @@ _EXTRA = [
                                                    "batch's rows per step (SURVEY.md 8f-3); same results within the golden tolerances; off automatically "
                                                    "when drop_rate > 0 or the mask branch is on")),
     ("device_sampler", dict(type=int, default=0, help="1: draw the batches on the GPU (non-parity RNG stream, SURVEY.md 8f-1); 0 replays the reference's host sampling")),
+    ("feat_dtype", dict(default="fp32", choices=["fp32", "bf16"], help="element type the side-feature tables (image, text, user profile, "
+                                                                      "attributes) are kept in: bf16 rounds them once (round-to-nearest-even) "
+                                                                      "when the model is built and halves their memory and projection reads; "
+                                                                      "the projections are then exact on the rounded tables. Not with the mask branch")),
 ]
 
 DATASET_ALIASES = {"netflix": "netflix_valid_item", "movielens": "preprocessed_raw_MovieLens", "movieLens": "preprocessed_raw_MovieLens"}
