@@ -1,5 +1,6 @@
 """Host-side SpMM tile planner (llmrec_spmm_plan_tiles): every row is covered exactly once, nnz bounds hold."""
 import numpy as np
+import pytest
 
 from llmrec_b200 import _native as N
 
@@ -47,3 +48,36 @@ def test_plan_covers_rows_once():
         for j, r in enumerate(srow):
             pcs = tiles[sfirst[j]:sfirst[j + 1], :4]
             assert (pcs[:, 0] == r).all() and pcs[0, 2] == rp[r] and pcs[-1, 3] == rp[r + 1]
+
+
+@pytest.mark.parametrize("max_rows", (1, 7, 15))
+@pytest.mark.parametrize("tile", (8, 248))
+def test_plan_at_the_boundaries(tile, max_rows):
+    """The boundary graphs of the kernel exactness tests: a row of exactly tile_nnz entries stays whole, one of tile_nnz + 1 is cut
+    into exactly 2 pieces (k * tile_nnz into k); groups hold at most max_rows rows, and their row-end bytes are the row ends."""
+    from test_spmm_exactness_gpu import boundary_degrees
+    deg = boundary_degrees(tile)
+    rp = np.concatenate([[0], np.cumsum(deg)])
+    tiles, srow, sfirst, counts = _plan(rp, tile, max_rows)
+    whole = {}
+    for i, (r0, nr, e0, e1) in enumerate(tiles[:, :4]):
+        deltas = tiles[i, 4:].view(np.uint8)
+        if nr:
+            assert nr <= max_rows and e1 - e0 <= tile and e0 == rp[r0] and e1 == rp[r0 + nr]
+            assert (e0 + deltas[:nr].astype(np.int64) == rp[r0 + 1:r0 + nr + 1]).all() and (deltas[nr:] == 0).all()
+            for r in range(r0, r0 + nr):
+                whole[r] = whole.get(r, 0) + 1
+        else:
+            j = int(np.searchsorted(srow, r0))
+            assert srow[j] == r0 and tuple(deltas.view(np.int32)[:3]) == (j, sfirst[j], sfirst[j + 1] - sfirst[j])
+    pieces = dict(zip(srow.tolist(), np.diff(sfirst).tolist()))
+    assert set(whole) | set(pieces) == set(range(len(deg))) and not set(whole) & set(pieces)
+    assert all(v == 1 for v in whole.values())
+    for r, dg in enumerate(deg):
+        if dg <= tile:
+            assert r in whole, (r, dg)
+        else:
+            assert pieces[r] == -(-dg // tile), (r, dg)
+            if dg == tile + 1:
+                assert pieces[r] == 2
+    assert {tile, tile + 1, 2 * tile, 3 * tile} <= set(deg.tolist())
