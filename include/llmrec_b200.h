@@ -101,6 +101,8 @@ int llmrec_row_softmax_bwd_rows_f32(const float* S, int64_t lds, const float* dS
 /* Device-side row sets: mask |= {col[e] : e in rows list[.] of the CSR}, mask |= {ids}, and mask -> (unordered) id list with *count += #bits. */
 int llmrec_mark_neighbors(const int32_t* rowptr, const int32_t* col, const int32_t* list, int32_t n_list, uint32_t* mask, llmrec_stream_t stream);
 int llmrec_mark_ids(const int32_t* ids, int32_t n, uint32_t* mask, llmrec_stream_t stream);
+/* mask |= {ids[0 .. min(*n_dev, max_n))}: the live length is read from device memory (a captured step's B', the first word of its meta row). */
+int llmrec_mark_ids_rows(const int32_t* ids, const int32_t* n_dev, int32_t max_n, uint32_t* mask, llmrec_stream_t stream);
 int llmrec_compact_mask(const uint32_t* mask, int32_t n_bits, int32_t* list_out, int32_t* count, llmrec_stream_t stream);
 int llmrec_zero_rows_f32(float* Y, int64_t ldy, const int32_t* idx, int32_t n, int32_t d, llmrec_stream_t stream);
 int llmrec_assign_rows_f32(const float* G, int64_t ldg, const int32_t* idx, int32_t n, int32_t d, float* Y, int64_t ldy, llmrec_stream_t stream);
@@ -198,6 +200,18 @@ int llmrec_fuse_bwd_f32(const float* g, int64_t ldg, int32_t n_layers, float* d_
                         const float* const* sides_host, const int64_t* ld_sides_host, const float* coef_host,
                         float* const* d_sides_host, const int64_t* ld_dsides_host, int32_t n_sides,
                         int32_t accumulate, const int32_t* rows, int64_t n, int32_t d, llmrec_stream_t stream);
+/* Row-LIST forms with a device-side length: only rows[0 .. min(*n_rows_dev, max_rows)) are processed (entries < 0 skipped), each by the
+ * same per-row code as the full form, so a listed row gets the same bits; every other row of out / d_layer / d_sides is left untouched.
+ * The grid is sized for max_rows, no host synchronisation.  The training step fuses only its batch's rows with these (the loss reads
+ * U / I there only, and the fused-output gradient is zero elsewhere); a row listed twice would be accumulated twice by the backward. */
+int llmrec_fuse_fwd_rows_f32(const float* const* layers_host, const int64_t* ld_layers_host, int32_t n_layers,
+                             const float* const* sides_host, const int64_t* ld_sides_host, const float* coef_host,
+                             int32_t n_sides, float* out, int64_t ldo, const int32_t* rows, const int32_t* n_rows_dev, int32_t max_rows,
+                             int32_t d, llmrec_stream_t stream);
+int llmrec_fuse_bwd_rows_f32(const float* g, int64_t ldg, int32_t n_layers, float* d_layer, int64_t lddl,
+                             const float* const* sides_host, const int64_t* ld_sides_host, const float* coef_host,
+                             float* const* d_sides_host, const int64_t* ld_dsides_host, int32_t n_sides, int32_t accumulate,
+                             const int32_t* rows, const int32_t* n_rows_dev, int32_t max_rows, int32_t d, llmrec_stream_t stream);
 
 /* ---------------------------------------------------------------------------------------------
  * BPR + prune heads (main.py:330-342 bpr_loss, :158-165 prune_loss, :232-254 the 8 heads).

@@ -79,6 +79,7 @@ SIGNATURES = {
     "llmrec_row_softmax_bwd_rows_f32": (C.c_int, [c_f32p, C.c_int64, c_f32p, C.c_int64, c_f32p, C.c_int64, c_i32p, c_i32p, C.c_int32, C.c_int32, c_stream]),
     "llmrec_mark_neighbors": (C.c_int, [c_i32p, c_i32p, c_i32p, C.c_int32, C.c_void_p, c_stream]),
     "llmrec_mark_ids": (C.c_int, [c_i32p, C.c_int32, C.c_void_p, c_stream]),
+    "llmrec_mark_ids_rows": (C.c_int, [c_i32p, c_i32p, C.c_int32, C.c_void_p, c_stream]),
     "llmrec_compact_mask": (C.c_int, [C.c_void_p, C.c_int32, c_i32p, c_i32p, c_stream]),
     "llmrec_zero_rows_f32": (C.c_int, [c_f32p, C.c_int64, c_i32p, C.c_int32, C.c_int32, c_stream]),
     "llmrec_assign_rows_f32": (C.c_int, [c_f32p, C.c_int64, c_i32p, C.c_int32, C.c_int32, c_f32p, C.c_int64, c_stream]),
@@ -100,6 +101,11 @@ SIGNATURES = {
     "llmrec_fuse_bwd_f32": (C.c_int, [c_f32p, C.c_int64, C.c_int32, c_f32p, C.c_int64, C.POINTER(C.c_void_p), C.POINTER(C.c_int64),
                                       C.POINTER(C.c_float), C.POINTER(C.c_void_p), C.POINTER(C.c_int64), C.c_int32, C.c_int32,
                                       c_i32p, C.c_int64, C.c_int32, c_stream]),
+    "llmrec_fuse_fwd_rows_f32": (C.c_int, [C.POINTER(C.c_void_p), C.POINTER(C.c_int64), C.c_int32, C.POINTER(C.c_void_p), C.POINTER(C.c_int64),
+                                           C.POINTER(C.c_float), C.c_int32, c_f32p, C.c_int64, c_i32p, c_i32p, C.c_int32, C.c_int32, c_stream]),
+    "llmrec_fuse_bwd_rows_f32": (C.c_int, [c_f32p, C.c_int64, C.c_int32, c_f32p, C.c_int64, C.POINTER(C.c_void_p), C.POINTER(C.c_int64),
+                                           C.POINTER(C.c_float), C.POINTER(C.c_void_p), C.POINTER(C.c_int64), C.c_int32, C.c_int32,
+                                           c_i32p, c_i32p, C.c_int32, C.c_int32, c_stream]),
     "llmrec_grad_init_f32": (C.c_int, [C.POINTER(GradRegion), C.c_int32, c_f32p, c_f32p, c_stream]),
     "llmrec_grad_init_scratch": (C.c_int64, []),
     "llmrec_bpr_heads_f32": (C.c_int, [C.POINTER(BprHead), C.c_int32, c_i32p, c_i32p, c_i32p, C.c_int32, C.c_int32, c_i32p, C.c_float,

@@ -18,7 +18,15 @@ struct FuseParams {
   const float* g; int64_t ldg;       // bwd only
   const int* rows; int64_t n; int d; int accumulate;
   int compact;                       // fwd only: layers are read at rows[item], sides and out at the compact position `item`
+  const int* n_dev;                  // row-list form with a device-side length: items [0, min(*n_dev, n)) of `rows`; the grid covers n
 };
+
+// Number of rows of this launch: n, or the device-side list length capped at n (the grid is sized for n).
+__device__ __forceinline__ int64_t live_rows(const FuseParams& p) {
+  if (!p.n_dev) return p.n;
+  const int64_t c = __ldg(p.n_dev);
+  return c < p.n ? c : p.n;
+}
 
 template <int LPR>
 __device__ __forceinline__ float grp_sum(float v) {
@@ -33,7 +41,7 @@ __global__ void __launch_bounds__(256) fuse_fwd_kernel(const FuseParams p) {
   __shared__ float sc[8][RPW][kMaxSides];
   const int wib = threadIdx.x >> 5, lane = threadIdx.x & 31, sub = lane / LPR, li = lane % LPR;
   const int64_t item = ((int64_t)blockIdx.x * 8 + wib) * RPW + sub;
-  const bool in_range = item < p.n;
+  const bool in_range = item < live_rows(p);
   const int64_t lrow = in_range ? (p.rows ? (int64_t)p.rows[item] : item) : 0;
   const bool valid = in_range && lrow >= 0;          // a negative list entry = "not mine": compact output row of zeros, nothing read
   const int64_t row = valid ? lrow : 0;
@@ -88,7 +96,7 @@ __global__ void __launch_bounds__(256) fuse_bwd_kernel(const FuseParams p) {
   __shared__ float sb[8][RPW][kMaxSides];
   const int wib = threadIdx.x >> 5, lane = threadIdx.x & 31, sub = lane / LPR, li = lane % LPR;
   const int64_t item = ((int64_t)blockIdx.x * 8 + wib) * RPW + sub;
-  const bool valid = item < p.n;
+  const bool valid = item < live_rows(p);
   const int64_t row = valid ? (p.rows ? (int64_t)p.rows[item] : item) : 0;
   const int nq = VEC ? p.d / 4 : p.d;
   const float* g = p.g + row * p.ldg;
@@ -157,14 +165,10 @@ static int launch_fuse(const FuseParams& p, bool vec, cudaStream_t st) {
   LLMREC_CHECK_LAUNCH(BWD ? "fuse_bwd" : "fuse_fwd");
   return 0;
 }
-}  // namespace llmrec
 
-using namespace llmrec;
-
-extern "C" int llmrec_fuse_fwd_f32(const float* const* layers, const int64_t* ld_layers, int32_t n_layers,
-                                   const float* const* sides, const int64_t* ld_sides, const float* coef,
-                                   int32_t n_sides, float* out, int64_t ldo, const int32_t* rows, int64_t n, int32_t d,
-                                   llmrec_stream_t stream) {
+static int fuse_fwd(const float* const* layers, const int64_t* ld_layers, int32_t n_layers, const float* const* sides,
+                    const int64_t* ld_sides, const float* coef, int32_t n_sides, float* out, int64_t ldo, const int32_t* rows,
+                    const int32_t* n_dev, int64_t n, int32_t d, cudaStream_t st) {
   LLMREC_REQUIRE_DEVICE();
   LLMREC_CHECK_ARG(n_layers >= 1 && n_layers <= kMaxLayers && n_sides >= 0 && n_sides <= kMaxSides,
                    "fuse_fwd: n_layers=%d n_sides=%d out of range", n_layers, n_sides);
@@ -173,15 +177,14 @@ extern "C" int llmrec_fuse_fwd_f32(const float* const* layers, const int64_t* ld
   p.n_layers = n_layers; p.n_sides = n_sides;
   for (int l = 0; l < n_layers; ++l) { p.layers[l] = layers[l]; p.ld_layers[l] = ld_layers[l]; vec = vec && aligned16(layers[l]) && ld_layers[l] % 4 == 0; }
   for (int t = 0; t < n_sides; ++t) { p.sides[t] = sides[t]; p.ld_sides[t] = ld_sides[t]; p.coef[t] = coef[t]; vec = vec && aligned16(sides[t]) && ld_sides[t] % 4 == 0; }
-  p.out = out; p.ldo = ldo; p.rows = rows; p.n = n < 0 ? -n : n; p.d = d;
+  p.out = out; p.ldo = ldo; p.rows = rows; p.n = n < 0 ? -n : n; p.d = d; p.n_dev = n_dev;
   p.compact = (n < 0 && rows) ? 1 : 0;
-  return launch_fuse<false>(p, vec, as_stream(stream));
+  return launch_fuse<false>(p, vec, st);
 }
 
-extern "C" int llmrec_fuse_bwd_f32(const float* g, int64_t ldg, int32_t n_layers, float* d_layer, int64_t lddl,
-                                   const float* const* sides, const int64_t* ld_sides, const float* coef,
-                                   float* const* d_sides, const int64_t* ld_dsides, int32_t n_sides,
-                                   int32_t accumulate, const int32_t* rows, int64_t n, int32_t d, llmrec_stream_t stream) {
+static int fuse_bwd(const float* g, int64_t ldg, int32_t n_layers, float* d_layer, int64_t lddl, const float* const* sides,
+                    const int64_t* ld_sides, const float* coef, float* const* d_sides, const int64_t* ld_dsides, int32_t n_sides,
+                    int32_t accumulate, const int32_t* rows, const int32_t* n_dev, int64_t n, int32_t d, cudaStream_t st) {
   LLMREC_REQUIRE_DEVICE();
   LLMREC_CHECK_ARG(n_layers >= 1 && n_sides >= 0 && n_sides <= kMaxSides, "fuse_bwd: n_layers=%d n_sides=%d out of range", n_layers, n_sides);
   FuseParams p{};
@@ -192,6 +195,41 @@ extern "C" int llmrec_fuse_bwd_f32(const float* g, int64_t ldg, int32_t n_layers
     p.dsides[t] = d_sides[t]; p.ld_dsides[t] = ld_dsides[t];
     vec = vec && aligned16(sides[t]) && ld_sides[t] % 4 == 0 && (!d_sides[t] || (aligned16(d_sides[t]) && ld_dsides[t] % 4 == 0));
   }
-  p.out = d_layer; p.ldo = lddl; p.g = g; p.ldg = ldg; p.rows = rows; p.n = n; p.d = d; p.accumulate = accumulate;
-  return launch_fuse<true>(p, vec, as_stream(stream));
+  p.out = d_layer; p.ldo = lddl; p.g = g; p.ldg = ldg; p.rows = rows; p.n = n; p.d = d; p.accumulate = accumulate; p.n_dev = n_dev;
+  return launch_fuse<true>(p, vec, st);
+}
+}  // namespace llmrec
+
+using namespace llmrec;
+
+extern "C" int llmrec_fuse_fwd_f32(const float* const* layers, const int64_t* ld_layers, int32_t n_layers,
+                                   const float* const* sides, const int64_t* ld_sides, const float* coef,
+                                   int32_t n_sides, float* out, int64_t ldo, const int32_t* rows, int64_t n, int32_t d,
+                                   llmrec_stream_t stream) {
+  return fuse_fwd(layers, ld_layers, n_layers, sides, ld_sides, coef, n_sides, out, ldo, rows, nullptr, n, d, as_stream(stream));
+}
+
+extern "C" int llmrec_fuse_bwd_f32(const float* g, int64_t ldg, int32_t n_layers, float* d_layer, int64_t lddl,
+                                   const float* const* sides, const int64_t* ld_sides, const float* coef,
+                                   float* const* d_sides, const int64_t* ld_dsides, int32_t n_sides,
+                                   int32_t accumulate, const int32_t* rows, int64_t n, int32_t d, llmrec_stream_t stream) {
+  return fuse_bwd(g, ldg, n_layers, d_layer, lddl, sides, ld_sides, coef, d_sides, ld_dsides, n_sides, accumulate, rows, nullptr, n, d,
+                  as_stream(stream));
+}
+
+extern "C" int llmrec_fuse_fwd_rows_f32(const float* const* layers, const int64_t* ld_layers, int32_t n_layers,
+                                        const float* const* sides, const int64_t* ld_sides, const float* coef,
+                                        int32_t n_sides, float* out, int64_t ldo, const int32_t* rows, const int32_t* n_rows_dev,
+                                        int32_t max_rows, int32_t d, llmrec_stream_t stream) {
+  LLMREC_CHECK_ARG(rows && n_rows_dev && max_rows >= 0, "fuse_fwd_rows: a row list and its device-side length are required");
+  return fuse_fwd(layers, ld_layers, n_layers, sides, ld_sides, coef, n_sides, out, ldo, rows, n_rows_dev, max_rows, d, as_stream(stream));
+}
+
+extern "C" int llmrec_fuse_bwd_rows_f32(const float* g, int64_t ldg, int32_t n_layers, float* d_layer, int64_t lddl,
+                                        const float* const* sides, const int64_t* ld_sides, const float* coef,
+                                        float* const* d_sides, const int64_t* ld_dsides, int32_t n_sides, int32_t accumulate,
+                                        const int32_t* rows, const int32_t* n_rows_dev, int32_t max_rows, int32_t d, llmrec_stream_t stream) {
+  LLMREC_CHECK_ARG(rows && n_rows_dev && max_rows >= 0, "fuse_bwd_rows: a row list and its device-side length are required");
+  return fuse_bwd(g, ldg, n_layers, d_layer, lddl, sides, ld_sides, coef, d_sides, ld_dsides, n_sides, accumulate, rows, n_rows_dev, max_rows,
+                  d, as_stream(stream));
 }

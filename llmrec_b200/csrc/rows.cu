@@ -64,8 +64,10 @@ __global__ void __launch_bounds__(256) mark_neighbors_kernel(const int* __restri
     if (!(mask[v >> 5] & bit)) atomicOr(mask + (v >> 5), bit);
   }
 }
-__global__ void mark_ids_kernel(const int* __restrict__ ids, int n, unsigned* __restrict__ mask) {
+// ids[0 .. n) -- or ids[0 .. min(*n_dev, n)) when the live length is only known on the device (a captured step's B')
+__global__ void mark_ids_kernel(const int* __restrict__ ids, int n, const int* __restrict__ n_dev, unsigned* __restrict__ mask) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (n_dev) { const int c = __ldg(n_dev); n = c < n ? c : n; }
   if (i >= n) return;
   const int v = ids[i];
   if (v >= 0) atomicOr(mask + (v >> 5), 1u << (v & 31));
@@ -117,8 +119,16 @@ extern "C" int llmrec_mark_neighbors(const int32_t* rowptr, const int32_t* col, 
 extern "C" int llmrec_mark_ids(const int32_t* ids, int32_t n, uint32_t* mask, llmrec_stream_t stream) {
   LLMREC_REQUIRE_DEVICE();
   if (n <= 0) return 0;
-  mark_ids_kernel<<<(n + 255) / 256, 256, 0, as_stream(stream)>>>(ids, n, mask);
+  mark_ids_kernel<<<(n + 255) / 256, 256, 0, as_stream(stream)>>>(ids, n, nullptr, mask);
   LLMREC_CHECK_LAUNCH("mark_ids");
+  return 0;
+}
+extern "C" int llmrec_mark_ids_rows(const int32_t* ids, const int32_t* n_dev, int32_t max_n, uint32_t* mask, llmrec_stream_t stream) {
+  LLMREC_REQUIRE_DEVICE();
+  LLMREC_CHECK_ARG(n_dev, "mark_ids_rows: the device-side length is required");
+  if (max_n <= 0) return 0;
+  mark_ids_kernel<<<(max_n + 255) / 256, 256, 0, as_stream(stream)>>>(ids, max_n, n_dev, mask);
+  LLMREC_CHECK_LAUNCH("mark_ids_rows");
   return 0;
 }
 extern "C" int llmrec_compact_mask(const uint32_t* mask, int32_t n_bits, int32_t* list_out, int32_t* count, llmrec_stream_t stream) {

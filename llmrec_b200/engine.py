@@ -19,6 +19,16 @@ the ID layers beside the projection kernel and the side-feature products, the fi
 tail of the forward pass, user- and item-side fusion side by side, the ID backward chain beside the side-feature chain and the
 weight-gradient kernel.  Captured, that is ONE CUDA graph with parallel branches (0.84 -> 0.74 ms per step at the netflix shape);
 on CPU stand-ins and under the span timer the same launches run in program order.
+
+Batch-row fusion: during training only the loss heads read U / I, at the batch's rows, and they scatter gU / gI into those rows only.
+So train_step fuses the batch's rows alone, in both directions.  A branch forked at the start of the step builds two device-side row
+sets from the index buffer (`_batch_rows`: users, and pos | neg items, augmented triplets included; a repeated id is one row; only the
+first B' entries of a captured step's buffer are live) -- no host sync, one graph for every B'.  The fusion kernels then take the
+row list with its device-side count; each listed row runs the same per-row code as the full form, so it gets the same bits.  Off the
+batch the full backward would write dUl = dIl = 0 and add an exact zero to GFu / GFi / Gprof_*; `_grad_init(id_grads=True)` zeroes
+dUl / dIl instead, and the side-feature gradients already hold their final values.  Rows of U / I outside the batch keep stale values
+after a training step: `forward()` (evaluation, MM_Model, the eager mask / MAE branch) fuses every row.  At the netflix shape the two
+fusion families drop from 0.041 + 0.081 ms to 0.008 + 0.011 ms (H100 SXM 80 GB HBM3, 700 W; DESIGN §5).
 """
 from __future__ import annotations
 
@@ -123,6 +133,13 @@ class HotPath:
         self.branches = dev.type == "cuda" and os.environ.get("LLMREC_BRANCHES", "1") != "0"
         self._side, self._forked = {}, set()
         self.force_split = False          # tests: run the branch SCHEDULE (split launches) even where nothing can overlap (CPU stand-ins)
+        # train_step fuses only the batch's rows, in both directions (`_batch_rows`).  Gated like `branches`: CUDA devices only, so the
+        # CPU stand-ins keep running the full-row schedule their emulated ops implement; and only with side features, so the ID-only
+        # engine keeps U / I whole after a step -- it is the single-GPU reference the sharded engines are compared with row by row.
+        self.demand_fuse = dev.type == "cuda" and self.has_feats
+        if self.demand_fuse:
+            self.batch_u, self.batch_i = ops.RowSet(nu, dev), ops.RowSet(ni, dev)
+            self._batch_max = (0, 0)
 
     def _t(self, name):
         return self.timer.span(name) if self.timer is not None else contextlib.nullcontext()
@@ -226,7 +243,29 @@ class HotPath:
                 if after_sides is not None and wf and t == 1:
                     after_sides()
 
-    def _fuse_fwd(self):
+    def _batch_rows(self, users, pos, neg, meta=None):
+        """Device-side row sets of the step's batch: its users, and its pos | neg items (augmented triplets included); a repeated id is
+        one row.  With `meta` only the first B' = meta[0] entries are live (the index buffer's later slots hold earlier batches' ids)."""
+        n = None if meta is None else meta[:1]
+        self.batch_u.clear()
+        self.batch_u.add_ids(users, n)
+        self.batch_u.compact()
+        self.batch_i.clear()
+        self.batch_i.add_ids(pos, n)
+        self.batch_i.add_ids(neg, n)
+        self.batch_i.compact()
+        self._batch_max = (min(self.nu, int(users.numel())), min(self.ni, int(pos.numel()) + int(neg.numel())))
+
+    def _rows_kw(self, batch_rows):
+        """Keyword arguments of the user- and item-side fusion: all rows, or the row sets of the last `_batch_rows`."""
+        if not batch_rows:
+            return {}, {}
+        mu, mi = self._batch_max
+        return (dict(rows=self.batch_u.list, count=self.batch_u.count, max_rows=mu),
+                dict(rows=self.batch_i.list, count=self.batch_i.count, max_rows=mi))
+
+    def _fuse_fwd(self, batch_rows=False):
+        """batch_rows: U / I on the batch's rows only (train_step); the other rows keep whatever they held."""
         c = self.cfg
         if self.has_feats:
             coefs = [c.model_cat_rate, c.model_cat_rate, c.user_cat_rate] + [c.item_cat_rate] * len(self.keys)
@@ -234,20 +273,23 @@ class HotPath:
             si = [self.blk(self.Fi, 0), self.blk(self.Fi, 1), self.prof_i] + [self.blk(self.Fi, 2 + j) for j in range(len(self.keys))]
         else:
             coefs, su, si = [], [], []
+        ku, ki = self._rows_kw(batch_rows)
         with self._t("fuse_fwd"):
-            self._fork(lambda: ops.fuse_fwd(self.Ul, su, coefs, self.U))                                               # :185-197
-            ops.fuse_fwd(self.Il, si, coefs, self.I)
+            self._fork(lambda: ops.fuse_fwd(self.Ul, su, coefs, self.U, **ku))                                         # :185-197
+            ops.fuse_fwd(self.Il, si, coefs, self.I, **ki)
             self._join()
         self._fuse_args = (coefs, su, si)
 
     # ---- backward: expects gU, gI and (GFu, GFi, Gprof_u, Gprof_i, GP_usr_direct) filled ---------------
-    def backward(self, gp_usr_direct=None, gpi_direct=None):
-        self._fuse_bwd()
+    def backward(self, gp_usr_direct=None, gpi_direct=None, batch_rows=False):
+        self._fuse_bwd(batch_rows)
         self._chain_bwd(gp_usr_direct, gpi_direct)
         self._wgrad()
         return self.grads
 
-    def _fuse_bwd(self):
+    def _fuse_bwd(self, batch_rows=False):
+        """batch_rows: the batch's rows only -- gU / gI are zero on every other row, where the full form writes dUl = dIl = 0 and adds an
+        exact zero to GFu / GFi / Gprof_*; `_grad_init(id_grads=True)` has zeroed dUl / dIl instead."""
         L = self.L
         coefs, su, si = self._fuse_args
         if self.has_feats:
@@ -255,9 +297,10 @@ class HotPath:
             dsi = [self.blk(self.GFi, 0), self.blk(self.GFi, 1), self.Gprof_i] + [self.blk(self.GFi, 2 + j) for j in range(len(self.keys))]
         else:
             dsu, dsi = [], []
+        ku, ki = self._rows_kw(batch_rows)
         with self._t("fuse_bwd"):
-            self._fork(lambda: ops.fuse_bwd(self.gU, L + 1, self.dUl, su, coefs, dsu, True))
-            ops.fuse_bwd(self.gI, L + 1, self.dIl, si, coefs, dsi, True)
+            self._fork(lambda: ops.fuse_bwd(self.gU, L + 1, self.dUl, su, coefs, dsu, True, **ku))
+            ops.fuse_bwd(self.gI, L + 1, self.dIl, si, coefs, dsi, True, **ki)
             self._join()
 
     def _chain_bwd(self, gp_usr_direct=None, gpi_direct=None, with_feats=None, with_ids=True, opset=None):
@@ -357,9 +400,10 @@ class HotPath:
             ops.bpr_heads(heads, users, pos, neg, n_keep, c.regs0 / c.batch_size, self.head_out, self.loss, self._bpr_work, meta=meta)
         return self.loss
 
-    def _grad_init(self):
+    def _grad_init(self, id_grads=False):
         """First touch of every gradient buffer the loss heads accumulate into: the feat_reg gradient c*X on the image/text blocks (its
-        value starts the loss, main.py:151-156), zeros elsewhere.  Needs Fu / Fi only, not the fused outputs."""
+        value starts the loss, main.py:151-156), zeros elsewhere.  Needs Fu / Fi only, not the fused outputs.
+        id_grads: also zero dUl / dIl, which the batch-row fusion backward writes on the batch's rows only."""
         c = self.cfg
         regions = [(self.gU, None, 0.0), (self.gI, None, 0.0)]
         if self.has_feats:
@@ -369,6 +413,8 @@ class HotPath:
                         (self.Gprof_u, None, 0.0), (self.Gprof_i, None, 0.0)]
             if self.S > 2:
                 regions += [(self.GFu[:, d2:], None, 0.0), (self.GFi[:, d2:], None, 0.0)]
+        if id_grads:          # last: the loss's partial sums keep their slots, so its fixed-order reduction gives the same bits
+            regions += [(self.dUl, None, 0.0), (self.dIl, None, 0.0)]
         with self._t("grad_init"):
             ops.grad_init(regions, self.loss)
 
@@ -377,6 +423,11 @@ class HotPath:
         if self.opt is None:
             raise RuntimeError("attach an optimizer with set_optimizer() first")
         split = self.has_feats and self.timer is None and (self.branches or self.force_split)
+        demand = self.demand_fuse
+        if demand:
+            # the batch's row sets depend on the indices only: a branch from the start of the step, joined before the fusion
+            self._fork(lambda: self._batch_rows(users, pos, neg, meta), lane=1)
+        grad_init = lambda: self._grad_init(id_grads=demand)
         if split:
             # the ID layers do not depend on the projections: they run as a branch (through operators with their own long-row scratch)
             # beside the projection kernel and the side-feature products; the first touch of the gradient buffers follows on the branch.
@@ -392,31 +443,40 @@ class HotPath:
 
             self._fork(id_layers, lane=0)
             self._proj_fwd()
-            self._prop_fwd(with_ids=False, after_sides=lambda: self._fork(self._grad_init, lane=0))
+            self._prop_fwd(with_ids=False, after_sides=lambda: self._fork(grad_init, lane=0))
             if self.branches:
                 torch.cuda.current_stream().wait_event(self._ev_ids)         # the item-side fusion below reads Il; grad_init may still run
         else:
             self._proj_fwd()
-            self._prop_fwd(after_sides=lambda: self._fork(self._grad_init))  # branch: runs beside the remaining products and the fusion
-        self._fuse_fwd()                                                     # joins
+            self._prop_fwd(after_sides=lambda: self._fork(grad_init))        # branch: runs beside the remaining products and the fusion
+        self._join([1])                                                      # the row sets
+        self._fuse_fwd(batch_rows=demand)                                    # joins
         self._join()
         self.loss_and_output_grads(users, pos, neg, meta, init_done=True)
         if split:
-            self._fuse_bwd()
+            self._fuse_bwd(batch_rows=demand)
             self._fork(lambda: self._chain_bwd(with_feats=False, opset=ids[2:]), lane=0)    # ID chain
             self._chain_bwd(with_ids=False)                                                  # side-feature operands
             self._wgrad()
             self._join()
         else:
-            self.backward()
+            self.backward(batch_rows=demand)
         with self._t("adamw"):
             self.opt.step([self.grads[k] for k in self._opt_names])
         return self.loss
 
     def families(self, users, pos, neg):
-        """name -> thunk launching one kernel family of the step (bench.py times each from its own CUDA graph)."""
-        f = {"spmm_fwd": self._prop_fwd, "fuse_fwd": self._fuse_fwd, "loss_heads": lambda: self.loss_and_output_grads(users, pos, neg),
-             "fuse_bwd": self._fuse_bwd, "spmm_bwd": self._chain_bwd, "adamw": lambda: self.opt.step([self.grads[k] for k in self._opt_names])}
+        """name -> thunk launching one kernel family of the step (bench.py times each from its own CUDA graph).  The fusion families run
+        as train_step runs them: with the batch-row fusion, on the row sets of this batch (built here, outside the timed thunks), and
+        the loss heads with the first touch of dUl / dIl that this fusion needs."""
+        fuse_fwd, fuse_bwd = self._fuse_fwd, self._fuse_bwd
+        loss_heads = lambda: self.loss_and_output_grads(users, pos, neg)
+        if self.demand_fuse:
+            self._batch_rows(users, pos, neg)
+            fuse_fwd, fuse_bwd = (lambda: self._fuse_fwd(batch_rows=True)), (lambda: self._fuse_bwd(batch_rows=True))
+            loss_heads = lambda: (self._grad_init(id_grads=True), self.loss_and_output_grads(users, pos, neg, init_done=True))
+        f = {"spmm_fwd": self._prop_fwd, "fuse_fwd": fuse_fwd, "loss_heads": loss_heads,
+             "fuse_bwd": fuse_bwd, "spmm_bwd": self._chain_bwd, "adamw": lambda: self.opt.step([self.grads[k] for k in self._opt_names])}
         if self.has_feats:
             f.update(proj_fwd=self._proj_fwd, proj_wgrad=self._wgrad)
         return f

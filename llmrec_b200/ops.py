@@ -185,8 +185,12 @@ class RowSet:
         N.check(N.lib().llmrec_mark_neighbors(_p(_i32(rowptr)), _p(_i32(col)), _p(_i32(rows)), rows.numel(), _p(self.mask), _stream()), "mark_neighbors")
         _count()
 
-    def add_ids(self, ids):
-        N.check(N.lib().llmrec_mark_ids(_p(_i32(ids)), ids.numel(), _p(self.mask), _stream()), "mark_ids")
+    def add_ids(self, ids, n=None):
+        """n: optional int32 CUDA tensor whose first entry is the live length (ids[0 .. min(n[0], len(ids))) are marked; no host sync)"""
+        if n is None:
+            N.check(N.lib().llmrec_mark_ids(_p(_i32(ids)), ids.numel(), _p(self.mask), _stream()), "mark_ids")
+        else:
+            N.check(N.lib().llmrec_mark_ids_rows(_p(_i32(ids)), _p(_i32(n, "live length")), ids.numel(), _p(self.mask), _stream()), "mark_ids_rows")
         _count()
 
     def compact(self):
@@ -313,28 +317,54 @@ def _ld_table(tensors):
     return arr
 
 
-def fuse_fwd(layers, sides, coefs, out, rows=None, compact=False):
+def _row_list(rows, count, max_rows, what):
+    """(rows, count, max_rows) of a row-list launch with a device-side length: rows[0 .. min(count[0], max_rows)) are processed."""
+    if rows is None:
+        raise ValueError(f"{what}: a device-side count needs a row list")
+    mx = int(rows.numel()) if max_rows is None else min(int(max_rows), int(rows.numel()))
+    return _i32(rows), _i32(count, "count"), mx
+
+
+def fuse_fwd(layers, sides, coefs, out, rows=None, compact=False, count=None, max_rows=None):
     """out = mean(layers) + sum_t coefs[t] * normalize(sides[t])   (Models.py:185-197).
-    rows: only these rows; compact=True: layers are read at rows[b], sides and out are [len(rows) x d] blocks indexed by b."""
+    rows: only these rows; compact=True: layers are read at rows[b], sides and out are [len(rows) x d] blocks indexed by b.
+    count: int32[1] CUDA tensor, the live length of `rows` (only rows[0 .. min(count[0], max_rows)) are fused; no host sync)."""
     for t in list(layers) + list(sides) + [out]:
         _mat(t)
+    cf = (C.c_float * max(1, len(coefs)))(*[float(c) for c in coefs])
+    if count is not None:
+        if compact:
+            raise ValueError("fuse_fwd: the device-count form is not compact")
+        rows, count, mx = _row_list(rows, count, max_rows, "fuse_fwd")
+        N.check(N.lib().llmrec_fuse_fwd_rows_f32(_ptr_table(layers), _ld_table(layers), len(layers), _ptr_table(sides), _ld_table(sides), cf,
+                                                  len(sides), _p(out), _ld(out), _p(rows), _p(count), mx, out.shape[1], _stream()), "fuse_fwd_rows")
+        _count()
+        return out
     n = out.shape[0] if rows is None else rows.numel()
     if compact:
         if rows is None:
             raise ValueError("fuse_fwd: compact form needs a row list")
         n = -n
-    cf = (C.c_float * max(1, len(coefs)))(*[float(c) for c in coefs])
     N.check(N.lib().llmrec_fuse_fwd_f32(_ptr_table(layers), _ld_table(layers), len(layers), _ptr_table(sides), _ld_table(sides), cf,
                                          len(sides), _p(out), _ld(out), _p(rows), n, out.shape[1], _stream()), "fuse_fwd")
     _count()
     return out
 
 
-def fuse_bwd(g, n_layers, d_layer, sides, coefs, d_sides, accumulate, rows=None):
+def fuse_bwd(g, n_layers, d_layer, sides, coefs, d_sides, accumulate, rows=None, count=None, max_rows=None):
+    """count: as for fuse_fwd; a row listed twice would be processed twice (accumulate=True adds twice): pass a set (RowSet.list)."""
     _mat(g)
-    n = g.shape[0] if rows is None else rows.numel()
     cf = (C.c_float * max(1, len(coefs)))(*[float(c) for c in coefs])
-    N.check(N.lib().llmrec_fuse_bwd_f32(_p(g), _ld(g), n_layers, _p(d_layer), _ld(d_layer) if d_layer is not None else 0,
+    dl = (_p(d_layer), _ld(d_layer) if d_layer is not None else 0)
+    if count is not None:
+        rows, count, mx = _row_list(rows, count, max_rows, "fuse_bwd")
+        N.check(N.lib().llmrec_fuse_bwd_rows_f32(_p(g), _ld(g), n_layers, *dl, _ptr_table(sides), _ld_table(sides), cf, _ptr_table(d_sides),
+                                                  _ld_table(d_sides), len(sides), 1 if accumulate else 0, _p(rows), _p(count), mx, g.shape[1],
+                                                  _stream()), "fuse_bwd_rows")
+        _count()
+        return
+    n = g.shape[0] if rows is None else rows.numel()
+    N.check(N.lib().llmrec_fuse_bwd_f32(_p(g), _ld(g), n_layers, *dl,
                                          _ptr_table(sides), _ld_table(sides), cf, _ptr_table(d_sides), _ld_table(d_sides), len(sides),
                                          1 if accumulate else 0, _p(rows), n, g.shape[1], _stream()), "fuse_bwd")
     _count()

@@ -40,7 +40,13 @@ def step_bytes(hp, nnz):
     out["spmm_bwd"] = sp(ni, nu, 1) + sp(nu, ni, S + 2) + sp(ni, nu, S + 1) + (sp(nu, ni, 1) + sp(ni, nu, 1) if L >= 2 else 0)
     out["adamw"] = 28 * sum(p.numel() for p in hp.opt.params)
     T = (3 + len(hp.keys)) if hp.has_feats else 0
-    fuse = 4 * d * (nu + ni) * ((L + 1) + T + 1)
+    # rows fused per step: every user and item, or with train_step's batch-row fusion the batch's distinct users and items (the row
+    # counts of the last row sets built -- a host read, so call this outside any timed region) plus one int32 id per row
+    n_fused, ids = nu + ni, 0
+    if getattr(hp, "demand_fuse", False):
+        n_fused = int(hp.batch_u.count.item()) + int(hp.batch_i.count.item())
+        ids = 4 * n_fused
+    fuse = 4 * d * n_fused * ((L + 1) + T + 1) + ids
     out["fuse_fwd"] = fuse
-    out["fuse_bwd"] = fuse + 4 * d * (nu + ni) * T
+    out["fuse_bwd"] = fuse + 4 * d * n_fused * T
     return out
