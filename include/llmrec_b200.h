@@ -136,12 +136,12 @@ int64_t llmrec_proj_wgrad_scratch(int64_t n, int32_t k, int32_t d, int32_t mode)
 typedef struct {
   const float* X; const float* W; const float* bias; float* Y; float* wsplit;
   int64_t ldx, ldy, n;
-  int32_t k, _reserved;       /* 0 */
+  int32_t k, _reserved;       /* flags: 0 or LLMREC_PROJ_ROW_MAP */
 } llmrec_proj_fwd_problem;
 typedef struct {
   const float* X; const float* dY; float* dW; float* db;
   int64_t ldx, lddy, n;
-  int32_t k, accumulate;      /* LLMREC_WGRAD_ACCUMULATE */
+  int32_t k, accumulate;      /* flags: LLMREC_WGRAD_ACCUMULATE | LLMREC_PROJ_ROW_MAP */
 } llmrec_proj_wgrad_problem;
 #define LLMREC_WGRAD_ACCUMULATE 1
 int llmrec_proj_fwd_group_f32(const llmrec_proj_fwd_problem* probs_host, int32_t n_prob, int32_t d, int32_t mode,
@@ -169,12 +169,12 @@ int64_t llmrec_proj_wgrad_group_scratch(const llmrec_proj_wgrad_problem* probs_h
 typedef struct {
   const uint16_t* X; const float* W; const float* bias; float* Y; float* wsplit;
   int64_t ldx, ldy, n;
-  int32_t k, _reserved;       /* 0 */
+  int32_t k, _reserved;       /* flags: 0 or LLMREC_PROJ_ROW_MAP */
 } llmrec_proj_fwd_problem_bf16;
 typedef struct {
   const uint16_t* X; const float* dY; float* dW; float* db;
   int64_t ldx, lddy, n;
-  int32_t k, accumulate;      /* LLMREC_WGRAD_ACCUMULATE */
+  int32_t k, accumulate;      /* flags: LLMREC_WGRAD_ACCUMULATE | LLMREC_PROJ_ROW_MAP */
 } llmrec_proj_wgrad_problem_bf16;
 int llmrec_proj_fwd_group_bf16(const llmrec_proj_fwd_problem_bf16* probs_host, int32_t n_prob, int32_t d, int32_t mode,
                                llmrec_stream_t stream);
@@ -182,6 +182,24 @@ int llmrec_proj_wgrad_group_bf16(const llmrec_proj_wgrad_problem_bf16* probs_hos
                                  float* scratch /* zero-initialised ONCE, as for llmrec_proj_wgrad_group_f32 */,
                                  int64_t scratch_elems, llmrec_stream_t stream);
 int64_t llmrec_proj_wgrad_group_bf16_scratch(const llmrec_proj_wgrad_problem_bf16* probs_host, int32_t n_prob, int32_t d, int32_t mode);
+
+/* Row maps, for X tables that hold a subset of the output's rows (the training step projects only the items with a training edge,
+ * from compact copies of the item tables).  A problem whose flags word -- `_reserved` of the forward problem, `accumulate` of the
+ * weight-gradient problem, both _f32 and _bf16 -- has LLMREC_PROJ_ROW_MAP set takes a map from an llmrec_proj_row_map record.  The
+ * records follow the n_prob problems in the same host array, one per problem in order (records of unflagged problems are ignored);
+ * callers that never set the bit pass plain problem arrays as before.  rows: a DEVICE int32 list of the problem's n X rows, every
+ * entry a valid row of Y / dY:
+ *   forward          X row r is written to Y[rows[r]]; Y rows not in the map are left untouched.  Each written row gets the bits
+ *                    of the same X row in an unmapped call (the per-row arithmetic is unchanged);
+ *   weight gradient  X row r pairs with dY[rows[r]]: dW (+)= sum_r dY[rows[r]]^T X[r].  The bias sums db (+)= colsum(dY) run over
+ *                    ALL n_dy rows of dY, so db gets the bits of an unmapped call on the full tables; dW differs from that call by
+ *                    rounding only (the row chunks see another row sequence).
+ * The _scratch queries take the same arrays (n = the X row count). */
+typedef struct {
+  const int32_t* rows;
+  int64_t n_dy;               /* weight gradient: row count of dY (the bias sums run over all of them); unused by the forward */
+} llmrec_proj_row_map;
+#define LLMREC_PROJ_ROW_MAP 2
 
 /* ---------------------------------------------------------------------------------------------
  * Fusion (Models.py:185-197):  out = mean(layer_0..layer_{L}) + sum_t coef[t] * x_t / max(||x_t||_2, 1e-12)

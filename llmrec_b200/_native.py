@@ -47,6 +47,14 @@ class ProjWgradProblemBf16(C.Structure):    # X: raw bfloat16 bits
     _fields_ = ProjWgradProblem._fields_
 
 
+class ProjRowMap(C.Structure):             # follows the problems of a grouped projection call that flags PROJ_ROW_MAP
+    _fields_ = [("rows", C.c_void_p), ("n_dy", C.c_int64)]
+
+
+PROJ_ROW_MAP = 2
+WGRAD_ACCUMULATE = 1
+
+
 class BprHead(C.Structure):
     _fields_ = [("XU", C.c_void_p), ("XI", C.c_void_p), ("GU", C.c_void_p), ("GI", C.c_void_p),
                 ("ldxu", C.c_int64), ("ldxi", C.c_int64), ("ldgu", C.c_int64), ("ldgi", C.c_int64),

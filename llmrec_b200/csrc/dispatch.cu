@@ -4,14 +4,14 @@
 #include "common.cuh"
 
 namespace llmrec {
-int proj_fwd_simt(const float*, int64_t, const float*, const float*, float*, int64_t, int64_t, int, int, cudaStream_t);
-int proj_fwd_simt(const uint16_t*, int64_t, const float*, const float*, float*, int64_t, int64_t, int, int, cudaStream_t);
-int proj_wgrad_simt(const float*, int64_t, const float*, int64_t, float*, float*, int64_t, int, int, int, cudaStream_t);
-int proj_wgrad_simt(const uint16_t*, int64_t, const float*, int64_t, float*, float*, int64_t, int, int, int, cudaStream_t);
+int proj_fwd_simt(const float*, int64_t, const float*, const float*, float*, int64_t, int64_t, int, int, const int*, cudaStream_t);
+int proj_fwd_simt(const uint16_t*, int64_t, const float*, const float*, float*, int64_t, int64_t, int, int, const int*, cudaStream_t);
+int proj_wgrad_simt(const float*, int64_t, const float*, int64_t, float*, float*, int64_t, int, int, int, const int*, int64_t, cudaStream_t);
+int proj_wgrad_simt(const uint16_t*, int64_t, const float*, int64_t, float*, float*, int64_t, int, int, int, const int*, int64_t, cudaStream_t);
 int score_topk_simt(const float*, int64_t, const float*, int64_t, const int*, int, int, int, const int*, const int*, int, int*, float*, float*, int64_t, cudaStream_t);
 bool proj_tc_supported(int d, int64_t ldx, const void* X, int k, bool wgrad, bool bf16);
-int proj_fwd_tc_group(const llmrec_proj_fwd_problem*, int, int, int, bool, cudaStream_t);
-int proj_wgrad_tc_group(const llmrec_proj_wgrad_problem*, int, int, int, bool, float*, int64_t, cudaStream_t);
+int proj_fwd_tc_group(const llmrec_proj_fwd_problem*, const int32_t* const*, int, int, int, bool, cudaStream_t);
+int proj_wgrad_tc_group(const llmrec_proj_wgrad_problem*, const int32_t* const*, const int64_t*, int, int, int, bool, float*, int64_t, cudaStream_t);
 int64_t proj_wgrad_tc_scratch(const llmrec_proj_wgrad_problem*, int, int, bool);
 bool score_tc_supported(int d, int K, long long ldu, long long ldi, const void* U, const void* I);
 long long score_tc_scratch(int n_batch, int n_items, int d, int K);
@@ -36,35 +36,71 @@ static bool wg_tc_ok(const llmrec_proj_wgrad_problem* pr, int n, int d, int mode
   return true;
 }
 
-static int proj_fwd_group(const llmrec_proj_fwd_problem* pr, int32_t n_prob, int32_t d, int32_t mode, bool bf16, llmrec_stream_t stream) {
+// Row maps (LLMREC_PROJ_ROW_MAP): the llmrec_proj_row_map records that follow the n_prob problems of a host array (same struct size for
+// the _f32 and _bf16 problems); rows / n_dy stay empty when no problem is flagged, and a flagged problem needs a non-NULL map.
+struct RowMaps { std::vector<const int32_t*> rows; std::vector<int64_t> n_dy; };
+static int32_t flags(const llmrec_proj_fwd_problem& p) { return p._reserved; }
+static int32_t flags(const llmrec_proj_fwd_problem_bf16& p) { return p._reserved; }
+static int32_t flags(const llmrec_proj_wgrad_problem& p) { return p.accumulate; }
+static int32_t flags(const llmrec_proj_wgrad_problem_bf16& p) { return p.accumulate; }
+template <class Prob>
+static int row_maps(const Prob* pr, int32_t n_prob, bool wgrad, RowMaps& M) {
+  bool any = false;
+  for (int p = 0; p < n_prob; ++p) any = any || (flags(pr[p]) & LLMREC_PROJ_ROW_MAP);
+  if (!any) return 0;
+  const llmrec_proj_row_map* rec = reinterpret_cast<const llmrec_proj_row_map*>(pr + n_prob);
+  M.rows.assign(n_prob, nullptr);
+  M.n_dy.assign(n_prob, 0);
+  for (int p = 0; p < n_prob; ++p) {
+    M.n_dy[p] = pr[p].n;
+    if (!(flags(pr[p]) & LLMREC_PROJ_ROW_MAP)) continue;
+    LLMREC_CHECK_ARG(rec[p].rows || pr[p].n <= 0, "proj: problem %d is flagged LLMREC_PROJ_ROW_MAP but its map is NULL", p);
+    LLMREC_CHECK_ARG(!wgrad || rec[p].n_dy >= 0, "proj_wgrad: problem %d has a negative dY row count", p);
+    M.rows[p] = rec[p].rows; M.n_dy[p] = rec[p].n_dy;
+  }
+  return 0;
+}
+
+// rows: NULL, or n_prob optional row maps
+static int proj_fwd_group(const llmrec_proj_fwd_problem* pr, const int32_t* const* rows, int32_t n_prob, int32_t d, int32_t mode, bool bf16,
+                          llmrec_stream_t stream) {
   LLMREC_REQUIRE_DEVICE();
   LLMREC_CHECK_ARG(n_prob >= 1 && d >= 1, "proj_fwd_group: bad sizes");
   cudaStream_t st = as_stream(stream);
   for (int p0 = 0; p0 < n_prob; p0 += 8) {
     int np = n_prob - p0 < 8 ? n_prob - p0 : 8;
     if (fwd_tc_ok(pr + p0, np, d, mode, bf16)) {
-      int rc = proj_fwd_tc_group(pr + p0, np, d, mode, bf16, st);
+      int rc = proj_fwd_tc_group(pr + p0, rows ? rows + p0 : nullptr, np, d, mode, bf16, st);
       if (rc) return rc;
     } else {
       for (int p = p0; p < p0 + np; ++p) {
         if (pr[p].n <= 0) continue;
-        int rc = bf16 ? proj_fwd_simt(reinterpret_cast<const uint16_t*>(pr[p].X), pr[p].ldx, pr[p].W, pr[p].bias, pr[p].Y, pr[p].ldy, pr[p].n, pr[p].k, d, st)
-                      : proj_fwd_simt(pr[p].X, pr[p].ldx, pr[p].W, pr[p].bias, pr[p].Y, pr[p].ldy, pr[p].n, pr[p].k, d, st);
+        const int32_t* map = rows ? rows[p] : nullptr;
+        int rc = bf16 ? proj_fwd_simt(reinterpret_cast<const uint16_t*>(pr[p].X), pr[p].ldx, pr[p].W, pr[p].bias, pr[p].Y, pr[p].ldy, pr[p].n, pr[p].k, d, map, st)
+                      : proj_fwd_simt(pr[p].X, pr[p].ldx, pr[p].W, pr[p].bias, pr[p].Y, pr[p].ldy, pr[p].n, pr[p].k, d, map, st);
         if (rc) return rc;
       }
     }
   }
   return 0;
 }
+static std::vector<llmrec_proj_fwd_problem> as_f32_layout(const llmrec_proj_fwd_problem_bf16* pr, int32_t n_prob) {
+  std::vector<llmrec_proj_fwd_problem> q(n_prob > 0 ? n_prob : 0);
+  for (int p = 0; p < n_prob; ++p)
+    q[p] = {reinterpret_cast<const float*>(pr[p].X), pr[p].W, pr[p].bias, pr[p].Y, pr[p].wsplit, pr[p].ldx, pr[p].ldy, pr[p].n, pr[p].k, 0};
+  return q;
+}
 extern "C" int llmrec_proj_fwd_group_f32(const llmrec_proj_fwd_problem* pr, int32_t n_prob, int32_t d, int32_t mode, llmrec_stream_t stream) {
-  return proj_fwd_group(pr, n_prob, d, mode, false, stream);
+  LLMREC_CHECK_ARG(pr && n_prob >= 1, "proj_fwd_group: bad sizes");
+  RowMaps M;
+  if (int rc = row_maps(pr, n_prob, false, M)) return rc;
+  return proj_fwd_group(pr, M.rows.empty() ? nullptr : M.rows.data(), n_prob, d, mode, false, stream);
 }
 extern "C" int llmrec_proj_fwd_group_bf16(const llmrec_proj_fwd_problem_bf16* pr, int32_t n_prob, int32_t d, int32_t mode, llmrec_stream_t stream) {
   LLMREC_CHECK_ARG(pr && n_prob >= 1, "proj_fwd_group: bad sizes");
-  std::vector<llmrec_proj_fwd_problem> q(n_prob);
-  for (int p = 0; p < n_prob; ++p)
-    q[p] = {reinterpret_cast<const float*>(pr[p].X), pr[p].W, pr[p].bias, pr[p].Y, pr[p].wsplit, pr[p].ldx, pr[p].ldy, pr[p].n, pr[p].k, 0};
-  return proj_fwd_group(q.data(), n_prob, d, mode, true, stream);
+  RowMaps M;
+  if (int rc = row_maps(pr, n_prob, false, M)) return rc;
+  return proj_fwd_group(as_f32_layout(pr, n_prob).data(), M.rows.empty() ? nullptr : M.rows.data(), n_prob, d, mode, true, stream);
 }
 extern "C" int llmrec_proj_fwd_f32(const float* X, int64_t ldx, const float* W, const float* bias, float* Y, int64_t ldy,
                                    int64_t n, int32_t k, int32_t d, int32_t mode, float* wsplit, llmrec_stream_t stream) {
@@ -81,21 +117,24 @@ static int64_t proj_wgrad_scratch(const llmrec_proj_wgrad_problem* pr, int32_t n
   }
   return need;
 }
-static int proj_wgrad_group(const llmrec_proj_wgrad_problem* pr, int32_t n_prob, int32_t d, int32_t mode, bool bf16,
-                            float* scratch, int64_t scratch_elems, llmrec_stream_t stream) {
+// rows / n_dy: NULL, or per problem an optional dY row map and the row count of dY
+static int proj_wgrad_group(const llmrec_proj_wgrad_problem* pr, const int32_t* const* rows, const int64_t* n_dy, int32_t n_prob, int32_t d,
+                            int32_t mode, bool bf16, float* scratch, int64_t scratch_elems, llmrec_stream_t stream) {
   LLMREC_REQUIRE_DEVICE();
   LLMREC_CHECK_ARG(n_prob >= 1 && d >= 1, "proj_wgrad_group: bad sizes");
   cudaStream_t st = as_stream(stream);
   for (int p0 = 0; p0 < n_prob; p0 += 8) {
     int np = n_prob - p0 < 8 ? n_prob - p0 : 8;
     if (wg_tc_ok(pr + p0, np, d, mode, bf16)) {
-      int rc = proj_wgrad_tc_group(pr + p0, np, d, mode, bf16, scratch, scratch_elems, st);
+      int rc = proj_wgrad_tc_group(pr + p0, rows ? rows + p0 : nullptr, rows ? n_dy + p0 : nullptr, np, d, mode, bf16, scratch, scratch_elems, st);
       if (rc) return rc;
     } else {
       for (int p = p0; p < p0 + np; ++p) {
         const int acc = pr[p].accumulate & LLMREC_WGRAD_ACCUMULATE;
-        int rc = bf16 ? proj_wgrad_simt(reinterpret_cast<const uint16_t*>(pr[p].X), pr[p].ldx, pr[p].dY, pr[p].lddy, pr[p].dW, pr[p].db, pr[p].n, pr[p].k, d, acc, st)
-                      : proj_wgrad_simt(pr[p].X, pr[p].ldx, pr[p].dY, pr[p].lddy, pr[p].dW, pr[p].db, pr[p].n, pr[p].k, d, acc, st);
+        const int32_t* map = rows ? rows[p] : nullptr;
+        const int64_t ndy = n_dy ? n_dy[p] : pr[p].n;
+        int rc = bf16 ? proj_wgrad_simt(reinterpret_cast<const uint16_t*>(pr[p].X), pr[p].ldx, pr[p].dY, pr[p].lddy, pr[p].dW, pr[p].db, pr[p].n, pr[p].k, d, acc, map, ndy, st)
+                      : proj_wgrad_simt(pr[p].X, pr[p].ldx, pr[p].dY, pr[p].lddy, pr[p].dW, pr[p].db, pr[p].n, pr[p].k, d, acc, map, ndy, st);
         if (rc) return rc;
       }
     }
@@ -116,12 +155,20 @@ extern "C" int64_t llmrec_proj_wgrad_group_bf16_scratch(const llmrec_proj_wgrad_
 }
 extern "C" int llmrec_proj_wgrad_group_f32(const llmrec_proj_wgrad_problem* pr, int32_t n_prob, int32_t d, int32_t mode,
                                            float* scratch, int64_t scratch_elems, llmrec_stream_t stream) {
-  return proj_wgrad_group(pr, n_prob, d, mode, false, scratch, scratch_elems, stream);
+  LLMREC_CHECK_ARG(pr && n_prob >= 1, "proj_wgrad_group: bad sizes");
+  RowMaps M;
+  if (int rc = row_maps(pr, n_prob, true, M)) return rc;
+  const bool mapped = !M.rows.empty();
+  return proj_wgrad_group(pr, mapped ? M.rows.data() : nullptr, mapped ? M.n_dy.data() : nullptr, n_prob, d, mode, false, scratch, scratch_elems, stream);
 }
 extern "C" int llmrec_proj_wgrad_group_bf16(const llmrec_proj_wgrad_problem_bf16* pr, int32_t n_prob, int32_t d, int32_t mode,
                                             float* scratch, int64_t scratch_elems, llmrec_stream_t stream) {
   LLMREC_CHECK_ARG(pr && n_prob >= 1, "proj_wgrad_group: bad sizes");
-  return proj_wgrad_group(as_f32_layout(pr, n_prob).data(), n_prob, d, mode, true, scratch, scratch_elems, stream);
+  RowMaps M;
+  if (int rc = row_maps(pr, n_prob, true, M)) return rc;
+  const bool mapped = !M.rows.empty();
+  return proj_wgrad_group(as_f32_layout(pr, n_prob).data(), mapped ? M.rows.data() : nullptr, mapped ? M.n_dy.data() : nullptr, n_prob, d, mode,
+                          true, scratch, scratch_elems, stream);
 }
 extern "C" int64_t llmrec_proj_wgrad_scratch(int64_t n, int32_t k, int32_t d, int32_t mode) {
   llmrec_proj_wgrad_problem p{nullptr, nullptr, nullptr, nullptr, 4, 4, n, k, 0};

@@ -10,11 +10,11 @@ namespace llmrec {
 __device__ __forceinline__ float x_f32(float x) { return x; }
 __device__ __forceinline__ float x_f32(uint16_t x) { return __uint_as_float((uint32_t)x << 16); }
 
-// Y[n x d] = X[n x k] W^T[k x d] + b ; 64x64 tile, K step 16, 4x4 per thread
+// Y[n x d] = X[n x k] W^T[k x d] + b ; 64x64 tile, K step 16, 4x4 per thread.  rows (optional): X row r is written to Y row rows[r]
 template <class T>
 __global__ void __launch_bounds__(256) proj_fwd_simt_kernel(const T* __restrict__ X, int64_t ldx, const float* __restrict__ W,
                                                             const float* __restrict__ bias, float* __restrict__ Y, int64_t ldy,
-                                                            int64_t n, int k, int d) {
+                                                            int64_t n, int k, int d, const int* __restrict__ rows) {
   __shared__ float Xs[16][64 + 4];
   __shared__ float Ws[16][64 + 4];
   const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;
@@ -46,18 +46,21 @@ __global__ void __launch_bounds__(256) proj_fwd_simt_kernel(const T* __restrict_
   for (int i = 0; i < 4; ++i) {
     int64_t gr = row0 + ty * 4 + i;
     if (gr >= n) continue;
+    const int64_t yr = rows ? (int64_t)rows[gr] : gr;
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
       int gc = col0 + tx * 4 + j;
-      if (gc < d) Y[gr * ldy + gc] = acc[i][j] + (bias ? bias[gc] : 0.f);
+      if (gc < d) Y[yr * ldy + gc] = acc[i][j] + (bias ? bias[gc] : 0.f);
     }
   }
 }
 
-// dW[d x k] += sum_r dY[r,:]^T X[r,:] over a row chunk ; db[d] += colsum(dY) (k-tile 0 only)
+// dW[d x k] += sum_r dY[r,:]^T X[r,:] over a row chunk ; db[d] += colsum(dY) (k-tile 0 only).
+// rows (optional): X row r pairs with dY row rows[r] (db is then NULL: colsum_simt_kernel sums every row of dY)
 template <class T>
 __global__ void __launch_bounds__(256) proj_wgrad_simt_kernel(const T* __restrict__ X, int64_t ldx, const float* __restrict__ dY, int64_t lddy,
-                                                              float* __restrict__ dW, float* __restrict__ db, int64_t n, int k, int d, int rows_per_chunk) {
+                                                              float* __restrict__ dW, float* __restrict__ db, int64_t n, int k, int d, int rows_per_chunk,
+                                                              const int* __restrict__ rows) {
   __shared__ float Gs[16][64 + 4];  // dY tile  [r][dcol]
   __shared__ float Xs[16][64 + 4];  // X tile   [r][kcol]
   const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;
@@ -70,7 +73,7 @@ __global__ void __launch_bounds__(256) proj_wgrad_simt_kernel(const T* __restric
     for (int i = threadIdx.x; i < 16 * 64; i += 256) {
       int r = i >> 6, c = i & 63;
       int64_t gr = r0 + r;
-      Gs[r][c] = (gr < r_end && d0 + c < d) ? dY[gr * lddy + d0 + c] : 0.f;
+      Gs[r][c] = (gr < r_end && d0 + c < d) ? dY[(rows ? (int64_t)rows[gr] : gr) * lddy + d0 + c] : 0.f;
       Xs[r][c] = (gr < r_end && k0 + c < k) ? x_f32(X[gr * ldx + k0 + c]) : 0.f;
     }
     __syncthreads();
@@ -101,35 +104,60 @@ __global__ void __launch_bounds__(256) proj_wgrad_simt_kernel(const T* __restric
   }
 }
 
+// db[d] += colsum(dY[n_dy x d]) for the row-mapped weight gradient: every row of dY, in row order within 1024-row chunks whose sums are
+// added atomically -- the order of the weight-gradient kernel's own bias sums, so one chunk gives its bits
+__global__ void __launch_bounds__(256) colsum_simt_kernel(const float* __restrict__ dY, int64_t lddy, float* __restrict__ db, int64_t n_dy, int d,
+                                                          int rows_per_chunk) {
+  const int c = blockIdx.y * 256 + threadIdx.x;
+  if (c >= d) return;
+  const int64_t r_beg = (int64_t)blockIdx.x * rows_per_chunk, r_end = min(n_dy, r_beg + rows_per_chunk);
+  float s = 0.f;
+  for (int64_t r = r_beg; r < r_end; ++r) s += dY[r * lddy + c];
+  atomicAdd(db + c, s);
+}
+
 template <class T>
-static int fwd_simt(const T* X, int64_t ldx, const float* W, const float* bias, float* Y, int64_t ldy, int64_t n, int k, int d, cudaStream_t st) {
+static int fwd_simt(const T* X, int64_t ldx, const float* W, const float* bias, float* Y, int64_t ldy, int64_t n, int k, int d, const int* rows,
+                    cudaStream_t st) {
   dim3 grid((unsigned)((n + 63) / 64), (d + 63) / 64);
-  proj_fwd_simt_kernel<T><<<grid, 256, 0, st>>>(X, ldx, W, bias, Y, ldy, n, k, d);
+  proj_fwd_simt_kernel<T><<<grid, 256, 0, st>>>(X, ldx, W, bias, Y, ldy, n, k, d, rows);
   LLMREC_CHECK_LAUNCH("proj_fwd_simt");
   return 0;
 }
 template <class T>
-static int wgrad_simt(const T* X, int64_t ldx, const float* dY, int64_t lddy, float* dW, float* db, int64_t n, int k, int d, int accumulate, cudaStream_t st) {
+static int wgrad_simt(const T* X, int64_t ldx, const float* dY, int64_t lddy, float* dW, float* db, int64_t n, int k, int d, int accumulate,
+                      const int* rows, int64_t n_dy, cudaStream_t st) {
   if (!accumulate) {
     cudaMemsetAsync(dW, 0, sizeof(float) * (size_t)d * k, st);
     if (db) cudaMemsetAsync(db, 0, sizeof(float) * d, st);
   }
   const int rows_per_chunk = 1024;
-  dim3 grid((k + 63) / 64, (d + 63) / 64, (unsigned)((n + rows_per_chunk - 1) / rows_per_chunk));
-  proj_wgrad_simt_kernel<T><<<grid, 256, 0, st>>>(X, ldx, dY, lddy, dW, db, n, k, d, rows_per_chunk);
-  LLMREC_CHECK_LAUNCH("proj_wgrad_simt");
+  const bool mapped = rows || n_dy != n;     // the bias sums then run over the n_dy rows of dY, not beside the weight gradient
+  if (n > 0) {
+    dim3 grid((k + 63) / 64, (d + 63) / 64, (unsigned)((n + rows_per_chunk - 1) / rows_per_chunk));
+    proj_wgrad_simt_kernel<T><<<grid, 256, 0, st>>>(X, ldx, dY, lddy, dW, mapped ? nullptr : db, n, k, d, rows_per_chunk, rows);
+    LLMREC_CHECK_LAUNCH("proj_wgrad_simt");
+  }
+  if (mapped && db && n_dy > 0) {
+    colsum_simt_kernel<<<dim3((unsigned)((n_dy + rows_per_chunk - 1) / rows_per_chunk), (d + 255) / 256), 256, 0, st>>>(dY, lddy, db, n_dy, d, rows_per_chunk);
+    LLMREC_CHECK_LAUNCH("colsum_simt");
+  }
   return 0;
 }
-int proj_fwd_simt(const float* X, int64_t ldx, const float* W, const float* bias, float* Y, int64_t ldy, int64_t n, int k, int d, cudaStream_t st) {
-  return fwd_simt(X, ldx, W, bias, Y, ldy, n, k, d, st);
+int proj_fwd_simt(const float* X, int64_t ldx, const float* W, const float* bias, float* Y, int64_t ldy, int64_t n, int k, int d, const int* rows,
+                  cudaStream_t st) {
+  return fwd_simt(X, ldx, W, bias, Y, ldy, n, k, d, rows, st);
 }
-int proj_fwd_simt(const uint16_t* X, int64_t ldx, const float* W, const float* bias, float* Y, int64_t ldy, int64_t n, int k, int d, cudaStream_t st) {
-  return fwd_simt(X, ldx, W, bias, Y, ldy, n, k, d, st);
+int proj_fwd_simt(const uint16_t* X, int64_t ldx, const float* W, const float* bias, float* Y, int64_t ldy, int64_t n, int k, int d, const int* rows,
+                  cudaStream_t st) {
+  return fwd_simt(X, ldx, W, bias, Y, ldy, n, k, d, rows, st);
 }
-int proj_wgrad_simt(const float* X, int64_t ldx, const float* dY, int64_t lddy, float* dW, float* db, int64_t n, int k, int d, int accumulate, cudaStream_t st) {
-  return wgrad_simt(X, ldx, dY, lddy, dW, db, n, k, d, accumulate, st);
+int proj_wgrad_simt(const float* X, int64_t ldx, const float* dY, int64_t lddy, float* dW, float* db, int64_t n, int k, int d, int accumulate,
+                    const int* rows, int64_t n_dy, cudaStream_t st) {
+  return wgrad_simt(X, ldx, dY, lddy, dW, db, n, k, d, accumulate, rows, n_dy, st);
 }
-int proj_wgrad_simt(const uint16_t* X, int64_t ldx, const float* dY, int64_t lddy, float* dW, float* db, int64_t n, int k, int d, int accumulate, cudaStream_t st) {
-  return wgrad_simt(X, ldx, dY, lddy, dW, db, n, k, d, accumulate, st);
+int proj_wgrad_simt(const uint16_t* X, int64_t ldx, const float* dY, int64_t lddy, float* dW, float* db, int64_t n, int k, int d, int accumulate,
+                    const int* rows, int64_t n_dy, cudaStream_t st) {
+  return wgrad_simt(X, ldx, dY, lddy, dW, db, n, k, d, accumulate, rows, n_dy, st);
 }
 }  // namespace llmrec

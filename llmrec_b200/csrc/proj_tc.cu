@@ -160,21 +160,26 @@ struct FwdUnit {
   static __device__ void ld_frag(uint32_t (&a)[4], uint32_t sx, int blk, int kk, int warp, int lane) { ld_frag_fwd(a, sx, blk, kk, warp, lane); }
   // bf16: descriptor of m64 block `blk` (64 rows x 128 bytes), k16 step kk (+32 bytes inside the swizzled rows)
   static __device__ uint64_t a_desc(uint32_t sx, int blk, int kk) { return gmma_desc_sw128(sx + blk * 8192u + kk * 32u); }
-  __device__ void store(float (&acc)[MB][D / 2], int cw, int warp, int lane) const {   // registers (+bias) -> Y
+  __device__ void store(float (&acc)[MB][D / 2], int cw, int warp, int lane) const {   // registers (+bias) -> Y (at rows[row] with a row map)
     const FwdProblem& pr = P.prob[p];
     const int g = lane >> 2, t = lane & 3;
 #pragma unroll
     for (int j = 0; j < MB; ++j) {
       const int row0 = mblk * Cfg::TM + (cw * MB + j) * 64 + warp * 16 + g;
+      long long yrow[2];
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int row = row0 + 8 * h;
+        yrow[h] = row < pr.n ? (pr.rows ? (long long)__ldg(pr.rows + row) : (long long)row) : -1;
+      }
 #pragma unroll
       for (int c = 0; c < D / 8; ++c) {
         const int col = c * 8 + 2 * t;
         const float2 b = pr.bias ? __ldg(reinterpret_cast<const float2*>(pr.bias + col)) : make_float2(0.f, 0.f);
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
-          const int row = row0 + 8 * h;
-          if (row < pr.n)
-            *reinterpret_cast<float2*>(pr.Y + (long long)row * pr.ldy + col) = make_float2(acc[j][4 * c + 2 * h] + b.x, acc[j][4 * c + 2 * h + 1] + b.y);
+          if (yrow[h] >= 0)
+            *reinterpret_cast<float2*>(pr.Y + yrow[h] * pr.ldy + col) = make_float2(acc[j][4 * c + 2 * h] + b.x, acc[j][4 * c + 2 * h + 1] + b.y);
         }
       }
     }
@@ -412,7 +417,9 @@ static int wgrad_launch(const WgParams& P, bool split, int mb, bool bf16, cudaSt
 // dY -> dY^T [hi ; lo] ([2d x ldt], hi exactly TF32-representable; [d x ldt] unsplit in mode 1) for every problem of a grouped
 // weight gradient in ONE launch (blockIdx.z): the B operand of the wgrad kernel, K-major (rows of dY contiguous), from strided views.
 // BF16 (the bf16-X kernels): dY^T as bf16 terms [w0 ; w1 ; w2] ([3d x ldt], bf16_split3) or [d x ldt] truncated in mode 1.
-struct DytParams { const float* dY[kMaxProb]; long long ld[kMaxProb]; int n[kMaxProb]; float* out[kMaxProb]; long long ldt[kMaxProb]; int d, split; };
+// rows (optional per problem): column r of dY^T is dY row rows[r], the row that X row r pairs with (the row-mapped weight gradient).
+struct DytParams { const float* dY[kMaxProb]; long long ld[kMaxProb]; int n[kMaxProb]; float* out[kMaxProb]; long long ldt[kMaxProb];
+                   const int* rows[kMaxProb]; int d, split; };
 template <bool BF16>
 __global__ void __launch_bounds__(256) dyt_split_kernel(const DytParams P) {
   __shared__ float tile[32][33];
@@ -420,8 +427,12 @@ __global__ void __launch_bounds__(256) dyt_split_kernel(const DytParams P) {
   if (r0 >= n) return;
   const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
   const float* __restrict__ src = P.dY[p];
+  const int* __restrict__ rows = P.rows[p];
 #pragma unroll
-  for (int i = ty; i < 32; i += 8) tile[i][tx] = r0 + i < n ? __ldg(src + (long long)(r0 + i) * P.ld[p] + e0 + tx) : 0.f;
+  for (int i = ty; i < 32; i += 8) {
+    const int r = r0 + i;
+    tile[i][tx] = r < n ? __ldg(src + (long long)(rows ? __ldg(rows + r) : r) * P.ld[p] + e0 + tx) : 0.f;
+  }
   __syncthreads();
   if (r0 + tx >= n) return;
   const long long ldt = P.ldt[p], lo = (long long)P.d * ldt;
@@ -570,7 +581,8 @@ bool proj_tc_supported(int d, int64_t ldx, const void* X, int k, bool wgrad, boo
 static CUtensorMapDataType x_type(bool bf16) { return bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32; }
 
 // bf16: pr[p].X holds the address of a bf16 table (llmrec_proj_fwd_problem_bf16 carried in the fp32 struct's layout)
-int proj_fwd_tc_group(const llmrec_proj_fwd_problem* pr, int n_prob, int d, int mode, bool bf16, cudaStream_t st) {
+// rows: NULL, or n_prob optional output row maps (X row r of problem p -> Y row rows[p][r])
+int proj_fwd_tc_group(const llmrec_proj_fwd_problem* pr, const int32_t* const* rows, int n_prob, int d, int mode, bool bf16, cudaStream_t st) {
   const bool split = (mode == 0);
   const bool need_ws = split || bf16;          // bf16 kernels read W as bf16 terms in both modes
   const int es = bf16 ? 2 : 4, bk = stage_k(bf16);
@@ -602,6 +614,7 @@ int proj_fwd_tc_group(const llmrec_proj_fwd_problem* pr, int n_prob, int d, int 
     }
     P.prob[p].n = (int)pr[p].n; P.prob[p].k = pr[p].k; P.prob[p].kblocks = (pr[p].k + bk - 1) / bk;
     P.prob[p].tile_start = tiles; P.prob[p].ldy = pr[p].ldy; P.prob[p].Y = pr[p].Y; P.prob[p].bias = pr[p].bias;
+    P.prob[p].rows = rows ? rows[p] : nullptr;
     tiles += (int)((pr[p].n + tm - 1) / tm);
   }
   P.total_tiles = tiles;
@@ -657,8 +670,10 @@ int64_t proj_wgrad_tc_scratch(const llmrec_proj_wgrad_problem* pr, int n_prob, i
 }
 
 // bf16: pr[p].X holds the address of a bf16 table (llmrec_proj_wgrad_problem_bf16 carried in the fp32 struct's layout)
-int proj_wgrad_tc_group(const llmrec_proj_wgrad_problem* pr, int n_prob, int d, int mode, bool bf16, float* scratch, int64_t scratch_elems,
-                        cudaStream_t st) {
+// rows / n_dy: NULL, or per problem an optional dY row map (X row r pairs with dY row rows[p][r]; NULL = identity) and the row count
+// of dY (n without a map), over all of which the bias sums run (the map changes only which dY rows the weight gradient reads)
+int proj_wgrad_tc_group(const llmrec_proj_wgrad_problem* pr, const int32_t* const* rows, const int64_t* n_dy, int n_prob, int d, int mode,
+                        bool bf16, float* scratch, int64_t scratch_elems, cudaStream_t st) {
   const bool split = (mode == 0);
   const int es = bf16 ? 2 : 4, bk = stage_k(bf16), pieces = split ? (bf16 ? 3 : 2) : 1;
   WgPlan W;
@@ -685,9 +700,11 @@ int proj_wgrad_tc_group(const llmrec_proj_wgrad_problem* pr, int n_prob, int d, 
       if (!make_tmap_2d(&P.tmX[p], x_type(bf16), pr[p].X, (uint64_t)pr[p].k, (uint64_t)pr[p].n, (uint64_t)pr[p].ldx * es, bk, bk)) return 4;
       if (!make_tmap_2d(&P.tmG[p], x_type(bf16), dyt, (uint64_t)pr[p].n, (uint64_t)(pieces * d), (uint64_t)W.ldt[p] * es, bk, (uint32_t)d)) return 4;
     }
-    T.dY[p] = pr[p].dY; T.ld[p] = pr[p].lddy; T.n[p] = (int)pr[p].n; T.out[p] = dyt; T.ldt[p] = W.ldt[p];
+    const int32_t* map = rows ? rows[p] : nullptr;
+    T.dY[p] = pr[p].dY; T.ld[p] = pr[p].lddy; T.n[p] = (int)pr[p].n; T.out[p] = dyt; T.ldt[p] = W.ldt[p]; T.rows[p] = map;
     n_max = pr[p].n > n_max ? pr[p].n : n_max;
-    C.dY[p] = pr[p].dY; C.ld[p] = pr[p].lddy; C.n[p] = pr[p].n; C.db[p] = pr[p].db; C.acc[p] = pr[p].accumulate & LLMREC_WGRAD_ACCUMULATE;
+    C.dY[p] = pr[p].dY; C.ld[p] = pr[p].lddy; C.n[p] = n_dy ? n_dy[p] : pr[p].n; C.db[p] = pr[p].db;
+    C.acc[p] = pr[p].accumulate & LLMREC_WGRAD_ACCUMULATE;
   }
   // The bias gradients depend on dY only: colsum runs as a BRANCH beside the weight-gradient kernel -- fork/join through events, so inside a stream capture it becomes a parallel graph branch.
   // The side stream and the two events are per device, created on first use (never during the call that is being captured in practice:

@@ -11,7 +11,8 @@ constexpr int stage_k(bool bf16) { return bf16 ? BK16 : BK; }
 // Tile = 2 consumer warpgroups x MB blocks of wgmma M = 64: 256 rows (fwd) / features (wgrad) when MB = 2, 128 when MB = 1.
 constexpr int tile_m(int mb) { return 128 * mb; }
 
-struct FwdProblem { int n, k, kblocks, tile_start; long long ldy; float* Y; const float* bias; };
+// rows: optional output row map (X row r -> Y row rows[r]); NULL = identity
+struct FwdProblem { int n, k, kblocks, tile_start; long long ldy; float* Y; const float* bias; const int* rows; };
 struct FwdParams {
   CUtensorMap tmA[kMaxProb];  // X [n x k], boxes [TM rows][32 k] (bf16: [TM rows][64 k]), 128-byte swizzle
   CUtensorMap tmW[kMaxProb];  // fp32: [2d x k] (hi rows then lo rows) when SPLIT, [d x k] otherwise; boxes [d][32 k]

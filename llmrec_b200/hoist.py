@@ -31,6 +31,8 @@ from .engine import HotPath, HotPathConfig
 
 
 class HoistedHotPath(HotPath):
+    compact_items = False             # projects gathered rows of the propagated tables, never the full item tables
+
     def __init__(self, operators, params, feats, cfg: HotPathConfig, graph_scalars):
         """graph_scalars: dict(cu, ci, ru, ri) fp32 CUDA vectors = ui.1, iu.ui.1, ui.iu.1, iu.1 (BipartiteGraph.ones_propagated())."""
         super().__init__(operators, params, feats, cfg)

@@ -214,6 +214,7 @@ class Trainer(object):
             for k in m._item_keys:
                 f = getattr(m, "item_feat__" + k)
                 f[i_mask] = f.mean(0)
+            self.hot.refresh_item_feats(i_mask)                           # the compact tables of the live items (engine.HotPath)
         u_mask = torch.randperm(self.n_users)[:int(args.mask_rate * self.n_users)].to(self.device)
         m.user_feats[u_mask] = m.user_feats.mean(0)
         return i_mask, u_mask

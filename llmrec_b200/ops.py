@@ -250,24 +250,50 @@ def _f32(t, name):
     return t
 
 
+def _row_map(rows, n, what):
+    """Optional row map of a projection problem: None, or a contiguous CUDA int32 list of the problem's n X rows."""
+    if rows is not None and (_i32(rows, what + " rows").dim() != 1 or rows.numel() != n):
+        raise ValueError(f"{what}: a row map needs one entry per X row ({n}), got {tuple(rows.shape)}")
+    return rows
+
+
+def _problem_array(prob_type, n, mapped):
+    """ctypes array of n problems; with row maps, followed in the same block by their n llmrec_proj_row_map records (the layout the
+    grouped entry points read when a problem flags LLMREC_PROJ_ROW_MAP).  -> (problems, records | None, block)"""
+    if not mapped:
+        arr = (prob_type * n)()
+        return arr, None, arr
+
+    class Block(C.Structure):
+        _fields_ = [("probs", prob_type * n), ("maps", N.ProjRowMap * n)]
+    blk = Block()
+    return blk.probs, blk.maps, blk
+
+
 def proj_fwd_group(problems, d, mode=0):
-    """problems: list of (X[n x k], W[d x k], bias[d]|None, out[n x d]).  One grouped launch (wgmma) --
+    """problems: list of (X[n x k], W[d x k], bias[d]|None, out[m x d] [, rows]).  One grouped launch (wgmma) --
     the 8 nn.Linear calls of Models.py:145-150.  Problems sharing W share the split buffer.  X is fp32 or bf16 (all problems
-    alike); W, bias and out are fp32."""
-    bf16 = _group_dtype([_feat(X) for X, _, _, _ in problems], "proj_fwd") == torch.bfloat16
-    arr = ((N.ProjFwdProblemBf16 if bf16 else N.ProjFwdProblem) * len(problems))()
-    for i, (X, W, b, out) in enumerate(problems):
+    alike); W, bias and out are fp32.  rows (optional, int32 CUDA [n]): X row r is written to out[rows[r]], the other rows of out
+    are left untouched (without it m == n and row r goes to out[r]); a written row gets the bits of the full-table call."""
+    bf16 = _group_dtype([_feat(pr[0]) for pr in problems], "proj_fwd") == torch.bfloat16
+    arr, recs, _blk = _problem_array(N.ProjFwdProblemBf16 if bf16 else N.ProjFwdProblem, len(problems), any(len(pr) > 4 and pr[4] is not None for pr in problems))
+    for i, (X, W, b, out, *rows) in enumerate(problems):
         _mat(out); _f32(W, "proj_fwd W"); _f32(b, "proj_fwd bias")
         n, k = X.shape
-        if not W.is_contiguous() or tuple(W.shape) != (d, k) or tuple(out.shape) != (n, d):
+        rows = _row_map(rows[0] if rows else None, n, "proj_fwd")
+        if not W.is_contiguous() or tuple(W.shape) != (d, k) or out.shape[1] != d or (rows is None and out.shape[0] != n):
             raise ValueError("proj_fwd: bad shapes")
         # the bf16 kernels read W as bf16 terms in modes 0 and 1: 3dk (or dk) bf16 in the 2dk floats of the fp32 hi/lo split
         ws = _get_scratch(("wsplit", W.data_ptr()), 2 * d * k, X.device) if mode == 0 or (bf16 and mode == 1) else None
-        arr[i] = (N.ProjFwdProblemBf16 if bf16 else N.ProjFwdProblem)(_p(X), _p(W), _p(b), _p(out), _p(ws), _ld(X), _ld(out), n, k, 0)
+        arr[i] = (N.ProjFwdProblemBf16 if bf16 else N.ProjFwdProblem)(_p(X), _p(W), _p(b), _p(out), _p(ws), _ld(X), _ld(out), n, k,
+                                                                        0 if rows is None else N.PROJ_ROW_MAP)
+        if rows is not None:
+            recs[i] = N.ProjRowMap(_p(rows), int(out.shape[0]))
+    lib = N.lib()
     if bf16:
-        N.check(N.lib().llmrec_proj_fwd_group_bf16(arr, len(problems), d, mode, _stream()), "proj_fwd_group_bf16")
+        N.check(lib.llmrec_proj_fwd_group_bf16(arr, len(problems), d, mode, _stream()), "proj_fwd_group_bf16")
     else:
-        N.check(N.lib().llmrec_proj_fwd_group_f32(arr, len(problems), d, mode, _stream()), "proj_fwd_group")
+        N.check(lib.llmrec_proj_fwd_group_f32(arr, len(problems), d, mode, _stream()), "proj_fwd_group")
     _count((2 if mode == 0 or (bf16 and mode == 1) else 1) * -(-len(problems) // 8))
 
 
@@ -278,16 +304,22 @@ def proj_fwd(X, W, b, out, mode=0):
 
 
 def proj_wgrad_group(problems, d, mode=0):
-    """problems: list of (X[n x k], dY[n x d], dW[d x k], db[d]|None, accumulate).  dW (+)= dY^T X ; db (+)= colsum(dY).
-    X is fp32 or bf16 (all problems alike); dY, dW and db are fp32."""
-    bf16 = _group_dtype([_feat(X) for X, _, _, _, _ in problems], "proj_wgrad") == torch.bfloat16
-    arr = ((N.ProjWgradProblemBf16 if bf16 else N.ProjWgradProblem) * len(problems))()
-    for i, (X, dY, dW, db, acc) in enumerate(problems):
+    """problems: list of (X[n x k], dY[m x d], dW[d x k], db[d]|None, accumulate [, rows]).  dW (+)= dY^T X ; db (+)= colsum(dY).
+    X is fp32 or bf16 (all problems alike); dY, dW and db are fp32.  rows (optional, int32 CUDA [n]): X row r pairs with dY[rows[r]]
+    (without it m == n); db still sums all m rows of dY, so it gets the bits of the full-table call, and dW differs from it by rounding."""
+    bf16 = _group_dtype([_feat(pr[0]) for pr in problems], "proj_wgrad") == torch.bfloat16
+    arr, recs, _blk = _problem_array(N.ProjWgradProblemBf16 if bf16 else N.ProjWgradProblem, len(problems),
+                                     any(len(pr) > 5 and pr[5] is not None for pr in problems))
+    for i, (X, dY, dW, db, acc, *rows) in enumerate(problems):
         _mat(dY); _f32(dW, "proj_wgrad dW"); _f32(db, "proj_wgrad db")
         n, k = X.shape
-        if not dW.is_contiguous() or tuple(dW.shape) != (d, k) or tuple(dY.shape) != (n, d):
+        rows = _row_map(rows[0] if rows else None, n, "proj_wgrad")
+        if not dW.is_contiguous() or tuple(dW.shape) != (d, k) or dY.shape[1] != d or (rows is None and dY.shape[0] != n):
             raise ValueError("proj_wgrad: bad shapes")
-        arr[i] = (N.ProjWgradProblemBf16 if bf16 else N.ProjWgradProblem)(_p(X), _p(dY), _p(dW), _p(db), _ld(X), _ld(dY), n, k, 1 if acc else 0)
+        flags = (N.WGRAD_ACCUMULATE if acc else 0) | (0 if rows is None else N.PROJ_ROW_MAP)
+        arr[i] = (N.ProjWgradProblemBf16 if bf16 else N.ProjWgradProblem)(_p(X), _p(dY), _p(dW), _p(db), _ld(X), _ld(dY), n, k, flags)
+        if rows is not None:
+            recs[i] = N.ProjRowMap(_p(rows), int(dY.shape[0]))
     lib = N.lib()
     need = int((lib.llmrec_proj_wgrad_group_bf16_scratch if bf16 else lib.llmrec_proj_wgrad_group_scratch)(arr, len(problems), d, mode))
     scratch = _get_scratch(("wgrad", problems[0][0].device.index), need, problems[0][0].device, zero=True) if need else None     # holds a ticket word

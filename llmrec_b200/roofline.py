@@ -32,7 +32,8 @@ def step_bytes(hp, nnz):
     out = {}
     if hp.has_feats:
         f = hp.feats
-        gemms = [(ni, f["image"].shape[1]), (ni, f["text"].shape[1])] + [(ni, v.shape[1]) for v in f["item"].values()] + [(nu, f["user"].shape[1])]
+        nl = getattr(hp, "n_live", ni)         # the item-side problems read the live items' rows only (engine.HotPath._build_live_items)
+        gemms = [(nl, f["image"].shape[1]), (nl, f["text"].shape[1])] + [(nl, v.shape[1]) for v in f["item"].values()] + [(nu, f["user"].shape[1])]
         xb = f["image"].element_size()
         out["proj_fwd"] = out["proj_wgrad"] = sum(proj_bytes(n, k, d, xb) for n, k in gemms)
     sp = lambda M, N, segs: spmm_bytes(nnz, M, N, d, segs)
