@@ -207,9 +207,11 @@ typedef struct {
  * d x_t (+)= coef[t] * (g - y_t (y_t . g)) / max(||x_t||,1e-12),  y_t = x_t/max(||x_t||,1e-12).
  * Pointer tables are HOST arrays (copied into the launch parameters).
  * --------------------------------------------------------------------------------------------- */
-/* rows: optional int32 device list of row ids to process (NULL = rows 0..n-1; n = list length otherwise).
+/* rows: optional int32 device list of row ids to process (NULL = rows 0..n-1; n = list length otherwise).  Entries < 0 are skipped:
+ * nothing is read or written for them, forward and backward.
  * llmrec_fuse_fwd_f32 with rows != NULL and n < 0: COMPACT form over |n| list entries -- the layer tables are read at rows[b], the
- * side operands and `out` at the compact position b (side features projected on the batch's rows only, hoisted mode). */
+ * side operands and `out` at the compact position b (side features projected on the batch's rows only, hoisted mode); a negative
+ * entry gives a zero row of `out`. */
 int llmrec_fuse_fwd_f32(const float* const* layers_host, const int64_t* ld_layers_host, int32_t n_layers,
                         const float* const* sides_host, const int64_t* ld_sides_host, const float* coef_host,
                         int32_t n_sides, float* out, int64_t ldo, const int32_t* rows, int64_t n, int32_t d,

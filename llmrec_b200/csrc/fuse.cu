@@ -96,8 +96,10 @@ __global__ void __launch_bounds__(256) fuse_bwd_kernel(const FuseParams p) {
   __shared__ float sb[8][RPW][kMaxSides];
   const int wib = threadIdx.x >> 5, lane = threadIdx.x & 31, sub = lane / LPR, li = lane % LPR;
   const int64_t item = ((int64_t)blockIdx.x * 8 + wib) * RPW + sub;
-  const bool valid = item < live_rows(p);
-  const int64_t row = valid ? (p.rows ? (int64_t)p.rows[item] : item) : 0;
+  const bool in_range = item < live_rows(p);
+  const int64_t lrow = in_range ? (p.rows ? (int64_t)p.rows[item] : item) : 0;
+  const bool valid = in_range && lrow >= 0;          // a negative list entry = "not mine", as in the forward: nothing read or written
+  const int64_t row = valid ? lrow : 0;
   const int nq = VEC ? p.d / 4 : p.d;
   const float* g = p.g + row * p.ldg;
   for (int t = 0; t < p.n_sides; ++t) {

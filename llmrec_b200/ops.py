@@ -384,7 +384,8 @@ def fuse_fwd(layers, sides, coefs, out, rows=None, compact=False, count=None, ma
 
 
 def fuse_bwd(g, n_layers, d_layer, sides, coefs, d_sides, accumulate, rows=None, count=None, max_rows=None):
-    """count: as for fuse_fwd; a row listed twice would be processed twice (accumulate=True adds twice): pass a set (RowSet.list)."""
+    """count: as for fuse_fwd; a row listed twice would be processed twice (accumulate=True adds twice): pass a set (RowSet.list).
+    Negative entries of `rows` are skipped, as in the forward."""
     _mat(g)
     cf = (C.c_float * max(1, len(coefs)))(*[float(c) for c in coefs])
     dl = (_p(d_layer), _ld(d_layer) if d_layer is not None else 0)
@@ -606,8 +607,19 @@ def scaled_colsum(terms, out, accumulate=False):
 
 
 def feat_reg_gram(W, b, G, h, n2, c, dW, db, loss):
-    """feat_reg over all rows through the Gram matrix G[k x k] of a propagated table (include/llmrec_b200.h)."""
+    """feat_reg over all rows through the Gram matrix G[k x k] of a propagated table (include/llmrec_b200.h).
+    The kernels read W, G and dW as dense row-major blocks and b, h, db as unit-stride vectors."""
+    if W.dim() != 2:
+        raise ValueError(f"feat_reg_gram: W must be 2-D, got {tuple(W.shape)}")
     d, k = W.shape
+    for name, t, shape in (("W", W, (d, k)), ("G", G, (k, k)), ("dW", dW, (d, k)), ("b", b, (d,)), ("db", db, (d,)), ("h", h, (k,)),
+                           ("loss", loss, None)):
+        if t is None and name in ("b", "db", "h", "loss"):
+            continue
+        if t is None or t.dtype != torch.float32 or not t.is_cuda or not t.is_contiguous() or (shape is not None and tuple(t.shape) != shape) \
+                or (shape is None and t.numel() < 1):
+            got = "None" if t is None else f"{tuple(t.shape)} {t.dtype} {t.device} strides {t.stride()}"
+            raise ValueError(f"feat_reg_gram: {name} must be a contiguous CUDA fp32 tensor of shape {shape or '[>= 1]'}, got {got}")
     key = ("gram", W.device.index, d, k)
     sc_ = _scratch.get(key)
     if sc_ is None:
