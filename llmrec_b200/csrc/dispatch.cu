@@ -12,7 +12,7 @@ int score_topk_simt(const float*, int64_t, const float*, int64_t, const int*, in
 bool proj_tc_supported(int d, int64_t ldx, const void* X, int k, bool wgrad, bool bf16);
 int proj_fwd_tc_group(const llmrec_proj_fwd_problem*, const int32_t* const*, int, int, int, bool, cudaStream_t);
 int proj_wgrad_tc_group(const llmrec_proj_wgrad_problem*, const int32_t* const*, const int64_t*, int, int, int, bool, float*, int64_t, cudaStream_t);
-int64_t proj_wgrad_tc_scratch(const llmrec_proj_wgrad_problem*, int, int, bool);
+int64_t proj_wgrad_tc_scratch(const llmrec_proj_wgrad_problem*, int, int, int, bool);
 bool score_tc_supported(int d, int K, long long ldu, long long ldi, const void* U, const void* I);
 long long score_tc_scratch(int n_batch, int n_items, int d, int K);
 int score_topk_tc(const float*, long long, const float*, long long, const int*, int, int, int, const int*, const int*, int, int*, float*, float*, long long, cudaStream_t);
@@ -113,7 +113,7 @@ static int64_t proj_wgrad_scratch(const llmrec_proj_wgrad_problem* pr, int32_t n
   int64_t need = 0;
   for (int p0 = 0; p0 < n_prob; p0 += 8) {
     int np = n_prob - p0 < 8 ? n_prob - p0 : 8;
-    if (wg_tc_ok(pr + p0, np, d, mode, bf16)) { int64_t s = proj_wgrad_tc_scratch(pr + p0, np, d, bf16); need = s > need ? s : need; }
+    if (wg_tc_ok(pr + p0, np, d, mode, bf16)) { int64_t s = proj_wgrad_tc_scratch(pr + p0, np, d, mode, bf16); need = s > need ? s : need; }
   }
   return need;
 }
@@ -174,7 +174,7 @@ extern "C" int64_t llmrec_proj_wgrad_scratch(int64_t n, int32_t k, int32_t d, in
   llmrec_proj_wgrad_problem p{nullptr, nullptr, nullptr, nullptr, 4, 4, n, k, 0};
   // alignment of real pointers is checked at call time; size the scratch for the tensor-core path
   if (mode == 2 || d % 32 != 0 || d > 256 || k % 4 != 0) return 0;
-  return proj_wgrad_tc_scratch(&p, 1, d, false);
+  return proj_wgrad_tc_scratch(&p, 1, d, mode, false);
 }
 extern "C" int llmrec_proj_wgrad_f32(const float* X, int64_t ldx, const float* dY, int64_t lddy, float* dW, float* db,
                                      int64_t n, int32_t k, int32_t d, int32_t accumulate, int32_t mode,

@@ -15,8 +15,10 @@
 // CTA = 3 warpgroups.  Warpgroup 0 is the producer: one thread keeps a ring of TMA stages in flight (a full and an empty
 // mbarrier per stage), running ahead across work units; it hands most of its registers to the two consumer warpgroups
 // (setmaxnreg).  Each consumer owns MB blocks of 64 rows (fwd) / features (wgrad) of the tile.  X goes into wgmma A-fragment
-// REGISTERS straight from the stage and is split there; B (W or dY^T, hi and lo) is consumed from shared memory as it arrived
-// from TMA, ready-made: W is split once per step by `wsplit`, dY^T is transposed and split once per step by `dyt_split`.  One
+// REGISTERS straight from the stage and is split there; B (W or dY^T, hi and lo) is consumed from shared memory.  W arrives from
+// TMA ready-made, split once per step by `wsplit`.  The fp32 3xTF32 weight gradient builds dY^T hi / lo in the kernel: the
+// producer's warps 1..3 gather the stage's dY rows (through the row map), split them and store them in the swizzled layout TMA
+// would give, so dY^T never goes through HBM (WgUnit::build).  bf16 X and mode 1 read dY^T from `dyt_split` by TMA.  One
 // wgmma group (one k8 step) stays in flight while the next A fragment is loaded; no CTA-wide barrier in the main loop.
 //   forward  A = X[rows][k]: the X tile [TM rows][32 k] arrives K-major with the 128-byte swizzle, exactly the A layout.
 //   wgrad    A = X^T (M = features, K = rows): the fragment is read transposed out of the raw X tile, which arrives as TM/32
@@ -91,7 +93,6 @@ __device__ __forceinline__ uint8_t* align1024(uint8_t* p) {
 // one main loop for both directions
 // ------------------------------------------------------------------------------------------------
 constexpr uint32_t kSmemMax = 227u * 1024u;   // dynamic shared memory per block on sm_90
-constexpr int kProducerRegs = 40, kConsumerRegs = 232;   // 128 * 40 + 256 * 232 <= 65536 (launched at 384 x 168)
 
 // BF16: X is a bf16 table.  A stage then covers 64 k (fwd) / rows (wgrad) in the same bytes, and a 3-way split of the fp32
 // operand (W or dY^T) gives three B tiles instead of two.
@@ -144,6 +145,9 @@ template <int D, bool SPLIT, int MB, bool BF16 = false>
 struct FwdUnit {
   using Cfg = ProjCfg<D, SPLIT, MB, BF16>;
   static constexpr int kTransA = 0;   // bf16: A = the X tile as it arrived, K-major
+  static constexpr int kBuilders = 0;            // warps that build B in the kernel: none, W arrives by TMA
+  static constexpr int kProducerRegs = 40, kConsumerRegs = 232;   // setmaxnreg: 128 * 40 + 256 * 232 = 384 * 168
+  static constexpr uint32_t kTx = Cfg::kStage;   // TMA bytes per stage: X and W
   const FwdParams& P; int p, mblk, kb_n;
   __device__ FwdUnit(const FwdParams& P_, int u) : P(P_) {
     p = 0;
@@ -201,6 +205,12 @@ struct WgUnit {
     r0 = chunk * pr.rows_per_chunk;
     kb_n = (min(pr.n, r0 + pr.rows_per_chunk) - r0 + kBk - 1) / kBk;   // chunks are stage-aligned; rows past n load as zeros
   }
+  // fp32 X, 3xTF32: producer warps 1..3 build B from dY (below).  bf16 X and mode 1 keep B = dY^T by TMA from `dyt_split`: their
+  // consumers finish a stage sooner than three warps build one, measured slower at the netflix and movielens shapes (H100 SXM, 700 W).
+  static constexpr int kBuilders = SPLIT && !BF16 ? 3 : 0;
+  static constexpr int kProducerRegs = kBuilders ? 72 : 40;     // 128 * 72 + 256 * 216 = 384 * 168: the builders' loads in flight
+  static constexpr int kConsumerRegs = kBuilders ? 216 : 232;
+  static constexpr uint32_t kTx = kBuilders ? Cfg::kX : Cfg::kStage;   // TMA bytes per stage: X, and B without builders
   __device__ void issue(uint8_t* st, uint64_t* bar, int kb, uint64_t pol) const {
     const int r = r0 + kb * kBk;
     if constexpr (BF16) {   // TM/64 boxes [64 rows][64 features], 8 KiB each: one per m64 block
@@ -210,8 +220,47 @@ struct WgUnit {
 #pragma unroll
       for (int b = 0; b < Cfg::TM / 32; ++b) tma_load_2d_hint(st + b * 4096, &P.tmX[p], bar, ft * Cfg::TM + 32 * b, r, pol);
     }
+    if constexpr (kBuilders == 0) {
 #pragma unroll
-    for (int i = 0; i < Cfg::NB; ++i) tma_load_2d(st + Cfg::kX + i * Cfg::kB, &P.tmG[p], bar, r, i * D);
+      for (int i = 0; i < Cfg::NB; ++i) tma_load_2d(st + Cfg::kX + i * Cfg::kB, &P.tmG[p], bar, r, i * D);
+    }
+  }
+  // B of stage kb = dY^T over the stage's kBk rows, split into hi and lo, written by builder warp bw (0 .. kBuilders-1) in the layout
+  // TMA gives a [D][32] box with the 128-byte swizzle: element (column c, stage row j) at c*128 + ((j/4 ^ c) % 8)*16 + (j%4)*4.  Lane l owns
+  // stage row l, so it reads its dY row through the row map once; a task is 8 columns (32 bytes of the row, two 16-byte loads),
+  // the warps take every kBuilders-th task.  Each store of a warp writes one column c: chunk (l/4 ^ c) % 8, word l%4 -- 32
+  // distinct banks, no conflict.  Rows at or past n are zeros, as TMA fills them.
+  static constexpr int kTasks = D / 8;
+  static constexpr int kBatch = 3;                   // tasks per thread whose loads are in flight together (24 floats)
+  __device__ void build(uint8_t* st, int kb, int bw, int lane) const {
+    const int n = P.prob[p].n, r = r0 + kb * kBk + lane;
+    const int* __restrict__ map = P.rows[p];
+    const float* src = r < n ? P.dY[p] + (long long)(map ? __ldg(map + r) : r) * P.lddy[p] : nullptr;
+    uint8_t* b = st + Cfg::kX + (lane & 3) * 4;
+    const int q = lane >> 2;
+    for (int t0 = bw; t0 < kTasks; t0 += kBuilders * kBatch) {
+      float4 v[kBatch][2];
+#pragma unroll
+      for (int j = 0; j < kBatch; ++j) {
+        const int t = t0 + kBuilders * j;
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+          v[j][h] = t < kTasks && src ? __ldg(reinterpret_cast<const float4*>(src + 8 * t + 4 * h)) : make_float4(0.f, 0.f, 0.f, 0.f);
+      }
+#pragma unroll
+      for (int j = 0; j < kBatch; ++j) {
+        const int t = t0 + kBuilders * j;
+        if (t >= kTasks) break;
+#pragma unroll
+        for (int e = 0; e < 8; ++e) {
+          const float4 w = v[j][e >> 2];
+          const float x = (e & 3) == 0 ? w.x : (e & 3) == 1 ? w.y : (e & 3) == 2 ? w.z : w.w, hi = tf32_hi(x);
+          uint8_t* o = b + (8 * t + e) * 128 + ((q ^ e) & 7) * 16;
+          *reinterpret_cast<float*>(o) = hi;
+          *reinterpret_cast<float*>(o + Cfg::kB) = x - hi;
+        }
+      }
+    }
   }
   static __device__ void ld_frag(uint32_t (&a)[4], uint32_t sx, int blk, int kk, int warp, int lane) { ld_frag_wgrad(a, sx, blk, kk, warp, lane); }
   // bf16: descriptor of m64 block `blk` (its own box), k16 step kk = rows 16kk .. 16kk + 15 (+2048 bytes)
@@ -240,13 +289,17 @@ __device__ __forceinline__ void proj_pipeline(const Params& P, int total) {
   uint64_t* empty = full + Cfg::kStages;
   const int tid = threadIdx.x, wg = tid >> 7, warp = (tid >> 5) & 3, lane = tid & 31;
   if (tid == 0) {
-    for (int s = 0; s < Cfg::kStages; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 8); }   // empty: one arrival per consumer warp
+    // full: the TMA thread's arrive (+ transaction bytes) and, when the kernel builds B, one arrival per builder warp;
+    // empty: one arrival per consumer warp
+    for (int s = 0; s < Cfg::kStages; ++s) { mbar_init(&full[s], 1 + Unit::kBuilders); mbar_init(&empty[s], 8); }
     fence_barrier_init();
   }
   __syncthreads();
 
-  if (wg == 0) {   // producer warpgroup: one thread issues every load, across work units
-    setmaxnreg_dec<kProducerRegs>();
+  // the CTA holds 384 x 168 registers (launch bounds): a larger split would block the consumers' setmaxnreg.inc for good
+  static_assert(128 * Unit::kProducerRegs + 256 * Unit::kConsumerRegs <= 384 * 168, "setmaxnreg split exceeds the CTA's registers");
+  if (wg == 0) {   // producer warpgroup: one thread issues every load, across work units; wgrad: warps 1..3 build B
+    setmaxnreg_dec<Unit::kProducerRegs>();
     if (tid == 0) {
       const uint64_t pol = l2_policy_evict_first();
       int s = 0; uint32_t ph = 0;
@@ -254,16 +307,32 @@ __device__ __forceinline__ void proj_pipeline(const Params& P, int total) {
         const Unit w(P, u);
         for (int kb = 0; kb < w.kb_n; ++kb) {
           mbar_wait(&empty[s], ph ^ 1u);
-          mbar_arrive_expect_tx(&full[s], Cfg::kStage);
+          mbar_arrive_expect_tx(&full[s], Unit::kTx);
           w.issue(smem + s * Cfg::kStage, &full[s], kb, pol);
           if (++s == Cfg::kStages) { s = 0; ph ^= 1u; }
+        }
+      }
+    }
+    if constexpr (Unit::kBuilders > 0) {
+      if (warp >= 1) {
+        int s = 0; uint32_t ph = 0;
+        for (int u = blockIdx.x; u < total; u += gridDim.x) {
+          const Unit w(P, u);
+          for (int kb = 0; kb < w.kb_n; ++kb) {
+            mbar_wait(&empty[s], ph ^ 1u);
+            w.build(smem + s * Cfg::kStage, kb, warp - 1, lane);
+            fence_proxy_async_smem();   // the generic-proxy stores -> visible to wgmma
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&full[s]);
+            if (++s == Cfg::kStages) { s = 0; ph ^= 1u; }
+          }
         }
       }
     }
     return;
   }
 
-  setmaxnreg_inc<kConsumerRegs>();
+  setmaxnreg_inc<Unit::kConsumerRegs>();
   const int cw = wg - 1;   // consumer warpgroup 0 / 1
   int s = 0; uint32_t ph = 0;
   float acc[MB][D / 2];
@@ -414,7 +483,7 @@ static int wgrad_launch(const WgParams& P, bool split, int mb, bool bf16, cudaSt
   return 1;
 }
 
-// dY -> dY^T [hi ; lo] ([2d x ldt], hi exactly TF32-representable; [d x ldt] unsplit in mode 1) for every problem of a grouped
+// dY -> dY^T ([d x ldt] unsplit in mode 1; the 3xTF32 fp32 kernels build their B in the kernel) for every problem of a grouped
 // weight gradient in ONE launch (blockIdx.z): the B operand of the wgrad kernel, K-major (rows of dY contiguous), from strided views.
 // BF16 (the bf16-X kernels): dY^T as bf16 terms [w0 ; w1 ; w2] ([3d x ldt], bf16_split3) or [d x ldt] truncated in mode 1.
 // rows (optional per problem): column r of dY^T is dY row rows[r], the row that X row r pairs with (the row-mapped weight gradient).
@@ -435,19 +504,18 @@ __global__ void __launch_bounds__(256) dyt_split_kernel(const DytParams P) {
   }
   __syncthreads();
   if (r0 + tx >= n) return;
-  const long long ldt = P.ldt[p], lo = (long long)P.d * ldt;
+  const long long ldt = P.ldt[p];
 #pragma unroll
   for (int i = ty; i < 32; i += 8) {
     const float v = tile[tx][i];
     const long long at = (long long)(e0 + i) * ldt + r0 + tx;
     if constexpr (BF16) {
       uint16_t* o = reinterpret_cast<uint16_t*>(P.out[p]) + at;
+      const long long lo = (long long)P.d * ldt;
       if (P.split) bf16_split3(v, o[0], o[lo], o[2 * lo]);
       else o[0] = bf16_bits(bf16_trunc(v));
     } else {
-      float* o = P.out[p] + at;
-      if (P.split) { const float h = tf32_hi(v); o[0] = h; o[lo] = v - h; }
-      else o[0] = v;
+      P.out[p][at] = v;
     }
   }
 }
@@ -634,10 +702,11 @@ static int wg_rows_per_chunk(int64_t n) {
 }
 
 // Work plan of a grouped weight gradient, shared by the scratch query and the launch.  Scratch layout (floats):
-//   [colsum ticket: 4] [partials: items x tm x d] [colsum partials: n_prob x kColsumSlices x d] [per problem dY^T hi, lo: 2 x d x ldt]
-// (bf16 X: the three bf16 terms of dY^T, 3 x d x ldt bf16, in the same 2 x d x ldt floats)
+//   [colsum ticket: 4] [partials: items x tm x d] [colsum partials: n_prob x kColsumSlices x d] [per problem dY^T: 2 x d x ldt]
+// The last region only when `dyt_split` makes B: bf16 X (three bf16 terms, 3 x d x ldt bf16) or mode 1 (d x ldt floats).
 struct WgPlan { WgProblem prob[kMaxProb]; int items, mb, tm; int64_t ldt[kMaxProb], dyt[kMaxProb], colsum, total; };
-static void wg_plan(const llmrec_proj_wgrad_problem* pr, int n_prob, int d, bool bf16, WgPlan& W) {
+static bool wg_builds_b(int mode, bool bf16) { return mode == 0 && !bf16; }   // WgUnit::kBuilders > 0
+static void wg_plan(const llmrec_proj_wgrad_problem* pr, int n_prob, int d, int mode, bool bf16, WgPlan& W) {
   long long items256 = 0;
   for (int p = 0; p < n_prob; ++p) {
     const int rpc = wg_rows_per_chunk(pr[p].n);
@@ -658,14 +727,14 @@ static void wg_plan(const llmrec_proj_wgrad_problem* pr, int n_prob, int d, bool
   for (int p = 0; p < n_prob; ++p) {
     W.ldt[p] = bf16 ? (pr[p].n + 7) & ~int64_t(7) : (pr[p].n + 3) & ~int64_t(3);   // TMA row pitch: a multiple of 16 bytes
     W.dyt[p] = off;
-    off += 2 * (int64_t)d * W.ldt[p];
+    if (!wg_builds_b(mode, bf16)) off += 2 * (int64_t)d * W.ldt[p];
   }
   W.total = off;
 }
 
-int64_t proj_wgrad_tc_scratch(const llmrec_proj_wgrad_problem* pr, int n_prob, int d, bool bf16) {
+int64_t proj_wgrad_tc_scratch(const llmrec_proj_wgrad_problem* pr, int n_prob, int d, int mode, bool bf16) {
   WgPlan W;
-  wg_plan(pr, n_prob, d, bf16, W);
+  wg_plan(pr, n_prob, d, mode, bf16, W);
   return W.total;   // the colsum ticket must start at zero; the kernel re-zeroes it
 }
 
@@ -676,8 +745,9 @@ int proj_wgrad_tc_group(const llmrec_proj_wgrad_problem* pr, const int32_t* cons
                         bool bf16, float* scratch, int64_t scratch_elems, cudaStream_t st) {
   const bool split = (mode == 0);
   const int es = bf16 ? 2 : 4, bk = stage_k(bf16), pieces = split ? (bf16 ? 3 : 2) : 1;
+  const bool build_b = wg_builds_b(mode, bf16);
   WgPlan W;
-  wg_plan(pr, n_prob, d, bf16, W);
+  wg_plan(pr, n_prob, d, mode, bf16, W);
   LLMREC_CHECK_ARG(scratch && scratch_elems >= W.total, "proj_wgrad: scratch too small (%lld < %lld)", (long long)scratch_elems, (long long)W.total);
   WgParams P;
   memset(&P, 0, sizeof(P));
@@ -693,14 +763,16 @@ int proj_wgrad_tc_group(const llmrec_proj_wgrad_problem* pr, const int32_t* cons
   int64_t n_max = 0;
   for (int p = 0; p < n_prob; ++p) {
     P.prob[p] = W.prob[p];
+    const int32_t* map = rows ? rows[p] : nullptr;
     float* dyt = scratch + W.dyt[p];
     // an empty problem has no work items (and a tensor map cannot have an empty dimension); colsum and the reduce still
     // write its dW / db: zeros, or the prior under accumulate
     if (pr[p].n > 0) {
       if (!make_tmap_2d(&P.tmX[p], x_type(bf16), pr[p].X, (uint64_t)pr[p].k, (uint64_t)pr[p].n, (uint64_t)pr[p].ldx * es, bk, bk)) return 4;
-      if (!make_tmap_2d(&P.tmG[p], x_type(bf16), dyt, (uint64_t)pr[p].n, (uint64_t)(pieces * d), (uint64_t)W.ldt[p] * es, bk, (uint32_t)d)) return 4;
+      if (!build_b &&
+          !make_tmap_2d(&P.tmG[p], x_type(bf16), dyt, (uint64_t)pr[p].n, (uint64_t)(pieces * d), (uint64_t)W.ldt[p] * es, bk, (uint32_t)d)) return 4;
     }
-    const int32_t* map = rows ? rows[p] : nullptr;
+    P.dY[p] = pr[p].dY; P.lddy[p] = pr[p].lddy; P.rows[p] = map;
     T.dY[p] = pr[p].dY; T.ld[p] = pr[p].lddy; T.n[p] = (int)pr[p].n; T.out[p] = dyt; T.ldt[p] = W.ldt[p]; T.rows[p] = map;
     n_max = pr[p].n > n_max ? pr[p].n : n_max;
     C.dY[p] = pr[p].dY; C.ld[p] = pr[p].lddy; C.n[p] = n_dy ? n_dy[p] : pr[p].n; C.db[p] = pr[p].db;
@@ -738,10 +810,12 @@ int proj_wgrad_tc_group(const llmrec_proj_wgrad_problem* pr, const int32_t* cons
     if (forked) LLMREC_CHECK_CUDA(cudaEventRecord(ev_join, side));
   }
   if (W.items > 0) {   // no items: every problem is empty, and only colsum and the reduce run
-    const dim3 grid((unsigned)((n_max + 31) / 32), (unsigned)(d / 32), (unsigned)n_prob);
-    if (bf16) dyt_split_kernel<true><<<grid, 256, 0, st>>>(T);
-    else dyt_split_kernel<false><<<grid, 256, 0, st>>>(T);
-    LLMREC_CHECK_LAUNCH("dyt_split");
+    if (!build_b) {
+      const dim3 grid((unsigned)((n_max + 31) / 32), (unsigned)(d / 32), (unsigned)n_prob);
+      if (bf16) dyt_split_kernel<true><<<grid, 256, 0, st>>>(T);
+      else dyt_split_kernel<false><<<grid, 256, 0, st>>>(T);
+      LLMREC_CHECK_LAUNCH("dyt_split");
+    }
     int rc = wgrad_launch(P, split, W.mb, bf16, st);
     if (rc) return rc;
   }

@@ -24,8 +24,10 @@ struct FwdParams {
 struct WgProblem { int n, k, ft_tiles, chunks, rows_per_chunk, item_start; };
 struct WgParams {
   CUtensorMap tmX[kMaxProb];  // X [n x k], boxes [32 rows][32 features] (bf16: [64 rows][64 features]), 128-byte swizzle
-  CUtensorMap tmG[kMaxProb];  // dY^T [2d x n] (hi rows then lo rows) when SPLIT, [d x n] otherwise; boxes [d][32 rows]
-                              // bf16: [3d x n] (three bf16 terms) when SPLIT, [d x n] otherwise; boxes [d][64 rows]
+  CUtensorMap tmG[kMaxProb];  // bf16 X or mode 1: dY^T from dyt_split, [d x n] (bf16 split: [3d x n] bf16 terms); boxes [d][32 | 64 rows]
+  const float* dY[kMaxProb];  // dY [m x d] with row stride lddy; fp32 X in mode 0: the kernel builds B (dY^T hi, lo) from it
+  long long lddy[kMaxProb];
+  const int* rows[kMaxProb];  // optional dY row map: X row r pairs with dY row rows[r]; NULL = identity
   WgProblem prob[kMaxProb];
   int n_prob, total_items, d;
   float* partial;  // [total_items][TM][d]
