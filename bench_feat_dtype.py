@@ -1,12 +1,12 @@
-"""bench_feat_dtype.py -- fp32 vs bf16 side-feature tables (--feat_dtype) on one H100.
+"""bench_feat_dtype.py -- fp32 vs bf16 (vs int8) side-feature tables (--feat_dtype) on one H100.
 
-    python bench_feat_dtype.py --steps 50 --blocks 5 --runs 3
+    python bench_feat_dtype.py --steps 50 --blocks 5 --runs 3 [--dtypes fp32,bf16,int8]
 
-For the netflix-shaped (d = 64) and movielens-shaped (d = 128, L = 3) workloads of bench.py, the fp32 and bf16 legs run
-ALTERNATELY in one process (fp32, bf16, fp32, bf16, ...), each on a fresh Trainer with the same seed, so clock and thermal drift
-hit both alike.  Every leg reports ms/step (median of --blocks blocks of --steps device-resident steps, min and max), the
-proj_fwd / proj_wgrad family times with GB/s from roofline's algorithmic bytes, the resident feature bytes, eval users/s and the
-leg's Recall@20 / NDCG@20.  One JSON line on stdout; a summary table on stderr.  Needs a CUDA device (no fallback).
+For the netflix-shaped (d = 64) and movielens-shaped (d = 128, L = 3) workloads of bench.py, the legs of --dtypes (default fp32,bf16)
+run ALTERNATELY in one process (fp32, bf16, fp32, bf16, ...), each on a fresh Trainer with the same seed, so clock and thermal drift
+hit all alike.  Every leg reports ms/step (median of --blocks blocks of --steps device-resident steps, min and max), the
+proj_fwd / proj_wgrad family times with GB/s from roofline's algorithmic bytes, the resident feature bytes (an int8 table's row
+scales and padding included), eval users/s and the leg's Recall@20 / NDCG@20 (bf16 and int8 legs train on rounded tables).  One JSON line on stdout; a summary table on stderr.  Needs a CUDA device (no fallback).
 """
 from __future__ import annotations
 
@@ -71,11 +71,15 @@ def main():
     ap.add_argument("--steps", type=int, default=50, help="steps per timed block")
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--blocks", type=int, default=5, help="timed blocks per leg (the median is reported)")
-    ap.add_argument("--runs", type=int, default=3, help="alternating fp32 / bf16 runs per workload")
+    ap.add_argument("--runs", type=int, default=3, help="alternating runs of the --dtypes legs per workload")
+    ap.add_argument("--dtypes", default="fp32,bf16", help="comma-separated --feat_dtype legs, run in this order (fp32 first: speedups are vs fp32)")
     ap.add_argument("--workloads", default="netflix,movielens")
     ap.add_argument("--proj_mode", default="3xtf32")
     ap.add_argument("--graph", type=int, default=1)
     c = ap.parse_args()
+    dtypes = c.dtypes.split(",")
+    if not dtypes or any(dt not in ("fp32", "bf16", "int8") for dt in dtypes) or len(set(dtypes)) != len(dtypes):
+        raise SystemExit(f"--dtypes: a list of distinct fp32 / bf16 / int8, got {c.dtypes!r}")
     import torch
     if not torch.cuda.is_available():
         raise SystemExit("bench_feat_dtype.py needs a CUDA (H100) device")
@@ -83,15 +87,18 @@ def main():
                               steps=c.steps, warmup=max(c.warmup, 3), blocks=c.blocks)
     name, limit = card()
     result = {"metric": "feat_dtype_ab", "gpu": name, "power_limit": limit, "proj_mode": c.proj_mode, "cuda_graph": bool(c.graph),
-              "timing": f"median of {c.blocks} blocks of {c.steps} device-resident steps per leg; legs alternate fp32 / bf16", "workloads": {}}
+              "timing": f"median of {c.blocks} blocks of {c.steps} device-resident steps per leg; legs alternate {' / '.join(dtypes)}", "workloads": {}}
     for wl in c.workloads.split(","):
-        runs = {"fp32": [], "bf16": []}
+        runs = {dt: [] for dt in dtypes}
         for _ in range(c.runs):
-            for dt in ("fp32", "bf16"):
+            for dt in dtypes:
                 runs[dt].append(leg(wl, dt, a))
         summary = {dt: {k: _median([r[k] for r in rs]) for k in ("ms_per_step", "proj_fwd_ms", "proj_wgrad_ms", "eval_users_per_sec")}
                    for dt, rs in runs.items()}
-        summary["speedup_ms_per_step"] = round(summary["fp32"]["ms_per_step"] / summary["bf16"]["ms_per_step"], 3)
+        if dtypes == ["fp32", "bf16"]:
+            summary["speedup_ms_per_step"] = round(summary["fp32"]["ms_per_step"] / summary["bf16"]["ms_per_step"], 3)
+        elif len(dtypes) > 1:
+            summary["speedup_ms_per_step"] = {dt: round(summary[dtypes[0]]["ms_per_step"] / summary[dt]["ms_per_step"], 3) for dt in dtypes[1:]}
         result["workloads"][wl] = {"workload": bench.workload_string(wl), "runs": runs, "median_of_runs": summary}
         for dt, rs in runs.items():
             for r in rs:

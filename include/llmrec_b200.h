@@ -7,7 +7,8 @@
  * cudaStream_t.  No torch types.  Conventions:
  *   - every pointer is a DEVICE pointer unless the name ends in _host;
  *   - all matrices are row-major fp32 with an explicit leading dimension (elements), except the side-feature table X of the
- *     _bf16 projection entry points: raw bfloat16 bits (uint16_t), row-major, leading dimension in elements;
+ *     _bf16 projection entry points: raw bfloat16 bits (uint16_t), row-major, leading dimension in elements; and of the _i8
+ *     entry points: the row-scaled int8 format described there, row pitch in bytes;
  *   - index arrays are int32 (CSR rowptr/col; nnz < 2^31) unless stated;
  *   - nothing is allocated, nothing synchronises the host; work is enqueued on `stream`;
  *   - return 0 on success, non-zero on error; llmrec_last_error() gives the message
@@ -183,9 +184,39 @@ int llmrec_proj_wgrad_group_bf16(const llmrec_proj_wgrad_problem_bf16* probs_hos
                                  int64_t scratch_elems, llmrec_stream_t stream);
 int64_t llmrec_proj_wgrad_group_bf16_scratch(const llmrec_proj_wgrad_problem_bf16* probs_host, int32_t n_prob, int32_t d, int32_t mode);
 
+/* int8 feature tables (--feat_dtype int8): the same grouped projections with X in a row-scaled 8-bit format.  Row r of a table with
+ * logical width k is ldx BYTES long (the row pitch; at least roundup(k, 16) + 4 and a multiple of 4, roundup(k, 16) + 16 as built by
+ * llmrec_b200/feat_int8.py) and holds
+ *   bytes [0, k)                       the int8 values q (|q| <= 127),
+ *   bytes [k, roundup(k, 16))          zero,
+ *   bytes [roundup(k, 16), +4)         the row's fp32 scale 2^e, e in [-126, 120] (1 for an all-zero row),
+ *   the rest of the row                zero.
+ * Every stored value x~ = q * 2^e is exactly a bf16 number, so the table is a lossless encoding of one bf16 table X~, and the results are
+ * BIT-IDENTICAL to the _bf16 entry points on X~ in every mode: the tensor-core path loads the raw q by TMA and expands q * 2^e to bf16 in
+ * shared memory, in the exact layout the bf16 kernels load, before the same wgmma consumers read it; the SIMT kernels widen q * 2^e on
+ * load.  k is the logical width; W, bias, Y, dY, dW, db stay fp32.  The tensor-core path takes d = 32..256 in steps of 32, k % 16 == 0,
+ * ldx % 16 == 0 and a 16-byte aligned X; other shapes run the SIMT kernels.  `wsplit`, scratch, row maps, accumulate, grouping and the
+ * side-stream bias sums are as for the _bf16 forms. */
+typedef struct {
+  const int8_t* X; const float* W; const float* bias; float* Y; float* wsplit;
+  int64_t ldx, ldy, n;        /* ldx: row pitch of X in bytes */
+  int32_t k, _reserved;       /* flags: 0 or LLMREC_PROJ_ROW_MAP */
+} llmrec_proj_fwd_problem_i8;
+typedef struct {
+  const int8_t* X; const float* dY; float* dW; float* db;
+  int64_t ldx, lddy, n;       /* ldx: row pitch of X in bytes */
+  int32_t k, accumulate;      /* flags: LLMREC_WGRAD_ACCUMULATE | LLMREC_PROJ_ROW_MAP */
+} llmrec_proj_wgrad_problem_i8;
+int llmrec_proj_fwd_group_i8(const llmrec_proj_fwd_problem_i8* probs_host, int32_t n_prob, int32_t d, int32_t mode,
+                             llmrec_stream_t stream);
+int llmrec_proj_wgrad_group_i8(const llmrec_proj_wgrad_problem_i8* probs_host, int32_t n_prob, int32_t d, int32_t mode,
+                               float* scratch /* zero-initialised ONCE, as for llmrec_proj_wgrad_group_f32 */,
+                               int64_t scratch_elems, llmrec_stream_t stream);
+int64_t llmrec_proj_wgrad_group_i8_scratch(const llmrec_proj_wgrad_problem_i8* probs_host, int32_t n_prob, int32_t d, int32_t mode);
+
 /* Row maps, for X tables that hold a subset of the output's rows (the training step projects only the items with a training edge,
  * from compact copies of the item tables).  A problem whose flags word -- `_reserved` of the forward problem, `accumulate` of the
- * weight-gradient problem, both _f32 and _bf16 -- has LLMREC_PROJ_ROW_MAP set takes a map from an llmrec_proj_row_map record.  The
+ * weight-gradient problem, _f32, _bf16 and _i8 -- has LLMREC_PROJ_ROW_MAP set takes a map from an llmrec_proj_row_map record.  The
  * records follow the n_prob problems in the same host array, one per problem in order (records of unflagged problems are ignored);
  * callers that never set the bit pass plain problem arrays as before.  rows: a DEVICE int32 list of the problem's n X rows, every
  * entry a valid row of Y / dY:

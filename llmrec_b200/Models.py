@@ -13,6 +13,7 @@ raises for those flags instead of silently differing.
 import torch
 import torch.nn as nn
 
+from . import feat_int8
 from .engine import HotPath, HotPathConfig, PARAM_ORDER
 from .graph import operators_from_coo
 from .ops import PROJ_MODE
@@ -83,9 +84,14 @@ class MM_Model(nn.Module):
         nn.init.xavier_uniform_(self.user_id_embedding.weight)
         nn.init.xavier_uniform_(self.item_id_embedding.weight)
         # --feat_dtype bf16: the constant feature tables are rounded once (torch's round-to-nearest-even cast; no RNG is drawn, so the
-        # seeded parameter init above is unchanged) and stay bf16; the projection kernels read them as they are
-        feat_dtype = torch.bfloat16 if getattr(args, "feat_dtype", "fp32") == "bf16" else torch.float32
-        as_feat = lambda a: torch.as_tensor(a).float().to(feat_dtype).contiguous()
+        # seeded parameter init above is unchanged) and stay bf16; the projection kernels read them as they are.  --feat_dtype int8:
+        # quantized once into the row-scaled int8 format of feat_int8 (no RNG either); the kernels expand it to bf16 on chip
+        feat_dtype = getattr(args, "feat_dtype", "fp32")
+        if feat_dtype == "int8":
+            as_feat = lambda a: feat_int8.quantize(torch.as_tensor(a).float()).contiguous()
+        else:
+            dt = torch.bfloat16 if feat_dtype == "bf16" else torch.float32
+            as_feat = lambda a: torch.as_tensor(a).float().to(dt).contiguous()
         self.register_buffer("image_feats", as_feat(image_feats), persistent=False)
         self.register_buffer("text_feats", as_feat(text_feats), persistent=False)
         self.register_buffer("user_feats", as_feat(user_init_embedding), persistent=False)

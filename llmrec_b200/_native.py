@@ -47,6 +47,14 @@ class ProjWgradProblemBf16(C.Structure):    # X: raw bfloat16 bits
     _fields_ = ProjWgradProblem._fields_
 
 
+class ProjFwdProblemI8(C.Structure):        # X: int8 table rows (llmrec_b200/feat_int8.py), ldx = row pitch in bytes
+    _fields_ = ProjFwdProblem._fields_
+
+
+class ProjWgradProblemI8(C.Structure):      # X: int8 table rows (llmrec_b200/feat_int8.py), ldx = row pitch in bytes
+    _fields_ = ProjWgradProblem._fields_
+
+
 class ProjRowMap(C.Structure):             # follows the problems of a grouped projection call that flags PROJ_ROW_MAP
     _fields_ = [("rows", C.c_void_p), ("n_dy", C.c_int64)]
 
@@ -101,6 +109,9 @@ SIGNATURES = {
     "llmrec_proj_fwd_group_bf16": (C.c_int, [C.POINTER(ProjFwdProblemBf16), C.c_int32, C.c_int32, C.c_int32, c_stream]),
     "llmrec_proj_wgrad_group_bf16": (C.c_int, [C.POINTER(ProjWgradProblemBf16), C.c_int32, C.c_int32, C.c_int32, c_f32p, C.c_int64, c_stream]),
     "llmrec_proj_wgrad_group_bf16_scratch": (C.c_int64, [C.POINTER(ProjWgradProblemBf16), C.c_int32, C.c_int32, C.c_int32]),
+    "llmrec_proj_fwd_group_i8": (C.c_int, [C.POINTER(ProjFwdProblemI8), C.c_int32, C.c_int32, C.c_int32, c_stream]),
+    "llmrec_proj_wgrad_group_i8": (C.c_int, [C.POINTER(ProjWgradProblemI8), C.c_int32, C.c_int32, C.c_int32, c_f32p, C.c_int64, c_stream]),
+    "llmrec_proj_wgrad_group_i8_scratch": (C.c_int64, [C.POINTER(ProjWgradProblemI8), C.c_int32, C.c_int32, C.c_int32]),
     "llmrec_proj_wgrad_f32": (C.c_int, [c_f32p, C.c_int64, c_f32p, C.c_int64, c_f32p, c_f32p, C.c_int64, C.c_int32, C.c_int32,
                                         C.c_int32, C.c_int32, c_f32p, C.c_int64, c_stream]),
     "llmrec_proj_wgrad_scratch": (C.c_int64, [C.c_int64, C.c_int32, C.c_int32, C.c_int32]),

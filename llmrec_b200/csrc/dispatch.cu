@@ -2,38 +2,50 @@
 // (0 = wgmma 3xTF32, 1 = wgmma TF32, 2 = fp32 SIMT) and by shape support.
 #include <vector>
 #include "common.cuh"
+#include "proj_tc.cuh"
 
 namespace llmrec {
 int proj_fwd_simt(const float*, int64_t, const float*, const float*, float*, int64_t, int64_t, int, int, const int*, cudaStream_t);
 int proj_fwd_simt(const uint16_t*, int64_t, const float*, const float*, float*, int64_t, int64_t, int, int, const int*, cudaStream_t);
 int proj_wgrad_simt(const float*, int64_t, const float*, int64_t, float*, float*, int64_t, int, int, int, const int*, int64_t, cudaStream_t);
 int proj_wgrad_simt(const uint16_t*, int64_t, const float*, int64_t, float*, float*, int64_t, int, int, int, const int*, int64_t, cudaStream_t);
+int proj_fwd_simt(const int8_t*, int64_t, const float*, const float*, float*, int64_t, int64_t, int, int, const int*, cudaStream_t);
+int proj_wgrad_simt(const int8_t*, int64_t, const float*, int64_t, float*, float*, int64_t, int, int, int, const int*, int64_t, cudaStream_t);
 int score_topk_simt(const float*, int64_t, const float*, int64_t, const int*, int, int, int, const int*, const int*, int, int*, float*, float*, int64_t, cudaStream_t);
-bool proj_tc_supported(int d, int64_t ldx, const void* X, int k, bool wgrad, bool bf16);
-int proj_fwd_tc_group(const llmrec_proj_fwd_problem*, const int32_t* const*, int, int, int, bool, cudaStream_t);
-int proj_wgrad_tc_group(const llmrec_proj_wgrad_problem*, const int32_t* const*, const int64_t*, int, int, int, bool, float*, int64_t, cudaStream_t);
-int64_t proj_wgrad_tc_scratch(const llmrec_proj_wgrad_problem*, int, int, int, bool);
+bool proj_tc_supported(int d, int64_t ldx, const void* X, int k, bool wgrad, XType xt);
+int proj_fwd_tc_group(const llmrec_proj_fwd_problem*, const int32_t* const*, int, int, int, XType, cudaStream_t);
+int proj_wgrad_tc_group(const llmrec_proj_wgrad_problem*, const int32_t* const*, const int64_t*, int, int, int, XType, float*, int64_t, cudaStream_t);
+int64_t proj_wgrad_tc_scratch(const llmrec_proj_wgrad_problem*, int, int, int, XType);
 bool score_tc_supported(int d, int K, long long ldu, long long ldi, const void* U, const void* I);
 long long score_tc_scratch(int n_batch, int n_items, int d, int K);
 int score_topk_tc(const float*, long long, const float*, long long, const int*, int, int, int, const int*, const int*, int, int*, float*, float*, long long, cudaStream_t);
 }  // namespace llmrec
 using namespace llmrec;
 
-// bf16 X: the bf16 problems travel in the fp32 structs (same layout; X then holds a bf16 table's address), the tensor-core path
-// reads W as bf16 terms in modes 0 and 1 (wsplit needed in both)
-static bool fwd_tc_ok(const llmrec_proj_fwd_problem* pr, int n, int d, int mode, bool bf16) {
+// bf16 / int8 X: the bf16 and int8 problems travel in the fp32 structs (same layout; X then holds a bf16 / int8 table's address), the
+// tensor-core path reads W as bf16 terms in modes 0 and 1 (wsplit needed in both)
+static bool fwd_tc_ok(const llmrec_proj_fwd_problem* pr, int n, int d, int mode, XType xt) {
   if (mode == 2 || n > 8) return false;
   for (int p = 0; p < n; ++p)
-    if (!proj_tc_supported(d, pr[p].ldx, pr[p].X, pr[p].k, false, bf16) || pr[p].ldy % 4 != 0 || !aligned16(pr[p].Y) || !aligned16(pr[p].W) ||
-        (pr[p].bias && !aligned16(pr[p].bias)) || ((mode == 0 || bf16) && !pr[p].wsplit))
+    if (!proj_tc_supported(d, pr[p].ldx, pr[p].X, pr[p].k, false, xt) || pr[p].ldy % 4 != 0 || !aligned16(pr[p].Y) || !aligned16(pr[p].W) ||
+        (pr[p].bias && !aligned16(pr[p].bias)) || ((mode == 0 || xt != XType::F32) && !pr[p].wsplit))
       return false;
   return true;
 }
-static bool wg_tc_ok(const llmrec_proj_wgrad_problem* pr, int n, int d, int mode, bool bf16) {
+static bool wg_tc_ok(const llmrec_proj_wgrad_problem* pr, int n, int d, int mode, XType xt) {
   if (mode == 2 || n > 8) return false;
   for (int p = 0; p < n; ++p)
-    if (!proj_tc_supported(d, pr[p].ldx, pr[p].X, pr[p].k, true, bf16) || pr[p].lddy % 4 != 0 || !aligned16(pr[p].dY)) return false;
+    if (!proj_tc_supported(d, pr[p].ldx, pr[p].X, pr[p].k, true, xt) || pr[p].lddy % 4 != 0 || !aligned16(pr[p].dY)) return false;
   return true;
+}
+// int8 X: every row must hold its scale at roundup(k, 16), 4-byte aligned, inside the row pitch
+template <class Prob>
+static int check_i8_rows(const Prob* pr, int32_t n_prob) {
+  for (int p = 0; p < n_prob; ++p)
+    LLMREC_CHECK_ARG(pr[p].k >= 1 && pr[p].ldx % 4 == 0 && pr[p].ldx >= i8_scale_offset(pr[p].k) + 4 && (reinterpret_cast<uintptr_t>(pr[p].X) & 3u) == 0,
+                     "proj (int8 X): problem %d: row pitch %lld bytes cannot hold k = %d values and the row scale (needs a multiple of 4, "
+                     ">= roundup(k, 16) + 4, and a 4-byte aligned table)", p, (long long)pr[p].ldx, pr[p].k);
+  return 0;
 }
 
 // Row maps (LLMREC_PROJ_ROW_MAP): the llmrec_proj_row_map records that follow the n_prob problems of a host array (same struct size for
@@ -43,6 +55,8 @@ static int32_t flags(const llmrec_proj_fwd_problem& p) { return p._reserved; }
 static int32_t flags(const llmrec_proj_fwd_problem_bf16& p) { return p._reserved; }
 static int32_t flags(const llmrec_proj_wgrad_problem& p) { return p.accumulate; }
 static int32_t flags(const llmrec_proj_wgrad_problem_bf16& p) { return p.accumulate; }
+static int32_t flags(const llmrec_proj_fwd_problem_i8& p) { return p._reserved; }
+static int32_t flags(const llmrec_proj_wgrad_problem_i8& p) { return p.accumulate; }
 template <class Prob>
 static int row_maps(const Prob* pr, int32_t n_prob, bool wgrad, RowMaps& M) {
   bool any = false;
@@ -62,29 +76,31 @@ static int row_maps(const Prob* pr, int32_t n_prob, bool wgrad, RowMaps& M) {
 }
 
 // rows: NULL, or n_prob optional row maps
-static int proj_fwd_group(const llmrec_proj_fwd_problem* pr, const int32_t* const* rows, int32_t n_prob, int32_t d, int32_t mode, bool bf16,
+static int proj_fwd_group(const llmrec_proj_fwd_problem* pr, const int32_t* const* rows, int32_t n_prob, int32_t d, int32_t mode, XType xt,
                           llmrec_stream_t stream) {
   LLMREC_REQUIRE_DEVICE();
   LLMREC_CHECK_ARG(n_prob >= 1 && d >= 1, "proj_fwd_group: bad sizes");
   cudaStream_t st = as_stream(stream);
   for (int p0 = 0; p0 < n_prob; p0 += 8) {
     int np = n_prob - p0 < 8 ? n_prob - p0 : 8;
-    if (fwd_tc_ok(pr + p0, np, d, mode, bf16)) {
-      int rc = proj_fwd_tc_group(pr + p0, rows ? rows + p0 : nullptr, np, d, mode, bf16, st);
+    if (fwd_tc_ok(pr + p0, np, d, mode, xt)) {
+      int rc = proj_fwd_tc_group(pr + p0, rows ? rows + p0 : nullptr, np, d, mode, xt, st);
       if (rc) return rc;
     } else {
       for (int p = p0; p < p0 + np; ++p) {
         if (pr[p].n <= 0) continue;
         const int32_t* map = rows ? rows[p] : nullptr;
-        int rc = bf16 ? proj_fwd_simt(reinterpret_cast<const uint16_t*>(pr[p].X), pr[p].ldx, pr[p].W, pr[p].bias, pr[p].Y, pr[p].ldy, pr[p].n, pr[p].k, d, map, st)
-                      : proj_fwd_simt(pr[p].X, pr[p].ldx, pr[p].W, pr[p].bias, pr[p].Y, pr[p].ldy, pr[p].n, pr[p].k, d, map, st);
+        int rc = xt == XType::I8   ? proj_fwd_simt(reinterpret_cast<const int8_t*>(pr[p].X), pr[p].ldx, pr[p].W, pr[p].bias, pr[p].Y, pr[p].ldy, pr[p].n, pr[p].k, d, map, st)
+                 : xt == XType::BF16 ? proj_fwd_simt(reinterpret_cast<const uint16_t*>(pr[p].X), pr[p].ldx, pr[p].W, pr[p].bias, pr[p].Y, pr[p].ldy, pr[p].n, pr[p].k, d, map, st)
+                                     : proj_fwd_simt(pr[p].X, pr[p].ldx, pr[p].W, pr[p].bias, pr[p].Y, pr[p].ldy, pr[p].n, pr[p].k, d, map, st);
         if (rc) return rc;
       }
     }
   }
   return 0;
 }
-static std::vector<llmrec_proj_fwd_problem> as_f32_layout(const llmrec_proj_fwd_problem_bf16* pr, int32_t n_prob) {
+template <class Prob>   // the _bf16 / _i8 forward problem
+static std::vector<llmrec_proj_fwd_problem> as_f32_layout(const Prob* pr, int32_t n_prob) {
   std::vector<llmrec_proj_fwd_problem> q(n_prob > 0 ? n_prob : 0);
   for (int p = 0; p < n_prob; ++p)
     q[p] = {reinterpret_cast<const float*>(pr[p].X), pr[p].W, pr[p].bias, pr[p].Y, pr[p].wsplit, pr[p].ldx, pr[p].ldy, pr[p].n, pr[p].k, 0};
@@ -94,13 +110,20 @@ extern "C" int llmrec_proj_fwd_group_f32(const llmrec_proj_fwd_problem* pr, int3
   LLMREC_CHECK_ARG(pr && n_prob >= 1, "proj_fwd_group: bad sizes");
   RowMaps M;
   if (int rc = row_maps(pr, n_prob, false, M)) return rc;
-  return proj_fwd_group(pr, M.rows.empty() ? nullptr : M.rows.data(), n_prob, d, mode, false, stream);
+  return proj_fwd_group(pr, M.rows.empty() ? nullptr : M.rows.data(), n_prob, d, mode, XType::F32, stream);
 }
 extern "C" int llmrec_proj_fwd_group_bf16(const llmrec_proj_fwd_problem_bf16* pr, int32_t n_prob, int32_t d, int32_t mode, llmrec_stream_t stream) {
   LLMREC_CHECK_ARG(pr && n_prob >= 1, "proj_fwd_group: bad sizes");
   RowMaps M;
   if (int rc = row_maps(pr, n_prob, false, M)) return rc;
-  return proj_fwd_group(as_f32_layout(pr, n_prob).data(), M.rows.empty() ? nullptr : M.rows.data(), n_prob, d, mode, true, stream);
+  return proj_fwd_group(as_f32_layout(pr, n_prob).data(), M.rows.empty() ? nullptr : M.rows.data(), n_prob, d, mode, XType::BF16, stream);
+}
+extern "C" int llmrec_proj_fwd_group_i8(const llmrec_proj_fwd_problem_i8* pr, int32_t n_prob, int32_t d, int32_t mode, llmrec_stream_t stream) {
+  LLMREC_CHECK_ARG(pr && n_prob >= 1, "proj_fwd_group: bad sizes");
+  if (int rc = check_i8_rows(pr, n_prob)) return rc;
+  RowMaps M;
+  if (int rc = row_maps(pr, n_prob, false, M)) return rc;
+  return proj_fwd_group(as_f32_layout(pr, n_prob).data(), M.rows.empty() ? nullptr : M.rows.data(), n_prob, d, mode, XType::I8, stream);
 }
 extern "C" int llmrec_proj_fwd_f32(const float* X, int64_t ldx, const float* W, const float* bias, float* Y, int64_t ldy,
                                    int64_t n, int32_t k, int32_t d, int32_t mode, float* wsplit, llmrec_stream_t stream) {
@@ -109,49 +132,54 @@ extern "C" int llmrec_proj_fwd_f32(const float* X, int64_t ldx, const float* W, 
   return llmrec_proj_fwd_group_f32(&p, 1, d, mode, stream);
 }
 
-static int64_t proj_wgrad_scratch(const llmrec_proj_wgrad_problem* pr, int32_t n_prob, int32_t d, int32_t mode, bool bf16) {
+static int64_t proj_wgrad_scratch(const llmrec_proj_wgrad_problem* pr, int32_t n_prob, int32_t d, int32_t mode, XType xt) {
   int64_t need = 0;
   for (int p0 = 0; p0 < n_prob; p0 += 8) {
     int np = n_prob - p0 < 8 ? n_prob - p0 : 8;
-    if (wg_tc_ok(pr + p0, np, d, mode, bf16)) { int64_t s = proj_wgrad_tc_scratch(pr + p0, np, d, mode, bf16); need = s > need ? s : need; }
+    if (wg_tc_ok(pr + p0, np, d, mode, xt)) { int64_t s = proj_wgrad_tc_scratch(pr + p0, np, d, mode, xt); need = s > need ? s : need; }
   }
   return need;
 }
 // rows / n_dy: NULL, or per problem an optional dY row map and the row count of dY
 static int proj_wgrad_group(const llmrec_proj_wgrad_problem* pr, const int32_t* const* rows, const int64_t* n_dy, int32_t n_prob, int32_t d,
-                            int32_t mode, bool bf16, float* scratch, int64_t scratch_elems, llmrec_stream_t stream) {
+                            int32_t mode, XType xt, float* scratch, int64_t scratch_elems, llmrec_stream_t stream) {
   LLMREC_REQUIRE_DEVICE();
   LLMREC_CHECK_ARG(n_prob >= 1 && d >= 1, "proj_wgrad_group: bad sizes");
   cudaStream_t st = as_stream(stream);
   for (int p0 = 0; p0 < n_prob; p0 += 8) {
     int np = n_prob - p0 < 8 ? n_prob - p0 : 8;
-    if (wg_tc_ok(pr + p0, np, d, mode, bf16)) {
-      int rc = proj_wgrad_tc_group(pr + p0, rows ? rows + p0 : nullptr, rows ? n_dy + p0 : nullptr, np, d, mode, bf16, scratch, scratch_elems, st);
+    if (wg_tc_ok(pr + p0, np, d, mode, xt)) {
+      int rc = proj_wgrad_tc_group(pr + p0, rows ? rows + p0 : nullptr, rows ? n_dy + p0 : nullptr, np, d, mode, xt, scratch, scratch_elems, st);
       if (rc) return rc;
     } else {
       for (int p = p0; p < p0 + np; ++p) {
         const int acc = pr[p].accumulate & LLMREC_WGRAD_ACCUMULATE;
         const int32_t* map = rows ? rows[p] : nullptr;
         const int64_t ndy = n_dy ? n_dy[p] : pr[p].n;
-        int rc = bf16 ? proj_wgrad_simt(reinterpret_cast<const uint16_t*>(pr[p].X), pr[p].ldx, pr[p].dY, pr[p].lddy, pr[p].dW, pr[p].db, pr[p].n, pr[p].k, d, acc, map, ndy, st)
-                      : proj_wgrad_simt(pr[p].X, pr[p].ldx, pr[p].dY, pr[p].lddy, pr[p].dW, pr[p].db, pr[p].n, pr[p].k, d, acc, map, ndy, st);
+        int rc = xt == XType::I8   ? proj_wgrad_simt(reinterpret_cast<const int8_t*>(pr[p].X), pr[p].ldx, pr[p].dY, pr[p].lddy, pr[p].dW, pr[p].db, pr[p].n, pr[p].k, d, acc, map, ndy, st)
+                 : xt == XType::BF16 ? proj_wgrad_simt(reinterpret_cast<const uint16_t*>(pr[p].X), pr[p].ldx, pr[p].dY, pr[p].lddy, pr[p].dW, pr[p].db, pr[p].n, pr[p].k, d, acc, map, ndy, st)
+                                     : proj_wgrad_simt(pr[p].X, pr[p].ldx, pr[p].dY, pr[p].lddy, pr[p].dW, pr[p].db, pr[p].n, pr[p].k, d, acc, map, ndy, st);
         if (rc) return rc;
       }
     }
   }
   return 0;
 }
-static std::vector<llmrec_proj_wgrad_problem> as_f32_layout(const llmrec_proj_wgrad_problem_bf16* pr, int32_t n_prob) {
+template <class Prob>   // the _bf16 / _i8 weight-gradient problem
+static std::vector<llmrec_proj_wgrad_problem> as_wgrad_f32_layout(const Prob* pr, int32_t n_prob) {
   std::vector<llmrec_proj_wgrad_problem> q(n_prob > 0 ? n_prob : 0);
   for (int p = 0; p < n_prob; ++p)
     q[p] = {reinterpret_cast<const float*>(pr[p].X), pr[p].dY, pr[p].dW, pr[p].db, pr[p].ldx, pr[p].lddy, pr[p].n, pr[p].k, pr[p].accumulate};
   return q;
 }
 extern "C" int64_t llmrec_proj_wgrad_group_scratch(const llmrec_proj_wgrad_problem* pr, int32_t n_prob, int32_t d, int32_t mode) {
-  return proj_wgrad_scratch(pr, n_prob, d, mode, false);
+  return proj_wgrad_scratch(pr, n_prob, d, mode, XType::F32);
 }
 extern "C" int64_t llmrec_proj_wgrad_group_bf16_scratch(const llmrec_proj_wgrad_problem_bf16* pr, int32_t n_prob, int32_t d, int32_t mode) {
-  return proj_wgrad_scratch(as_f32_layout(pr, n_prob).data(), n_prob, d, mode, true);
+  return proj_wgrad_scratch(as_wgrad_f32_layout(pr, n_prob).data(), n_prob, d, mode, XType::BF16);
+}
+extern "C" int64_t llmrec_proj_wgrad_group_i8_scratch(const llmrec_proj_wgrad_problem_i8* pr, int32_t n_prob, int32_t d, int32_t mode) {
+  return proj_wgrad_scratch(as_wgrad_f32_layout(pr, n_prob).data(), n_prob, d, mode, XType::I8);
 }
 extern "C" int llmrec_proj_wgrad_group_f32(const llmrec_proj_wgrad_problem* pr, int32_t n_prob, int32_t d, int32_t mode,
                                            float* scratch, int64_t scratch_elems, llmrec_stream_t stream) {
@@ -159,7 +187,7 @@ extern "C" int llmrec_proj_wgrad_group_f32(const llmrec_proj_wgrad_problem* pr, 
   RowMaps M;
   if (int rc = row_maps(pr, n_prob, true, M)) return rc;
   const bool mapped = !M.rows.empty();
-  return proj_wgrad_group(pr, mapped ? M.rows.data() : nullptr, mapped ? M.n_dy.data() : nullptr, n_prob, d, mode, false, scratch, scratch_elems, stream);
+  return proj_wgrad_group(pr, mapped ? M.rows.data() : nullptr, mapped ? M.n_dy.data() : nullptr, n_prob, d, mode, XType::F32, scratch, scratch_elems, stream);
 }
 extern "C" int llmrec_proj_wgrad_group_bf16(const llmrec_proj_wgrad_problem_bf16* pr, int32_t n_prob, int32_t d, int32_t mode,
                                             float* scratch, int64_t scratch_elems, llmrec_stream_t stream) {
@@ -167,14 +195,24 @@ extern "C" int llmrec_proj_wgrad_group_bf16(const llmrec_proj_wgrad_problem_bf16
   RowMaps M;
   if (int rc = row_maps(pr, n_prob, true, M)) return rc;
   const bool mapped = !M.rows.empty();
-  return proj_wgrad_group(as_f32_layout(pr, n_prob).data(), mapped ? M.rows.data() : nullptr, mapped ? M.n_dy.data() : nullptr, n_prob, d, mode,
-                          true, scratch, scratch_elems, stream);
+  return proj_wgrad_group(as_wgrad_f32_layout(pr, n_prob).data(), mapped ? M.rows.data() : nullptr, mapped ? M.n_dy.data() : nullptr, n_prob, d, mode,
+                          XType::BF16, scratch, scratch_elems, stream);
+}
+extern "C" int llmrec_proj_wgrad_group_i8(const llmrec_proj_wgrad_problem_i8* pr, int32_t n_prob, int32_t d, int32_t mode,
+                                          float* scratch, int64_t scratch_elems, llmrec_stream_t stream) {
+  LLMREC_CHECK_ARG(pr && n_prob >= 1, "proj_wgrad_group: bad sizes");
+  if (int rc = check_i8_rows(pr, n_prob)) return rc;
+  RowMaps M;
+  if (int rc = row_maps(pr, n_prob, true, M)) return rc;
+  const bool mapped = !M.rows.empty();
+  return proj_wgrad_group(as_wgrad_f32_layout(pr, n_prob).data(), mapped ? M.rows.data() : nullptr, mapped ? M.n_dy.data() : nullptr, n_prob, d, mode,
+                          XType::I8, scratch, scratch_elems, stream);
 }
 extern "C" int64_t llmrec_proj_wgrad_scratch(int64_t n, int32_t k, int32_t d, int32_t mode) {
   llmrec_proj_wgrad_problem p{nullptr, nullptr, nullptr, nullptr, 4, 4, n, k, 0};
   // alignment of real pointers is checked at call time; size the scratch for the tensor-core path
   if (mode == 2 || d % 32 != 0 || d > 256 || k % 4 != 0) return 0;
-  return proj_wgrad_tc_scratch(&p, 1, d, mode, false);
+  return proj_wgrad_tc_scratch(&p, 1, d, mode, XType::F32);
 }
 extern "C" int llmrec_proj_wgrad_f32(const float* X, int64_t ldx, const float* dY, int64_t lddy, float* dW, float* db,
                                      int64_t n, int32_t k, int32_t d, int32_t accumulate, int32_t mode,

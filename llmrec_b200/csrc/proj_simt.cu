@@ -2,13 +2,21 @@
 // (nn.Linear at Models.py:145-150).  mode 2 of llmrec_proj_*: the bit-conservative path used as the
 // on-device checker for the wgmma kernels (proj_tc.cu) and for shapes those do not cover.
 // Templated on the element type of X: fp32, or bf16 (raw uint16_t bits) widened to fp32 on load -- the same FMA order, so a bf16
-// table gives the bits of the fp32 kernel on its upcast copy.
+// table gives the bits of the fp32 kernel on its upcast copy -- or int8 rows (include/llmrec_b200.h: ldx is the row pitch in bytes,
+// the row's scale sits at byte roundup(k, 16)) widened to q * scale, the exact value of the bf16 table the int8 one encodes.
 #include "common.cuh"
 
 namespace llmrec {
 
 __device__ __forceinline__ float x_f32(float x) { return x; }
 __device__ __forceinline__ float x_f32(uint16_t x) { return __uint_as_float((uint32_t)x << 16); }
+// X[r][c] of a table of logical width k
+template <class T>
+__device__ __forceinline__ float x_at(const T* X, int64_t ldx, int64_t r, int c, int) { return x_f32(X[r * ldx + c]); }
+__device__ __forceinline__ float x_at(const int8_t* X, int64_t ldx, int64_t r, int c, int k) {
+  const int8_t* row = X + r * ldx;
+  return (float)row[c] * __ldg(reinterpret_cast<const float*>(row + ((k + 15) & ~15)));
+}
 
 // Y[n x d] = X[n x k] W^T[k x d] + b ; 64x64 tile, K step 16, 4x4 per thread.  rows (optional): X row r is written to Y row rows[r]
 template <class T>
@@ -25,7 +33,7 @@ __global__ void __launch_bounds__(256) proj_fwd_simt_kernel(const T* __restrict_
     for (int i = threadIdx.x; i < 64 * 16; i += 256) {
       int r = i >> 4, kk = i & 15;
       int64_t gr = row0 + r;
-      Xs[kk][r] = (gr < n && k0 + kk < k) ? x_f32(X[gr * ldx + k0 + kk]) : 0.f;
+      Xs[kk][r] = (gr < n && k0 + kk < k) ? x_at(X, ldx, gr, k0 + kk, k) : 0.f;
       int gc = col0 + r;
       Ws[kk][r] = (gc < d && k0 + kk < k) ? W[(int64_t)gc * k + k0 + kk] : 0.f;
     }
@@ -74,7 +82,7 @@ __global__ void __launch_bounds__(256) proj_wgrad_simt_kernel(const T* __restric
       int r = i >> 6, c = i & 63;
       int64_t gr = r0 + r;
       Gs[r][c] = (gr < r_end && d0 + c < d) ? dY[(rows ? (int64_t)rows[gr] : gr) * lddy + d0 + c] : 0.f;
-      Xs[r][c] = (gr < r_end && k0 + c < k) ? x_f32(X[gr * ldx + k0 + c]) : 0.f;
+      Xs[r][c] = (gr < r_end && k0 + c < k) ? x_at(X, ldx, gr, k0 + c, k) : 0.f;
     }
     __syncthreads();
 #pragma unroll
@@ -157,6 +165,14 @@ int proj_wgrad_simt(const float* X, int64_t ldx, const float* dY, int64_t lddy, 
   return wgrad_simt(X, ldx, dY, lddy, dW, db, n, k, d, accumulate, rows, n_dy, st);
 }
 int proj_wgrad_simt(const uint16_t* X, int64_t ldx, const float* dY, int64_t lddy, float* dW, float* db, int64_t n, int k, int d, int accumulate,
+                    const int* rows, int64_t n_dy, cudaStream_t st) {
+  return wgrad_simt(X, ldx, dY, lddy, dW, db, n, k, d, accumulate, rows, n_dy, st);
+}
+int proj_fwd_simt(const int8_t* X, int64_t ldx, const float* W, const float* bias, float* Y, int64_t ldy, int64_t n, int k, int d, const int* rows,
+                  cudaStream_t st) {
+  return fwd_simt(X, ldx, W, bias, Y, ldy, n, k, d, rows, st);
+}
+int proj_wgrad_simt(const int8_t* X, int64_t ldx, const float* dY, int64_t lddy, float* dW, float* db, int64_t n, int k, int d, int accumulate,
                     const int* rows, int64_t n_dy, cudaStream_t st) {
   return wgrad_simt(X, ldx, dY, lddy, dW, db, n, k, d, accumulate, rows, n_dy, st);
 }

@@ -27,6 +27,8 @@
 // bf16 X (--feat_dtype bf16, BF16 = true): the same pipeline with 64 k / rows per stage.  X is exact in bf16, so it is not split and
 // A is read by descriptor straight from the stage (wgrad: MN-major, no permutation); W / dY^T arrive as three exact bf16 terms
 // (wsplit_bf16, dyt_split<true>) and each k16 step issues X*w2 + X*w1 + X*w0: no product term is dropped (mode 1: X*w0 only).
+// int8 X (--feat_dtype int8, XType::I8): every stored q * 2^e is a bf16 number, so the bf16 pipeline runs unchanged on stages that
+// producer warps 1..3 expand from the raw q the TMA brings (I8Stage): the bits of the bf16 kernels on the dequantized table.
 #include <mutex>
 #include <stdlib.h>
 #include <vector>
@@ -105,7 +107,7 @@ struct ProjCfg {
   static constexpr uint32_t kStage = kX + kB * NB;
   static constexpr int kFit = (int)((kSmemMax - 1024u - 256u) / kStage);
   static constexpr int kStages = kFit > 4 ? 4 : kFit;          // 4 at d = 64, 3 at d = 128, 2 at d = 256
-  static constexpr uint32_t kSmem = 1024u /*align slack*/ + kStages * kStage + 2u * kStages * 8u;
+  static constexpr uint32_t kSmem = 1024u /*align slack*/ + kStages * kStage + 3u * kStages * 8u;   // + full, empty, raw barriers
   static_assert(kStages >= 2, "projection ring needs two stages");
 };
 
@@ -140,14 +142,94 @@ __device__ __forceinline__ void ld_frag_wgrad(uint32_t (&a)[4], uint32_t sx, int
   a[3] = lds_u32(base + 512 + ((q ^ 5) << 4));
 }
 
+// ---- int8 X: a raw stage expanded into the bf16 stage layout --------------------------------------------------------------------
+// 16 int8 q (one 16-byte word) times the row scale 2^e -> 16 bf16, exactly: q * 2^e has at most 7 significant bits and is a normal
+// fp32 (the format clamps e to [-126, 120]), so its top 16 bits are the bf16.  q is widened without a conversion instruction: q + 128
+// goes into the low byte of 2^23's significand, and float(0x4B000000 | (q + 128)) - (2^23 + 128) = q exactly.
+__device__ __forceinline__ uint32_t i8_pair_bf16(uint32_t w, int b, float s) {   // w: four q + 128; elements b, b + 1 -> packed bf16
+  const float x0 = (__uint_as_float(__byte_perm(w, 0x4B000000u, 0x7650u + b)) - 8388736.0f) * s;
+  const float x1 = (__uint_as_float(__byte_perm(w, 0x4B000000u, 0x7651u + b)) - 8388736.0f) * s;
+  return __byte_perm(__float_as_uint(x0), __float_as_uint(x1), 0x7632u);
+}
+__device__ __forceinline__ void i8x16_bf16(const uint4& q, float s, uint4& lo, uint4& hi) {
+  const uint32_t w0 = q.x ^ 0x80808080u, w1 = q.y ^ 0x80808080u, w2 = q.z ^ 0x80808080u, w3 = q.w ^ 0x80808080u;
+  lo = make_uint4(i8_pair_bf16(w0, 0, s), i8_pair_bf16(w0, 2, s), i8_pair_bf16(w1, 0, s), i8_pair_bf16(w1, 2, s));
+  hi = make_uint4(i8_pair_bf16(w2, 0, s), i8_pair_bf16(w2, 2, s), i8_pair_bf16(w3, 0, s), i8_pair_bf16(w3, 2, s));
+}
+__device__ __forceinline__ void converters_sync() { asm volatile("bar.sync 1, 96;" ::: "memory"); }   // producer warps 1..3
+
+// The converter warps (producer warps 1..3, ct = 0..95) of an int8 unit.  TMA put the stage's raw q into the UPPER half of the stage's
+// X area (TM * 64 bytes), as TM/64 groups of 4 KiB: group g = 64 rows (fwd) / 64 features (wgrad) at TM*64 + 4096 g.  A task expands
+// 16 q at Unit::raw_off into the two 16-byte bf16 chunks at Unit::out_off -- the bytes the bf16 TMA load of the dequantized table
+// writes there (128-byte swizzle; rows past n and columns past k are zeros, as TMA fills them).  Group g's bf16 output is the 8 KiB at
+// 8192 g: the groups of the lower half touch no raw byte; group g >= TM/128 overwrites raw groups 2g - TM/64 and 2g - TM/64 + 1, the
+// earlier one of which (and at the last group, its own) is still input.  So before writing such a group every converter has loaded the
+// group's inputs, and the three warps meet at a named barrier.
+template <class Unit>
+struct I8Stage {
+  static constexpr int kGroups = Unit::Cfg::TM / 64, kTasks = 256;   // per group: 64 x 64 q, 16 per task
+  static constexpr int kPer = (kTasks + 95) / 96;                    // 3 tasks per converter thread and group
+  float sc[kPer];                // wgrad: the scales of the tasks' stage rows (the same 64 rows in every group)
+  const float* tile_sc = nullptr;   // fwd: the tile's TM row scales in shared memory (Unit::kScalesPerUnit)
+  // wgrad: global loads, issued before the wait for the raw box
+  __device__ void load_scales(const Unit& w, int kb, int ct) {
+#pragma unroll
+    for (int m = 0; m < kPer; ++m) {
+      const int t = ct + 96 * m;
+      sc[m] = t < kTasks ? w.row_scale(w.task_row(0, t, kb)) : 0.f;
+    }
+  }
+  __device__ void expand(uint8_t* sx, int ct) const {
+#pragma unroll
+    for (int g = 0; g < kGroups; ++g) {
+      uint4 v[kPer];
+#pragma unroll
+      for (int m = 0; m < kPer; ++m) {
+        const int t = ct + 96 * m;
+        if (t < kTasks) v[m] = *reinterpret_cast<const uint4*>(sx + Unit::Cfg::TM * 64u + g * 4096u + Unit::raw_off(t));
+      }
+      if (2 * g >= kGroups) converters_sync();
+#pragma unroll
+      for (int m = 0; m < kPer; ++m) {
+        const int t = ct + 96 * m;
+        if (t >= kTasks) continue;
+        uint4 lo, hi;
+        uint32_t o_lo, o_hi;
+        i8x16_bf16(v[m], Unit::kScalesPerUnit ? tile_sc[64 * g + (t >> 2)] : sc[m], lo, hi);
+        Unit::out_off(t, o_lo, o_hi);
+        *reinterpret_cast<uint4*>(sx + g * 8192u + o_lo) = lo;
+        *reinterpret_cast<uint4*>(sx + g * 8192u + o_hi) = hi;
+      }
+    }
+  }
+};
+
+// task t of a group: 16 q of group row i = t / 4 (fwd: tile row 64g + i; wgrad: stage row i), columns 16 (t % 4) .. + 15 of the group
+// (fwd: k; wgrad: features 64g ..); raw row i at 64 i, the bf16 row at 128 i with chunk c at ((c ^ i) % 8) * 16
+__device__ __forceinline__ uint32_t i8_raw_off(int t) { return (t >> 2) * 64u + (t & 3) * 16u; }
+__device__ __forceinline__ void i8_out_off(int t, uint32_t& lo, uint32_t& hi) {
+  const int i = t >> 2, c = 2 * (t & 3);
+  lo = i * 128u + (((c ^ i) & 7) << 4);
+  hi = i * 128u + ((((c + 1) ^ i) & 7) << 4);
+}
+
+// scale of table row `row` of problem p (0 past the table: those rows load as q = 0)
+__device__ __forceinline__ float i8_row_scale(const RowScales& xs, int p, int n, int row) {
+  return row < n ? __ldg(reinterpret_cast<const float*>(xs.scale[p] + (long long)row * xs.pitch[p])) : 0.f;
+}
+
 // work unit -> (problem, number of k-blocks, what the producer loads for k-block kb, where the epilogue writes)
-template <int D, bool SPLIT, int MB, bool BF16 = false>
+// I8 (with BF16): X is an int8 table; the bf16 pipeline runs on the stages the converter warps expand (I8Stage).
+template <int D, bool SPLIT, int MB, bool BF16 = false, bool I8 = false>
 struct FwdUnit {
   using Cfg = ProjCfg<D, SPLIT, MB, BF16>;
+  static_assert(!I8 || BF16, "int8 X runs the bf16 pipeline");
   static constexpr int kTransA = 0;   // bf16: A = the X tile as it arrived, K-major
-  static constexpr int kBuilders = 0;            // warps that build B in the kernel: none, W arrives by TMA
-  static constexpr int kProducerRegs = 40, kConsumerRegs = 232;   // setmaxnreg: 128 * 40 + 256 * 232 = 384 * 168
-  static constexpr uint32_t kTx = Cfg::kStage;   // TMA bytes per stage: X and W
+  static constexpr int kBuilders = I8 ? 3 : 0;   // warps that write stage operands in the kernel: the int8 converters; W arrives by TMA
+  // setmaxnreg: 128 * 40 + 256 * 232 = 384 * 168; the int8 converters hold a group's raw words in flight: 128 * 72 + 256 * 216
+  static constexpr int kProducerRegs = I8 ? 72 : 40, kConsumerRegs = I8 ? 216 : 232;
+  static constexpr uint32_t kRawTx = I8 ? Cfg::TM * 64u : 0u;   // raw q bytes per stage, on the stage's own raw barrier
+  static constexpr uint32_t kTx = I8 ? Cfg::kStage - Cfg::kX : Cfg::kStage;   // TMA bytes per stage on `full`: X and W (int8: W)
   const FwdParams& P; int p, mblk, kb_n;
   __device__ FwdUnit(const FwdParams& P_, int u) : P(P_) {
     p = 0;
@@ -155,12 +237,21 @@ struct FwdUnit {
     mblk = u - P.prob[p].tile_start;
     kb_n = P.prob[p].kblocks;
   }
-  __device__ void issue(uint8_t* st, uint64_t* bar, int kb, uint64_t pol) const {
+  __device__ void issue(uint8_t* st, uint64_t* bar, uint64_t* raw_bar, int kb, uint64_t pol) const {
     constexpr int bk = stage_k(BF16);
-    tma_load_2d_hint(st, &P.tmA[p], bar, kb * bk, mblk * Cfg::TM, pol);
+    if constexpr (I8) tma_load_2d_hint(st + Cfg::TM * 64, &P.tmA[p], raw_bar, kb * bk, mblk * Cfg::TM, pol);   // [TM rows][64 q]: the groups in order
+    else tma_load_2d_hint(st, &P.tmA[p], bar, kb * bk, mblk * Cfg::TM, pol);
 #pragma unroll
     for (int i = 0; i < Cfg::NB; ++i) tma_load_2d(st + Cfg::kX + i * Cfg::kB, &P.tmW[p], bar, kb * bk, i * D);
   }
+  // int8 (I8Stage): group g = tile rows 64g .. 64g + 63, the same rows at every k-block: the converters put the tile's row scales
+  // into shared memory once per unit (ts[i] = scale of tile row i)
+  static constexpr bool kScalesPerUnit = true;
+  __device__ void tile_scales(float* ts, int ct) const {
+    for (int i = ct; i < Cfg::TM; i += 96) ts[i] = i8_row_scale(P.xs, p, P.prob[p].n, mblk * Cfg::TM + i);
+  }
+  static __device__ uint32_t raw_off(int t) { return i8_raw_off(t); }
+  static __device__ void out_off(int t, uint32_t& lo, uint32_t& hi) { i8_out_off(t, lo, hi); }
   static __device__ void ld_frag(uint32_t (&a)[4], uint32_t sx, int blk, int kk, int warp, int lane) { ld_frag_fwd(a, sx, blk, kk, warp, lane); }
   // bf16: descriptor of m64 block `blk` (64 rows x 128 bytes), k16 step kk (+32 bytes inside the swizzled rows)
   static __device__ uint64_t a_desc(uint32_t sx, int blk, int kk) { return gmma_desc_sw128(sx + blk * 8192u + kk * 32u); }
@@ -190,9 +281,10 @@ struct FwdUnit {
   }
 };
 
-template <int D, bool SPLIT, int MB, bool BF16 = false>
+template <int D, bool SPLIT, int MB, bool BF16 = false, bool I8 = false>
 struct WgUnit {
   using Cfg = ProjCfg<D, SPLIT, MB, BF16>;
+  static_assert(!I8 || BF16, "int8 X runs the bf16 pipeline");
   static constexpr int kBk = stage_k(BF16);
   static constexpr int kTransA = 1;   // bf16: A = X^T, read MN-major out of the raw X tile (no feature permutation)
   const WgParams& P; int p, u, ft, r0, kb_n;
@@ -205,26 +297,39 @@ struct WgUnit {
     r0 = chunk * pr.rows_per_chunk;
     kb_n = (min(pr.n, r0 + pr.rows_per_chunk) - r0 + kBk - 1) / kBk;   // chunks are stage-aligned; rows past n load as zeros
   }
-  // fp32 X, 3xTF32: producer warps 1..3 build B from dY (below).  bf16 X and mode 1 keep B = dY^T by TMA from `dyt_split`: their
+  // fp32 X, 3xTF32: producer warps 1..3 build B from dY (below).  bf16 / int8 X and mode 1 keep B = dY^T by TMA from `dyt_split`: their
   // consumers finish a stage sooner than three warps build one, measured slower at the netflix and movielens shapes (H100 SXM, 700 W).
-  static constexpr int kBuilders = SPLIT && !BF16 ? 3 : 0;
+  // int8 X: warps 1..3 expand the raw X stage instead (I8Stage).
+  static constexpr bool kBuildsB = SPLIT && !BF16;
+  static constexpr int kBuilders = kBuildsB || I8 ? 3 : 0;
   static constexpr int kProducerRegs = kBuilders ? 72 : 40;     // 128 * 72 + 256 * 216 = 384 * 168: the builders' loads in flight
   static constexpr int kConsumerRegs = kBuilders ? 216 : 232;
-  static constexpr uint32_t kTx = kBuilders ? Cfg::kX : Cfg::kStage;   // TMA bytes per stage: X, and B without builders
-  __device__ void issue(uint8_t* st, uint64_t* bar, int kb, uint64_t pol) const {
+  static constexpr uint32_t kRawTx = I8 ? Cfg::TM * 64u : 0u;   // raw q bytes per stage, on the stage's own raw barrier
+  static constexpr uint32_t kTx = kBuildsB ? Cfg::kX : I8 ? Cfg::kStage - Cfg::kX : Cfg::kStage;   // TMA bytes per stage on `full`
+  __device__ void issue(uint8_t* st, uint64_t* bar, uint64_t* raw_bar, int kb, uint64_t pol) const {
     const int r = r0 + kb * kBk;
-    if constexpr (BF16) {   // TM/64 boxes [64 rows][64 features], 8 KiB each: one per m64 block
+    if constexpr (I8) {     // TM/64 boxes [64 rows][64 features] of raw q, 4 KiB each, into the upper half of the X area
+#pragma unroll
+      for (int b = 0; b < Cfg::TM / 64; ++b) tma_load_2d_hint(st + Cfg::TM * 64 + b * 4096, &P.tmX[p], raw_bar, ft * Cfg::TM + 64 * b, r, pol);
+    } else if constexpr (BF16) {   // TM/64 boxes [64 rows][64 features], 8 KiB each: one per m64 block
 #pragma unroll
       for (int b = 0; b < Cfg::TM / 64; ++b) tma_load_2d_hint(st + b * 8192, &P.tmX[p], bar, ft * Cfg::TM + 64 * b, r, pol);
     } else {
 #pragma unroll
       for (int b = 0; b < Cfg::TM / 32; ++b) tma_load_2d_hint(st + b * 4096, &P.tmX[p], bar, ft * Cfg::TM + 32 * b, r, pol);
     }
-    if constexpr (kBuilders == 0) {
+    if constexpr (!kBuildsB) {
 #pragma unroll
       for (int i = 0; i < Cfg::NB; ++i) tma_load_2d(st + Cfg::kX + i * Cfg::kB, &P.tmG[p], bar, r, i * D);
     }
   }
+  // int8 (I8Stage): group g = tile features 64g .. 64g + 63 (the bf16 box of m64 block g) over the stage's 64 rows
+  static constexpr bool kScalesPerUnit = false;
+  __device__ void tile_scales(float*, int) const {}
+  __device__ int task_row(int, int t, int kb) const { return r0 + kb * kBk + (t >> 2); }
+  __device__ float row_scale(int row) const { return i8_row_scale(P.xs, p, P.prob[p].n, row); }
+  static __device__ uint32_t raw_off(int t) { return i8_raw_off(t); }
+  static __device__ void out_off(int t, uint32_t& lo, uint32_t& hi) { i8_out_off(t, lo, hi); }
   // B of stage kb = dY^T over the stage's kBk rows, split into hi and lo, written by builder warp bw (0 .. kBuilders-1) in the layout
   // TMA gives a [D][32] box with the 128-byte swizzle: element (column c, stage row j) at c*128 + ((j/4 ^ c) % 8)*16 + (j%4)*4.  Lane l owns
   // stage row l, so it reads its dY row through the row map once; a task is 8 columns (32 bytes of the row, two 16-byte loads),
@@ -287,18 +392,20 @@ __device__ __forceinline__ void proj_pipeline(const Params& P, int total) {
   uint8_t* smem = align1024(smem_raw);
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + Cfg::kStages * Cfg::kStage);
   uint64_t* empty = full + Cfg::kStages;
+  uint64_t* raw = empty + Cfg::kStages;   // int8 X: the raw q box of the stage has landed
+  float* tile_sc = reinterpret_cast<float*>(raw + Cfg::kStages);   // int8 forward: the tile's TM row scales (launch_fwd sizes them)
   const int tid = threadIdx.x, wg = tid >> 7, warp = (tid >> 5) & 3, lane = tid & 31;
   if (tid == 0) {
-    // full: the TMA thread's arrive (+ transaction bytes) and, when the kernel builds B, one arrival per builder warp;
-    // empty: one arrival per consumer warp
-    for (int s = 0; s < Cfg::kStages; ++s) { mbar_init(&full[s], 1 + Unit::kBuilders); mbar_init(&empty[s], 8); }
+    // full: the TMA thread's arrive (+ transaction bytes) and, when the kernel builds B or expands int8 X, one arrival per builder warp;
+    // empty: one arrival per consumer warp; raw: the TMA thread's arrive (+ the raw q bytes)
+    for (int s = 0; s < Cfg::kStages; ++s) { mbar_init(&full[s], 1 + Unit::kBuilders); mbar_init(&empty[s], 8); mbar_init(&raw[s], 1); }
     fence_barrier_init();
   }
   __syncthreads();
 
   // the CTA holds 384 x 168 registers (launch bounds): a larger split would block the consumers' setmaxnreg.inc for good
   static_assert(128 * Unit::kProducerRegs + 256 * Unit::kConsumerRegs <= 384 * 168, "setmaxnreg split exceeds the CTA's registers");
-  if (wg == 0) {   // producer warpgroup: one thread issues every load, across work units; wgrad: warps 1..3 build B
+  if (wg == 0) {   // producer warpgroup: one thread issues every load, across work units; warps 1..3 build B or expand int8 X
     setmaxnreg_dec<Unit::kProducerRegs>();
     if (tid == 0) {
       const uint64_t pol = l2_policy_evict_first();
@@ -308,7 +415,8 @@ __device__ __forceinline__ void proj_pipeline(const Params& P, int total) {
         for (int kb = 0; kb < w.kb_n; ++kb) {
           mbar_wait(&empty[s], ph ^ 1u);
           mbar_arrive_expect_tx(&full[s], Unit::kTx);
-          w.issue(smem + s * Cfg::kStage, &full[s], kb, pol);
+          if constexpr (Unit::kRawTx > 0) mbar_arrive_expect_tx(&raw[s], Unit::kRawTx);
+          w.issue(smem + s * Cfg::kStage, &full[s], &raw[s], kb, pol);
           if (++s == Cfg::kStages) { s = 0; ph ^= 1u; }
         }
       }
@@ -318,9 +426,23 @@ __device__ __forceinline__ void proj_pipeline(const Params& P, int total) {
         int s = 0; uint32_t ph = 0;
         for (int u = blockIdx.x; u < total; u += gridDim.x) {
           const Unit w(P, u);
+          [[maybe_unused]] I8Stage<Unit> cv;
+          if constexpr (Unit::kRawTx > 0 && Unit::kScalesPerUnit) {
+            converters_sync();            // every converter is done with the previous unit's scales
+            w.tile_scales(tile_sc, tid - 32);
+            converters_sync();
+            cv.tile_sc = tile_sc;
+          }
           for (int kb = 0; kb < w.kb_n; ++kb) {
-            mbar_wait(&empty[s], ph ^ 1u);
-            w.build(smem + s * Cfg::kStage, kb, warp - 1, lane);
+            if constexpr (Unit::kRawTx > 0) {
+              // the raw box is issued after the stage was released, so its arrival also means the X area is free
+              if constexpr (!Unit::kScalesPerUnit) cv.load_scales(w, kb, tid - 32);
+              mbar_wait(&raw[s], ph);
+              cv.expand(smem + s * Cfg::kStage, tid - 32);
+            } else {
+              mbar_wait(&empty[s], ph ^ 1u);
+              w.build(smem + s * Cfg::kStage, kb, warp - 1, lane);
+            }
             fence_proxy_async_smem();   // the generic-proxy stores -> visible to wgmma
             __syncwarp();
             if (lane == 0) mbar_arrive(&full[s]);
@@ -404,14 +526,16 @@ __device__ __forceinline__ void proj_pipeline(const Params& P, int total) {
   }
 }
 
-template <int D, bool SPLIT, int MB, bool BF16>
+template <int D, bool SPLIT, int MB, XType XT>
 __global__ void __launch_bounds__(384, 1) proj_fwd_tc_kernel(const __grid_constant__ FwdParams P) {
-  proj_pipeline<D, SPLIT, MB, BF16, FwdUnit<D, SPLIT, MB, BF16>>(P, P.total_tiles);
+  constexpr bool BF16 = XT != XType::F32;
+  proj_pipeline<D, SPLIT, MB, BF16, FwdUnit<D, SPLIT, MB, BF16, XT == XType::I8>>(P, P.total_tiles);
 }
 
-template <int D, bool SPLIT, int MB, bool BF16>
+template <int D, bool SPLIT, int MB, XType XT>
 __global__ void __launch_bounds__(384, 1) proj_wgrad_tc_kernel(const __grid_constant__ WgParams P) {
-  proj_pipeline<D, SPLIT, MB, BF16, WgUnit<D, SPLIT, MB, BF16>>(P, P.total_items);
+  constexpr bool BF16 = XT != XType::F32;
+  proj_pipeline<D, SPLIT, MB, BF16, WgUnit<D, SPLIT, MB, BF16, XT == XType::I8>>(P, P.total_items);
 }
 
 static int num_sms() {
@@ -425,45 +549,48 @@ static int num_sms() {
 // MB = 2 (256-wide tiles: half the W / dY^T re-reads from L2) where the accumulators fit (d <= 128) and the tiles still fill every SM
 static int pick_mb(int d, long long units_at_256) { return d <= 128 && units_at_256 >= num_sms() ? 2 : 1; }
 
-template <int D, bool SPLIT, int MB, bool BF16>
+template <int D, bool SPLIT, int MB, XType XT>
 static int launch_fwd(const FwdParams& P, cudaStream_t st) {
-  using Cfg = ProjCfg<D, SPLIT, MB, BF16>;
-  LLMREC_CHECK_CUDA(cudaFuncSetAttribute(proj_fwd_tc_kernel<D, SPLIT, MB, BF16>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Cfg::kSmem));
+  using Cfg = ProjCfg<D, SPLIT, MB, XT != XType::F32>;
+  constexpr uint32_t smem = Cfg::kSmem + (XT == XType::I8 ? Cfg::TM * 4u : 0u);   // int8: + the converters' tile scales
+  static_assert(smem <= kSmemMax, "projection stages and tile scales exceed shared memory");
+  LLMREC_CHECK_CUDA(cudaFuncSetAttribute(proj_fwd_tc_kernel<D, SPLIT, MB, XT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   const int grid = P.total_tiles < num_sms() ? P.total_tiles : num_sms();
-  proj_fwd_tc_kernel<D, SPLIT, MB, BF16><<<grid, 384, Cfg::kSmem, st>>>(P);
+  proj_fwd_tc_kernel<D, SPLIT, MB, XT><<<grid, 384, smem, st>>>(P);
   LLMREC_CHECK_LAUNCH("proj_fwd_tc");
   return 0;
 }
 
-template <int D, bool SPLIT, int MB, bool BF16>
+template <int D, bool SPLIT, int MB, XType XT>
 static int launch_wgrad(const WgParams& P, cudaStream_t st) {
-  using Cfg = ProjCfg<D, SPLIT, MB, BF16>;
-  LLMREC_CHECK_CUDA(cudaFuncSetAttribute(proj_wgrad_tc_kernel<D, SPLIT, MB, BF16>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Cfg::kSmem));
+  using Cfg = ProjCfg<D, SPLIT, MB, XT != XType::F32>;
+  LLMREC_CHECK_CUDA(cudaFuncSetAttribute(proj_wgrad_tc_kernel<D, SPLIT, MB, XT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Cfg::kSmem));
   const int grid = P.total_items < num_sms() ? P.total_items : num_sms();
-  proj_wgrad_tc_kernel<D, SPLIT, MB, BF16><<<grid, 384, Cfg::kSmem, st>>>(P);
+  proj_wgrad_tc_kernel<D, SPLIT, MB, XT><<<grid, 384, Cfg::kSmem, st>>>(P);
   LLMREC_CHECK_LAUNCH("proj_wgrad_tc");
   return 0;
 }
 
 // MB = 2 exists for d <= 128 only (its accumulators at d > 128 would not fit next to the fragments)
-template <int D, bool SPLIT, bool BF16>
+template <int D, bool SPLIT, XType XT>
 static int launch_fwd_mb(const FwdParams& P, int mb, cudaStream_t st) {
-  if constexpr (D <= 128) { if (mb == 2) return launch_fwd<D, SPLIT, 2, BF16>(P, st); }
-  return launch_fwd<D, SPLIT, 1, BF16>(P, st);
+  if constexpr (D <= 128) { if (mb == 2) return launch_fwd<D, SPLIT, 2, XT>(P, st); }
+  return launch_fwd<D, SPLIT, 1, XT>(P, st);
 }
-template <int D, bool SPLIT, bool BF16>
+template <int D, bool SPLIT, XType XT>
 static int launch_wgrad_mb(const WgParams& P, int mb, cudaStream_t st) {
-  if constexpr (D <= 128) { if (mb == 2) return launch_wgrad<D, SPLIT, 2, BF16>(P, st); }
-  return launch_wgrad<D, SPLIT, 1, BF16>(P, st);
+  if constexpr (D <= 128) { if (mb == 2) return launch_wgrad<D, SPLIT, 2, XT>(P, st); }
+  return launch_wgrad<D, SPLIT, 1, XT>(P, st);
 }
 
 #define LLMREC_PROJ_WIDTHS(X) X(32) X(64) X(96) X(128) X(160) X(192) X(224) X(256)
 
-static int fwd_launch(const FwdParams& P, bool split, int mb, bool bf16, cudaStream_t st) {
+static int fwd_launch(const FwdParams& P, bool split, int mb, XType xt, cudaStream_t st) {
   switch (P.d) {
 #define LLMREC_CASE(W) case W: \
-    if (bf16) return split ? launch_fwd_mb<W, true, true>(P, mb, st) : launch_fwd_mb<W, false, true>(P, mb, st); \
-    return split ? launch_fwd_mb<W, true, false>(P, mb, st) : launch_fwd_mb<W, false, false>(P, mb, st);
+    if (xt == XType::I8) return split ? launch_fwd_mb<W, true, XType::I8>(P, mb, st) : launch_fwd_mb<W, false, XType::I8>(P, mb, st); \
+    if (xt == XType::BF16) return split ? launch_fwd_mb<W, true, XType::BF16>(P, mb, st) : launch_fwd_mb<W, false, XType::BF16>(P, mb, st); \
+    return split ? launch_fwd_mb<W, true, XType::F32>(P, mb, st) : launch_fwd_mb<W, false, XType::F32>(P, mb, st);
     LLMREC_PROJ_WIDTHS(LLMREC_CASE)
 #undef LLMREC_CASE
   }
@@ -471,11 +598,12 @@ static int fwd_launch(const FwdParams& P, bool split, int mb, bool bf16, cudaStr
   return 1;
 }
 
-static int wgrad_launch(const WgParams& P, bool split, int mb, bool bf16, cudaStream_t st) {
+static int wgrad_launch(const WgParams& P, bool split, int mb, XType xt, cudaStream_t st) {
   switch (P.d) {
 #define LLMREC_CASE(W) case W: \
-    if (bf16) return split ? launch_wgrad_mb<W, true, true>(P, mb, st) : launch_wgrad_mb<W, false, true>(P, mb, st); \
-    return split ? launch_wgrad_mb<W, true, false>(P, mb, st) : launch_wgrad_mb<W, false, false>(P, mb, st);
+    if (xt == XType::I8) return split ? launch_wgrad_mb<W, true, XType::I8>(P, mb, st) : launch_wgrad_mb<W, false, XType::I8>(P, mb, st); \
+    if (xt == XType::BF16) return split ? launch_wgrad_mb<W, true, XType::BF16>(P, mb, st) : launch_wgrad_mb<W, false, XType::BF16>(P, mb, st); \
+    return split ? launch_wgrad_mb<W, true, XType::F32>(P, mb, st) : launch_wgrad_mb<W, false, XType::F32>(P, mb, st);
     LLMREC_PROJ_WIDTHS(LLMREC_CASE)
 #undef LLMREC_CASE
   }
@@ -639,19 +767,32 @@ __global__ void __launch_bounds__(256) colsum_kernel(const ColsumParams P) {
 // ------------------------------------------------------------------------------------------------
 // host API (grouped)
 // ------------------------------------------------------------------------------------------------
-// bf16 X: a 16-byte TMA row pitch needs ldx % 8 == 0, and the bf16 W terms [3d x k] need k % 8 == 0
-bool proj_tc_supported(int d, int64_t ldx, const void* X, int k, bool wgrad, bool bf16) {
+// bf16 X: a 16-byte TMA row pitch needs ldx % 8 == 0, and the bf16 W terms [3d x k] need k % 8 == 0.  int8 X (ldx = the row pitch in
+// bytes): k % 16 == 0 and a 16-byte pitch, so that the raw boxes and the row scales are aligned.
+bool proj_tc_supported(int d, int64_t ldx, const void* X, int k, bool wgrad, XType xt) {
   (void)wgrad;   // both directions take d in multiples of 32 (wgmma N = d)
-  const int q = bf16 ? 8 : 4;
+  const int q = xt == XType::I8 ? 16 : xt == XType::BF16 ? 8 : 4;
   return d % 32 == 0 && d >= 32 && d <= 256 && ldx % q == 0 && aligned16(X) && k >= 1 && k % q == 0;
 }
 
 static CUtensorMapDataType x_type(bool bf16) { return bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32; }
 
-// bf16: pr[p].X holds the address of a bf16 table (llmrec_proj_fwd_problem_bf16 carried in the fp32 struct's layout)
+// The X tensor map: fp32 / bf16 boxes with the 128-byte swizzle; int8 boxes of raw q without swizzle, over the k logical columns of the
+// rows (the padding and the scale past them are never loaded: columns past k read as zeros)
+static bool x_tmap(CUtensorMap* m, XType xt, const void* X, int k, int64_t n, int64_t ldx, uint32_t box_k, uint32_t box_rows) {
+  if (xt == XType::I8) return make_tmap_2d(m, CU_TENSOR_MAP_DATA_TYPE_UINT8, X, (uint64_t)k, (uint64_t)n, (uint64_t)ldx, box_k, box_rows, false);
+  return make_tmap_2d(m, x_type(xt == XType::BF16), X, (uint64_t)k, (uint64_t)n, (uint64_t)ldx * (xt == XType::BF16 ? 2 : 4), box_k, box_rows);
+}
+
+static void set_row_scales(RowScales& xs, int p, XType xt, const void* X, int k, int64_t ldx) {
+  xs.scale[p] = xt == XType::I8 ? static_cast<const uint8_t*>(X) + i8_scale_offset(k) : nullptr;
+  xs.pitch[p] = xt == XType::I8 ? ldx : 0;
+}
+
+// bf16 / int8: pr[p].X holds the address of a bf16 / int8 table (the _bf16 / _i8 problem carried in the fp32 struct's layout)
 // rows: NULL, or n_prob optional output row maps (X row r of problem p -> Y row rows[p][r])
-int proj_fwd_tc_group(const llmrec_proj_fwd_problem* pr, const int32_t* const* rows, int n_prob, int d, int mode, bool bf16, cudaStream_t st) {
-  const bool split = (mode == 0);
+int proj_fwd_tc_group(const llmrec_proj_fwd_problem* pr, const int32_t* const* rows, int n_prob, int d, int mode, XType xt, cudaStream_t st) {
+  const bool split = (mode == 0), bf16 = xt != XType::F32;    // int8 X runs the bf16 kernels on expanded stages
   const bool need_ws = split || bf16;          // bf16 kernels read W as bf16 terms in both modes
   const int es = bf16 ? 2 : 4, bk = stage_k(bf16);
   FwdParams P;
@@ -677,12 +818,13 @@ int proj_fwd_tc_group(const llmrec_proj_fwd_problem* pr, const int32_t* const* r
     // an empty problem has no tiles (and a tensor map cannot have an empty dimension); its W is still split when a later problem shares it
     if (pr[p].n > 0) {
       const int pieces = split ? (bf16 ? 3 : 2) : 1;
-      if (!make_tmap_2d(&P.tmA[p], x_type(bf16), pr[p].X, (uint64_t)pr[p].k, (uint64_t)pr[p].n, (uint64_t)pr[p].ldx * es, bk, (uint32_t)tm)) return 4;
+      if (!x_tmap(&P.tmA[p], xt, pr[p].X, pr[p].k, pr[p].n, pr[p].ldx, bk, (uint32_t)tm)) return 4;
       if (!make_tmap_2d(&P.tmW[p], x_type(bf16), wsrc, (uint64_t)pr[p].k, (uint64_t)(pieces * d), (uint64_t)pr[p].k * es, bk, (uint32_t)d)) return 4;
     }
     P.prob[p].n = (int)pr[p].n; P.prob[p].k = pr[p].k; P.prob[p].kblocks = (pr[p].k + bk - 1) / bk;
     P.prob[p].tile_start = tiles; P.prob[p].ldy = pr[p].ldy; P.prob[p].Y = pr[p].Y; P.prob[p].bias = pr[p].bias;
     P.prob[p].rows = rows ? rows[p] : nullptr;
+    set_row_scales(P.xs, p, xt, pr[p].X, pr[p].k, pr[p].ldx);
     tiles += (int)((pr[p].n + tm - 1) / tm);
   }
   P.total_tiles = tiles;
@@ -692,7 +834,7 @@ int proj_fwd_tc_group(const llmrec_proj_fwd_problem* pr, const int32_t* const* r
     LLMREC_CHECK_LAUNCH("wsplit");
   }
   if (tiles <= 0) return 0;
-  return fwd_launch(P, split, mb, bf16, st);
+  return fwd_launch(P, split, mb, xt, st);
 }
 
 static int wg_rows_per_chunk(int64_t n) {
@@ -732,18 +874,18 @@ static void wg_plan(const llmrec_proj_wgrad_problem* pr, int n_prob, int d, int 
   W.total = off;
 }
 
-int64_t proj_wgrad_tc_scratch(const llmrec_proj_wgrad_problem* pr, int n_prob, int d, int mode, bool bf16) {
+int64_t proj_wgrad_tc_scratch(const llmrec_proj_wgrad_problem* pr, int n_prob, int d, int mode, XType xt) {
   WgPlan W;
-  wg_plan(pr, n_prob, d, mode, bf16, W);
+  wg_plan(pr, n_prob, d, mode, xt != XType::F32, W);
   return W.total;   // the colsum ticket must start at zero; the kernel re-zeroes it
 }
 
-// bf16: pr[p].X holds the address of a bf16 table (llmrec_proj_wgrad_problem_bf16 carried in the fp32 struct's layout)
+// bf16 / int8: pr[p].X holds the address of a bf16 / int8 table (the _bf16 / _i8 problem carried in the fp32 struct's layout)
 // rows / n_dy: NULL, or per problem an optional dY row map (X row r pairs with dY row rows[p][r]; NULL = identity) and the row count
 // of dY (n without a map), over all of which the bias sums run (the map changes only which dY rows the weight gradient reads)
 int proj_wgrad_tc_group(const llmrec_proj_wgrad_problem* pr, const int32_t* const* rows, const int64_t* n_dy, int n_prob, int d, int mode,
-                        bool bf16, float* scratch, int64_t scratch_elems, cudaStream_t st) {
-  const bool split = (mode == 0);
+                        XType xt, float* scratch, int64_t scratch_elems, cudaStream_t st) {
+  const bool split = (mode == 0), bf16 = xt != XType::F32;    // int8 X runs the bf16 kernels on expanded stages
   const int es = bf16 ? 2 : 4, bk = stage_k(bf16), pieces = split ? (bf16 ? 3 : 2) : 1;
   const bool build_b = wg_builds_b(mode, bf16);
   WgPlan W;
@@ -768,11 +910,13 @@ int proj_wgrad_tc_group(const llmrec_proj_wgrad_problem* pr, const int32_t* cons
     // an empty problem has no work items (and a tensor map cannot have an empty dimension); colsum and the reduce still
     // write its dW / db: zeros, or the prior under accumulate
     if (pr[p].n > 0) {
-      if (!make_tmap_2d(&P.tmX[p], x_type(bf16), pr[p].X, (uint64_t)pr[p].k, (uint64_t)pr[p].n, (uint64_t)pr[p].ldx * es, bk, bk)) return 4;
+      // boxes [bk rows][bk features] (int8: 64 x 64 bytes of raw q)
+      if (!x_tmap(&P.tmX[p], xt, pr[p].X, pr[p].k, pr[p].n, pr[p].ldx, bk, bk)) return 4;
       if (!build_b &&
           !make_tmap_2d(&P.tmG[p], x_type(bf16), dyt, (uint64_t)pr[p].n, (uint64_t)(pieces * d), (uint64_t)W.ldt[p] * es, bk, (uint32_t)d)) return 4;
     }
     P.dY[p] = pr[p].dY; P.lddy[p] = pr[p].lddy; P.rows[p] = map;
+    set_row_scales(P.xs, p, xt, pr[p].X, pr[p].k, pr[p].ldx);
     T.dY[p] = pr[p].dY; T.ld[p] = pr[p].lddy; T.n[p] = (int)pr[p].n; T.out[p] = dyt; T.ldt[p] = W.ldt[p]; T.rows[p] = map;
     n_max = pr[p].n > n_max ? pr[p].n : n_max;
     C.dY[p] = pr[p].dY; C.ld[p] = pr[p].lddy; C.n[p] = n_dy ? n_dy[p] : pr[p].n; C.db[p] = pr[p].db;
@@ -816,7 +960,7 @@ int proj_wgrad_tc_group(const llmrec_proj_wgrad_problem* pr, const int32_t* cons
       else dyt_split_kernel<false><<<grid, 256, 0, st>>>(T);
       LLMREC_CHECK_LAUNCH("dyt_split");
     }
-    int rc = wgrad_launch(P, split, W.mb, bf16, st);
+    int rc = wgrad_launch(P, split, W.mb, xt, st);
     if (rc) return rc;
   }
   ReduceParams R;

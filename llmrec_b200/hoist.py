@@ -26,7 +26,7 @@ from __future__ import annotations
 
 import torch
 
-from . import ops
+from . import feat_int8, ops
 from .engine import HotPath, HotPathConfig
 
 
@@ -48,7 +48,10 @@ class HoistedHotPath(HotPath):
         f, dev = self.feats, self.E_u.device
         names = ["image", "text"] + ["item:" + k for k in self.keys] + ["user"]
         raw = [f["image"], f["text"]] + [f["item"][k] for k in self.keys] + [f["user"]]
-        widths = [int(x.shape[1]) for x in raw]
+        w_of = ["image_trans", "text_trans"] + ["item_trans"] * len(self.keys) + ["user_trans"]
+        # the logical widths come from the weights (an int8 table's rows are wider: values, padding and the row scale)
+        widths = [int(self.p[w + ".weight"].shape[1]) for w in w_of]
+        wide = lambda X, w: feat_int8.dequantize(X, w) if X.dtype == torch.int8 else X.float()
         self.col0 = [0]
         for w in widths:
             self.col0.append(self.col0[-1] + w)
@@ -57,13 +60,13 @@ class HoistedHotPath(HotPath):
         self.Kc = Kc
         TU = torch.zeros(self.nu, Kc, dtype=torch.float32, device=dev)
         TI = torch.zeros(self.ni, Kc, dtype=torch.float32, device=dev)
-        # bf16 feature tables (--feat_dtype bf16) are widened to fp32 one table at a time for these one-time products; TU / TI stay fp32
+        # bf16 / int8 feature tables (--feat_dtype) are widened to fp32 one table at a time for these one-time products; TU / TI stay fp32
         for j, X in enumerate(raw[:-1]):                          # item-side raw tables: TU_s = ui.X, TI_s = iu.TU_s
             c0, w = self.col0[j], widths[j]
-            self.ui.apply([(X.float(), TU[:, c0:c0 + w], None, False)])
+            self.ui.apply([(wide(X, w), TU[:, c0:c0 + w], None, False)])
             self.iu.apply([(TU[:, c0:c0 + w], TI[:, c0:c0 + w], None, False)])
         c0, w = self.col0[-2], widths[-1]                          # user table: TI_usr = iu.X_usr (prof_i), TU_usr = ui.TI_usr (prof_u)
-        self.iu.apply([(raw[-1].float(), TI[:, c0:c0 + w], None, False)])
+        self.iu.apply([(wide(raw[-1], w), TI[:, c0:c0 + w], None, False)])
         self.ui.apply([(TI[:, c0:c0 + w], TU[:, c0:c0 + w], None, False)])
         sc = self.col0[-1]
         TU[:, sc] = gs["cu"]; TU[:, sc + 1] = gs["ru"]             # Fu bias scale, prof_u bias scale

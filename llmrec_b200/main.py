@@ -68,8 +68,9 @@ class Trainer(object):
         args = self.args = get_args()
         if not torch.cuda.is_available():
             raise RuntimeError("llmrec_b200.Trainer needs a CUDA (H100) device: there is no CPU fallback")
-        if getattr(args, "feat_dtype", "fp32") == "bf16" and (args.mask or args.mask_rate > 0):
-            raise ValueError("--feat_dtype bf16 cannot be combined with --mask / --mask_rate > 0: the mask branch overwrites rows of the "
+        feat_dtype = getattr(args, "feat_dtype", "fp32")
+        if feat_dtype in ("bf16", "int8") and (args.mask or args.mask_rate > 0):
+            raise ValueError(f"--feat_dtype {feat_dtype} cannot be combined with --mask / --mask_rate > 0: the mask branch overwrites rows of the "
                              "feature tables with fp32 column means in place (Trainer._mask_features); use --feat_dtype fp32")
         self.device = torch.device(device)
         self.task_name = "%s_%s_%s" % (datetime.now().strftime("%Y-%m-%d %H:%M:%S"), args.dataset, args.cf_model)
@@ -216,7 +217,8 @@ class Trainer(object):
                 f[i_mask] = f.mean(0)
             self.hot.refresh_item_feats(i_mask)                           # the compact tables of the live items (engine.HotPath)
         u_mask = torch.randperm(self.n_users)[:int(args.mask_rate * self.n_users)].to(self.device)
-        m.user_feats[u_mask] = m.user_feats.mean(0)
+        if u_mask.numel():                # (--drop_rate alone masks no row; a bf16 / int8 table has no fp32 mean to write)
+            m.user_feats[u_mask] = m.user_feats.mean(0)
         return i_mask, u_mask
 
     @staticmethod

@@ -14,6 +14,7 @@ import numpy as np
 import torch
 
 from . import _native as N
+from . import feat_int8
 
 
 STATS = {"launches": 0}     # kernels of libllmrec_b200 launched through this module (bench.py reports it)
@@ -226,18 +227,31 @@ def _get_scratch(key, n, device, zero=False):
     return t
 
 
-FEAT_DTYPES = (torch.float32, torch.bfloat16)     # element types of the side-feature table X the projections accept
+FEAT_DTYPES = (torch.float32, torch.bfloat16, torch.int8)     # element types of the side-feature table X the projections accept
 
 
 def _feat(X, name="X"):
-    """X of a projection: a CUDA fp32 or bf16 row-major 2-D tensor (column slices fine)."""
+    """X of a projection: a CUDA fp32 or bf16 row-major 2-D tensor (column slices fine), or an int8 table (feat_int8)."""
     if X.dim() != 2 or X.dtype not in FEAT_DTYPES or not X.is_cuda or (X.shape[1] > 1 and X.stride(1) != 1):
-        raise ValueError(f"{name}: need a CUDA fp32 or bf16 row-major 2-D tensor, got {tuple(X.shape)} {X.dtype} {X.device} strides {X.stride()}")
+        raise ValueError(f"{name}: need a CUDA fp32, bf16 or int8 row-major 2-D tensor, got {tuple(X.shape)} {X.dtype} {X.device} strides {X.stride()}")
     return X
 
 
+def _feat_k(X, k, what):
+    """Logical width of X for a problem whose weights are k wide: X's width, or for an int8 table the k its row pitch must hold."""
+    if X.dtype == torch.int8:
+        if X.shape[1] != feat_int8.pitch(k):
+            raise ValueError(f"{what}: an int8 table of width k = {k} has rows of {feat_int8.pitch(k)} bytes, got {X.shape[1]}")
+        return k
+    return int(X.shape[1])
+
+
+_PROBLEMS = {torch.float32: (N.ProjFwdProblem, N.ProjWgradProblem, "f32"), torch.bfloat16: (N.ProjFwdProblemBf16, N.ProjWgradProblemBf16, "bf16"),
+             torch.int8: (N.ProjFwdProblemI8, N.ProjWgradProblemI8, "i8")}
+
+
 def _group_dtype(Xs, what):
-    """The one X dtype of a grouped call: a bf16 group runs the _bf16 entry points, and one call never mixes the two."""
+    """The one X dtype of a grouped call: a bf16 / int8 group runs the _bf16 / _i8 entry points, and one call never mixes them."""
     dt = {X.dtype for X in Xs}
     if len(dt) != 1:
         raise ValueError(f"{what}: every problem of one call must share the X dtype, got {sorted(str(t) for t in dt)}")
@@ -246,7 +260,7 @@ def _group_dtype(Xs, what):
 
 def _f32(t, name):
     if t is not None and t.dtype != torch.float32:
-        raise ValueError(f"{name}: must be fp32 (only the feature table X may be bf16), got {t.dtype}")
+        raise ValueError(f"{name}: must be fp32 (only the feature table X may be bf16 or int8), got {t.dtype}")
     return t
 
 
@@ -272,26 +286,28 @@ def _problem_array(prob_type, n, mapped):
 
 def proj_fwd_group(problems, d, mode=0):
     """problems: list of (X[n x k], W[d x k], bias[d]|None, out[m x d] [, rows]).  One grouped launch (wgmma) --
-    the 8 nn.Linear calls of Models.py:145-150.  Problems sharing W share the split buffer.  X is fp32 or bf16 (all problems
-    alike); W, bias and out are fp32.  rows (optional, int32 CUDA [n]): X row r is written to out[rows[r]], the other rows of out
-    are left untouched (without it m == n and row r goes to out[r]); a written row gets the bits of the full-table call."""
-    bf16 = _group_dtype([_feat(pr[0]) for pr in problems], "proj_fwd") == torch.bfloat16
-    arr, recs, _blk = _problem_array(N.ProjFwdProblemBf16 if bf16 else N.ProjFwdProblem, len(problems), any(len(pr) > 4 and pr[4] is not None for pr in problems))
+    the 8 nn.Linear calls of Models.py:145-150.  Problems sharing W share the split buffer.  X is fp32, bf16 or an int8 table
+    (feat_int8; k is then W's width) -- all problems alike; W, bias and out are fp32.  rows (optional, int32 CUDA [n]): X row r is
+    written to out[rows[r]], the other rows of out are left untouched (without it m == n and row r goes to out[r]); a written row
+    gets the bits of the full-table call."""
+    dt = _group_dtype([_feat(pr[0]) for pr in problems], "proj_fwd")
+    bf16 = dt != torch.float32             # bf16 and int8 run the bf16 kernels: W as bf16 terms
+    prob_t, _, suffix = _PROBLEMS[dt]
+    arr, recs, _blk = _problem_array(prob_t, len(problems), any(len(pr) > 4 and pr[4] is not None for pr in problems))
     for i, (X, W, b, out, *rows) in enumerate(problems):
         _mat(out); _f32(W, "proj_fwd W"); _f32(b, "proj_fwd bias")
-        n, k = X.shape
+        n, k = int(X.shape[0]), _feat_k(X, int(W.shape[1]) if W.dim() == 2 else -1, "proj_fwd")
         rows = _row_map(rows[0] if rows else None, n, "proj_fwd")
         if not W.is_contiguous() or tuple(W.shape) != (d, k) or out.shape[1] != d or (rows is None and out.shape[0] != n):
             raise ValueError("proj_fwd: bad shapes")
         # the bf16 kernels read W as bf16 terms in modes 0 and 1: 3dk (or dk) bf16 in the 2dk floats of the fp32 hi/lo split
         ws = _get_scratch(("wsplit", W.data_ptr()), 2 * d * k, X.device) if mode == 0 or (bf16 and mode == 1) else None
-        arr[i] = (N.ProjFwdProblemBf16 if bf16 else N.ProjFwdProblem)(_p(X), _p(W), _p(b), _p(out), _p(ws), _ld(X), _ld(out), n, k,
-                                                                        0 if rows is None else N.PROJ_ROW_MAP)
+        arr[i] = prob_t(_p(X), _p(W), _p(b), _p(out), _p(ws), _ld(X), _ld(out), n, k, 0 if rows is None else N.PROJ_ROW_MAP)
         if rows is not None:
             recs[i] = N.ProjRowMap(_p(rows), int(out.shape[0]))
     lib = N.lib()
     if bf16:
-        N.check(lib.llmrec_proj_fwd_group_bf16(arr, len(problems), d, mode, _stream()), "proj_fwd_group_bf16")
+        N.check(getattr(lib, "llmrec_proj_fwd_group_" + suffix)(arr, len(problems), d, mode, _stream()), "proj_fwd_group_" + suffix)
     else:
         N.check(lib.llmrec_proj_fwd_group_f32(arr, len(problems), d, mode, _stream()), "proj_fwd_group")
     _count((2 if mode == 0 or (bf16 and mode == 1) else 1) * -(-len(problems) // 8))
@@ -305,26 +321,28 @@ def proj_fwd(X, W, b, out, mode=0):
 
 def proj_wgrad_group(problems, d, mode=0):
     """problems: list of (X[n x k], dY[m x d], dW[d x k], db[d]|None, accumulate [, rows]).  dW (+)= dY^T X ; db (+)= colsum(dY).
-    X is fp32 or bf16 (all problems alike); dY, dW and db are fp32.  rows (optional, int32 CUDA [n]): X row r pairs with dY[rows[r]]
-    (without it m == n); db still sums all m rows of dY, so it gets the bits of the full-table call, and dW differs from it by rounding."""
-    bf16 = _group_dtype([_feat(pr[0]) for pr in problems], "proj_wgrad") == torch.bfloat16
-    arr, recs, _blk = _problem_array(N.ProjWgradProblemBf16 if bf16 else N.ProjWgradProblem, len(problems),
-                                     any(len(pr) > 5 and pr[5] is not None for pr in problems))
+    X is fp32, bf16 or an int8 table (feat_int8; k is then dW's width) -- all problems alike; dY, dW and db are fp32.  rows (optional,
+    int32 CUDA [n]): X row r pairs with dY[rows[r]] (without it m == n); db still sums all m rows of dY, so it gets the bits of the
+    full-table call, and dW differs from it by rounding."""
+    dt = _group_dtype([_feat(pr[0]) for pr in problems], "proj_wgrad")
+    _, prob_t, suffix = _PROBLEMS[dt]
+    arr, recs, _blk = _problem_array(prob_t, len(problems), any(len(pr) > 5 and pr[5] is not None for pr in problems))
     for i, (X, dY, dW, db, acc, *rows) in enumerate(problems):
         _mat(dY); _f32(dW, "proj_wgrad dW"); _f32(db, "proj_wgrad db")
-        n, k = X.shape
+        n, k = int(X.shape[0]), _feat_k(X, int(dW.shape[1]) if dW.dim() == 2 else -1, "proj_wgrad")
         rows = _row_map(rows[0] if rows else None, n, "proj_wgrad")
         if not dW.is_contiguous() or tuple(dW.shape) != (d, k) or dY.shape[1] != d or (rows is None and dY.shape[0] != n):
             raise ValueError("proj_wgrad: bad shapes")
         flags = (N.WGRAD_ACCUMULATE if acc else 0) | (0 if rows is None else N.PROJ_ROW_MAP)
-        arr[i] = (N.ProjWgradProblemBf16 if bf16 else N.ProjWgradProblem)(_p(X), _p(dY), _p(dW), _p(db), _ld(X), _ld(dY), n, k, flags)
+        arr[i] = prob_t(_p(X), _p(dY), _p(dW), _p(db), _ld(X), _ld(dY), n, k, flags)
         if rows is not None:
             recs[i] = N.ProjRowMap(_p(rows), int(dY.shape[0]))
     lib = N.lib()
-    need = int((lib.llmrec_proj_wgrad_group_bf16_scratch if bf16 else lib.llmrec_proj_wgrad_group_scratch)(arr, len(problems), d, mode))
+    name = "llmrec_proj_wgrad_group" + ("" if dt == torch.float32 else "_" + suffix)
+    need = int(getattr(lib, name + "_scratch")(arr, len(problems), d, mode))
     scratch = _get_scratch(("wgrad", problems[0][0].device.index), need, problems[0][0].device, zero=True) if need else None     # holds a ticket word
-    if bf16:
-        N.check(lib.llmrec_proj_wgrad_group_bf16(arr, len(problems), d, mode, _p(scratch), need, _stream()), "proj_wgrad_group_bf16")
+    if dt != torch.float32:
+        N.check(getattr(lib, name)(arr, len(problems), d, mode, _p(scratch), need, _stream()), "proj_wgrad_group_" + suffix)
     else:
         N.check(lib.llmrec_proj_wgrad_group_f32(arr, len(problems), d, mode, _p(scratch), need, _stream()), "proj_wgrad_group")
     _count(4 if need else len(problems))

@@ -22,8 +22,9 @@ def spmm_bytes(nnz, M, N, d, segs=1):
 
 
 def proj_bytes(n, k, d, x_bytes=4):
-    """Y[n x d] = X[n x k] W^T (or its weight gradient): X read once at x_bytes per element (4 fp32, 2 bf16), fp32 W and Y."""
-    return x_bytes * n * k + 4 * k * d + 4 * n * d
+    """Y[n x d] = X[n x k] W^T (or its weight gradient): X read once at x_bytes per element (4 fp32, 2 bf16, 1 int8 -- plus the
+    int8 table's fp32 row scale, 4 per row), fp32 W and Y."""
+    return x_bytes * n * k + (4 * n if x_bytes == 1 else 0) + 4 * k * d + 4 * n * d
 
 
 def step_bytes(hp, nnz):
@@ -31,9 +32,10 @@ def step_bytes(hp, nnz):
     nu, ni, d, S, L = hp.nu, hp.ni, hp.d, hp.S, hp.L
     out = {}
     if hp.has_feats:
-        f = hp.feats
+        f, p = hp.feats, hp.p
         nl = getattr(hp, "n_live", ni)         # the item-side problems read the live items' rows only (engine.HotPath._build_live_items)
-        gemms = [(nl, f["image"].shape[1]), (nl, f["text"].shape[1])] + [(nl, v.shape[1]) for v in f["item"].values()] + [(nu, f["user"].shape[1])]
+        k = lambda name: int(p[name + ".weight"].shape[1])      # logical widths from the weights (an int8 row also holds its scale)
+        gemms = [(nl, k("image_trans")), (nl, k("text_trans"))] + [(nl, k("item_trans"))] * len(f["item"]) + [(nu, k("user_trans"))]
         xb = f["image"].element_size()
         out["proj_fwd"] = out["proj_wgrad"] = sum(proj_bytes(n, k, d, xb) for n, k in gemms)
     sp = lambda M, N, segs: spmm_bytes(nnz, M, N, d, segs)

@@ -79,9 +79,11 @@ _EXTRA = [
                                                    "batch's rows per step (SURVEY.md 8f-3); same results within the golden tolerances; off automatically "
                                                    "when drop_rate > 0 or the mask branch is on")),
     ("device_sampler", dict(type=int, default=0, help="1: draw the batches on the GPU (non-parity RNG stream, SURVEY.md 8f-1); 0 replays the reference's host sampling")),
-    ("feat_dtype", dict(default="fp32", choices=["fp32", "bf16"], help="element type the side-feature tables (image, text, user profile, "
+    ("feat_dtype", dict(default="fp32", choices=["fp32", "bf16", "int8"], help="element type the side-feature tables (image, text, user profile, "
                                                                       "attributes) are kept in: bf16 rounds them once (round-to-nearest-even) "
                                                                       "when the model is built and halves their memory and projection reads; "
+                                                                      "int8 quantizes each row once to int8 values and a power-of-two scale "
+                                                                      "(every stored value an exact bf16), a quarter of the fp32 bytes; "
                                                                       "the projections are then exact on the rounded tables. Not with the mask branch")),
 ]
 
