@@ -294,6 +294,31 @@ int llmrec_bpr_heads_f32(const llmrec_bpr_head* heads_host, int32_t n_heads,
                          float* work /* llmrec_bpr_work_elems() floats, zeroed once */, llmrec_stream_t stream);
 int64_t llmrec_bpr_work_elems(int32_t n_heads, int32_t B);
 
+/* Ordered (bit-reproducible) form of the heads' row gradients.  Forward values (`out`, loss) are those of llmrec_bpr_heads_f32;
+ * the row gradients are gathered instead of scattered with float atomics.  Definition of the result: every element G[row, j]
+ * starts from the value it holds at the call (what llmrec_grad_init_f32 left: zero, or c * X) and takes its contributions one
+ * fp32 add at a time (each add flushes denormals, as the device's float atomic does), in this order:
+ *   1. heads in ascending index;  2. within a head, ascending batch position b;  3. at one position, pos[b] before neg[b].
+ * Each contribution is computed by the instructions of the atomic form, and its early-outs are kept (a triplet with g == 0 of a
+ * head with w_emb == 0 adds nothing; a head with GU == GI == NULL is skipped), so a row with one contribution gets the atomic
+ * form's bits and every result is one the atomic form could have produced.  The bits do not depend on the grid, the stream
+ * schedule or timing.  Heads that accumulate into one buffer must name it by the same pointer and leading dimension (the
+ * attribute heads' shared Gprof_u); gradient buffers of different pointers must not overlap.
+ * llmrec_bpr_slot_plan sorts the batch's slots -- user slots b; item slots 2b (pos) and 2b + 1 (neg) -- by (row, slot) into
+ * `plan` (llmrec_bpr_slot_plan_elems(B) int32).  It reads the index arrays (and meta[0]) only, so it may run on another stream
+ * as soon as they are staged; the ordered call must be ordered after it.  B is the capacity as above; entries past the live
+ * length are never read.  Capacity: B <= 65536 triplets (an argument error above; there is no fall-back to the atomic form).
+ * Any d and leading dimensions; a row that occurs many times in one batch is walked by one warp per destination buffer. */
+int64_t llmrec_bpr_slot_plan_elems(int32_t B);
+int llmrec_bpr_slot_plan(const int32_t* users, const int32_t* pos, const int32_t* neg, int32_t B, const int32_t* meta,
+                         int32_t* plan, llmrec_stream_t stream);
+int llmrec_bpr_heads_ordered_f32(const llmrec_bpr_head* heads_host, int32_t n_heads,
+                                 const int32_t* users, const int32_t* pos, const int32_t* neg, int32_t B,
+                                 int32_t n_keep, const int32_t* meta, float regs0_over_bs, int32_t d,
+                                 float* out /* [n_heads*4] */, float* loss_accum /* [1], += */,
+                                 float* work /* llmrec_bpr_work_elems() floats, zeroed once */,
+                                 const int32_t* plan /* llmrec_bpr_slot_plan of the same index arrays */, llmrec_stream_t stream);
+
 /* First touch of every gradient buffer of a step, one launch instead of a memset per buffer: region r is written
  * G_r[n x width] = X_r ? c_r * X_r : 0, and *loss = sum_r 0.5 * c_r * sum(X_r^2) (OVERWRITTEN: this is the first term of
  * the step's loss) -- feat_reg_loss_calculation (main.py:151-156) and its gradient for the regions with X, plain zeroing
@@ -400,6 +425,11 @@ int llmrec_gather_rows_f32(const float* X, int64_t ldx, const int32_t* idx, int3
                            llmrec_stream_t stream);
 int llmrec_scatter_add_rows_f32(const float* G, int64_t ldg, const int32_t* idx, int32_t n, int32_t d, float* Y, int64_t ldy,
                                 llmrec_stream_t stream);
+/* Ordered form of llmrec_scatter_add_rows_f32: Y[idx[b], :] += G[b, :] one fp32 add at a time in ascending b (idx[b] < 0
+ * skipped), so the result does not depend on the schedule.  n <= 131072; scratch: llmrec_scatter_add_rows_ordered_scratch(n) int32. */
+int llmrec_scatter_add_rows_ordered_f32(const float* G, int64_t ldg, const int32_t* idx, int32_t n, int32_t d, float* Y, int64_t ldy,
+                                        int32_t* scratch, int64_t scratch_elems, llmrec_stream_t stream);
+int64_t llmrec_scatter_add_rows_ordered_scratch(int32_t n);
 
 /* ---------------------------------------------------------------------------------------------
  * Hoisted side-feature mode (SURVEY.md 8f-3; Models.py:145-167 with dropout p = 0 and the mask branch off):

@@ -124,7 +124,8 @@ class MM_Model(nn.Module):
                                 mm_mf_rate=args.mm_mf_rate, prune_loss_drop_rate=args.prune_loss_drop_rate,
                                 feat_reg_decay=args.feat_reg_decay, regs0=eval(args.regs)[0], batch_size=args.batch_size,
                                 aug_sample_rate=args.aug_sample_rate,
-                                proj_mode=PROJ_MODE[getattr(args, "proj_mode", "3xtf32")])
+                                proj_mode=PROJ_MODE[getattr(args, "proj_mode", "3xtf32")],
+                                deterministic=bool(getattr(args, "deterministic", 0)))
             if hoisted:
                 from .hoist import HoistedHotPath
                 self._hp = HoistedHotPath((ui_f, iu_f, ui_b, iu_b), params, feats, cfg, graph_scalars)

@@ -130,6 +130,10 @@ SIGNATURES = {
     "llmrec_bpr_heads_f32": (C.c_int, [C.POINTER(BprHead), C.c_int32, c_i32p, c_i32p, c_i32p, C.c_int32, C.c_int32, c_i32p, C.c_float,
                                        C.c_int32, c_f32p, c_f32p, c_f32p, c_stream]),
     "llmrec_bpr_work_elems": (C.c_int64, [C.c_int32, C.c_int32]),
+    "llmrec_bpr_slot_plan_elems": (C.c_int64, [C.c_int32]),
+    "llmrec_bpr_slot_plan": (C.c_int, [c_i32p, c_i32p, c_i32p, C.c_int32, c_i32p, c_i32p, c_stream]),
+    "llmrec_bpr_heads_ordered_f32": (C.c_int, [C.POINTER(BprHead), C.c_int32, c_i32p, c_i32p, c_i32p, C.c_int32, C.c_int32, c_i32p, C.c_float,
+                                               C.c_int32, c_f32p, c_f32p, c_f32p, c_i32p, c_stream]),
     "llmrec_sqnorm_grad_f32": (C.c_int, [c_f32p, C.c_int64, c_f32p, C.c_int64, C.c_int64, C.c_int32, C.c_float, C.c_int32,
                                          c_f32p, c_f32p, c_stream]),
     "llmrec_adamw_advance": (C.c_int, [C.c_void_p, C.c_double, C.c_double, C.c_double, c_stream]),
@@ -150,6 +154,8 @@ SIGNATURES = {
     "llmrec_row_scale_softmax_f32": (C.c_int, [c_f32p, C.c_int64, c_f32p, c_f32p, C.c_int64, C.c_int64, C.c_int32, C.c_int32, c_stream]),
     "llmrec_gather_rows_f32": (C.c_int, [c_f32p, C.c_int64, c_i32p, C.c_int32, C.c_int32, c_f32p, C.c_int64, c_stream]),
     "llmrec_scatter_add_rows_f32": (C.c_int, [c_f32p, C.c_int64, c_i32p, C.c_int32, C.c_int32, c_f32p, C.c_int64, c_stream]),
+    "llmrec_scatter_add_rows_ordered_f32": (C.c_int, [c_f32p, C.c_int64, c_i32p, C.c_int32, C.c_int32, c_f32p, C.c_int64, c_i32p, C.c_int64, c_stream]),
+    "llmrec_scatter_add_rows_ordered_scratch": (C.c_int64, [C.c_int32]),
     "llmrec_rank1_add_f32": (C.c_int, [C.POINTER(Rank1Block), C.c_int32, c_stream]),
     "llmrec_scaled_colsum_f32": (C.c_int, [C.POINTER(ColsumTerm), C.c_int32, C.c_int32, c_f32p, C.c_int32, c_f32p, c_stream]),
     "llmrec_scaled_colsum_scratch": (C.c_int64, [C.c_int32]),

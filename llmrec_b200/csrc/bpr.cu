@@ -9,7 +9,8 @@
 //               n_keep smallest log-sigmoids of that head with a 4-pass radix select over order-preserving keys
 //               (O(B), ties -> lower batch position like the reference's stable argsort), sums them in a fixed
 //               order, and emits the per-triplet gradient coefficients; the last head adds the weighted losses;
-//   bpr_grad    scatter-add of the row gradients.
+//   bpr_grad    scatter-add of the row gradients (float atomics), or bpr_grad_ordered: the same sums gathered in a fixed order from a
+//               slot plan (slot_rank), bit-reproducible.
 // The live batch length B' and n_keep may come from a 2-int DEVICE block (`meta`), so one captured CUDA graph
 // serves every batch length up to the capacity the grid was sized for.
 #include "common.cuh"
@@ -243,6 +244,168 @@ __global__ void __launch_bounds__(256) bpr_grad_kernel(const BprParams p) {
   }
 }
 
+// ---- ordered row gradients (deterministic form of bpr_grad) --------------------------------------------------------
+// G[row, j] starts from what grad_init left and takes its contributions one fp32 add at a time: heads in ascending index,
+// within a head ascending batch position, at one position pos before neg.  Gather, not scatter: the slot plan lists the
+// batch's slots sorted by (row, slot) -- user slots b, item slots 2b (pos) and 2b + 1 (neg) -- so the slots of one row are a
+// run in slot order.  The warp at the first entry of a run owns that row of one destination buffer: it folds every head that
+// writes the buffer, in head order, in registers and stores each element once; the warps at the other entries retire.
+//
+// Plan layout (int32, 6 * cap): slot_u[cap] row_u[cap] slot_i[2 cap] row_i[2 cap]; only the live prefixes are written / read.
+// slot_rank_kernel: one warp per slot counts the slots that sort before it -- its rank; keys (row, slot) are unique, so the
+// ranks are a permutation whatever the schedule.  O(n^2 / 32) per warp-step: 2 252 item slots at the netflix batch are 71
+// iterations per warp; at the capacity limit (131 072 slots) it is milliseconds, which is why the limit is where it is.
+constexpr int kOrderedMaxSlots = 1 << 17;
+
+__device__ __forceinline__ bool sorts_before(int rt, int t, int r, int s) { return rt < r || (rt == r && t < s); }
+
+// a (and b: slots 2i -> a[i], 2i + 1 -> b[i]); n_host entries per array, or min(*n_dev, n_host)
+__global__ void __launch_bounds__(256) slot_rank_kernel(const int* __restrict__ a, const int* __restrict__ b, int n_host, const int* __restrict__ n_dev,
+                                                        int* __restrict__ slot_out, int* __restrict__ row_out) {
+  const int lane = threadIdx.x & 31;
+  int n = n_host;
+  if (n_dev) { const int c = __ldg(n_dev); n = c < n ? c : n; }
+  const int s = blockIdx.x * 8 + (threadIdx.x >> 5);
+  if (s >= (b ? 2 * n : n)) return;
+  const int r = b ? ((s & 1) ? b[s >> 1] : a[s >> 1]) : a[s];
+  int rank = 0;
+  if (b) {
+    for (int i = lane; i < n; i += 32) rank += (int)sorts_before(a[i], 2 * i, r, s) + (int)sorts_before(b[i], 2 * i + 1, r, s);
+  } else {
+    for (int i = lane; i < n; i += 32) rank += (int)sorts_before(a[i], i, r, s);
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) rank += __shfl_xor_sync(0xffffffffu, rank, o);
+  if (lane == 0) { slot_out[rank] = s; row_out[rank] = r; }
+}
+
+// the float atomic of bpr_grad / scatter_add_rows is an add that flushes denormals; so is every add of the ordered forms
+__device__ __forceinline__ float add_ftz(float a, float b) {
+  float r;
+  asm("add.rn.ftz.f32 %0, %1, %2;" : "=f"(r) : "f"(a), "f"(b));
+  return r;
+}
+
+// length of the run of `row` in rowv[q0 .. n) as seen by this warp's 32 lanes (<= 32; 32 = the run may go on)
+__device__ __forceinline__ int run_ahead(const int* __restrict__ rowv, int q0, int n, int row) {
+  const int q = q0 + (threadIdx.x & 31);
+  const unsigned m = __ballot_sync(0xffffffffu, q < n && rowv[q] == row);
+  return m == 0xffffffffu ? 32 : __ffs(~m) - 1;
+}
+
+constexpr int kMaxOrdGroups = 2 * kMaxHeads;
+struct OrdGroup { float* G; int64_t ldg; unsigned heads; };      // one destination buffer and the heads (bit h) that accumulate into it
+struct OrdParams { OrdGroup grp[kMaxOrdGroups]; int n_user_groups; const int* plan; };
+
+__global__ void __launch_bounds__(256) bpr_grad_ordered_kernel(const BprParams p, const OrdParams o) {
+  const int lane = threadIdx.x & 31;
+  const bool item = (int)blockIdx.y >= o.n_user_groups;
+  const int B = live_B(p);
+  const int n = item ? 2 * B : B;
+  const int q_first = blockIdx.x * 8 + (threadIdx.x >> 5);
+  if (q_first >= n) return;
+  const int* slotv = o.plan + (item ? 2 * (size_t)p.cap : 0);
+  const int* rowv = slotv + (item ? 2 * (size_t)p.cap : (size_t)p.cap);
+  const int row = rowv[q_first];
+  if (q_first > 0 && rowv[q_first - 1] == row) return;      // not the first slot of its row
+  const OrdGroup gr = o.grp[blockIdx.y];
+  float* dst = gr.G + (int64_t)row * gr.ldg;
+  for (int jb = 0; jb < p.d; jb += 128) {                   // 4 columns per lane and pass; every lane walks (the walk shuffles)
+    const int j0 = jb + lane;
+    float acc[4];
+#pragma unroll
+    for (int c = 0; c < 4; ++c) acc[c] = j0 + 32 * c < p.d ? dst[j0 + 32 * c] : 0.f;
+    for (unsigned hm = gr.heads; hm; hm &= hm - 1) {
+      const int h = __ffs(hm) - 1;
+      const float* XU = p.head[h].XU; const float* XI = p.head[h].XI;
+      const int64_t ldxu = p.head[h].ldxu, ldxi = p.head[h].ldxi;
+      const bool no_emb = p.head[h].w_emb == 0.f;
+      const float* w = work_of(p, h);
+      const float* gco = w + 5 * (size_t)p.cap;
+      const float eu = w[7 * (size_t)p.cap + 0], ep = w[7 * (size_t)p.cap + 1], en = w[7 * (size_t)p.cap + 2];
+      for (int q0 = q_first; q0 < n; q0 += 32) {
+        const int cnt = run_ahead(rowv, q0, n, row);
+        // lane k fetches what slot k of the run needs; the walk below broadcasts it
+        int s_l = 0, iu_l = 0, io_l = 0; float g_l = 0.f;
+        if (lane < cnt) {
+          s_l = slotv[q0 + lane];
+          const int b = item ? s_l >> 1 : s_l;
+          g_l = gco[b]; iu_l = p.users[b];
+          io_l = item ? ((s_l & 1) ? p.neg[b] : p.pos[b]) : p.pos[b];
+          if (!item) s_l = p.neg[b];
+        }
+        for (int k = 0; k < cnt; ++k) {
+          const float g = __shfl_sync(0xffffffffu, g_l, k);
+          const int s = __shfl_sync(0xffffffffu, s_l, k), iu = __shfl_sync(0xffffffffu, iu_l, k), io = __shfl_sync(0xffffffffu, io_l, k);
+          if (g == 0.f && no_emb) continue;                 // bpr_grad's early-out: this triplet adds nothing, not even a zero
+          const float* u = XU + (int64_t)iu * ldxu;
+          const float* x = XI + (int64_t)io * ldxi;         // user rows: the positive item; item rows: this slot's item
+          // the three contributions below are the instructions nvcc emits for bpr_grad's g*(q-r)+eu*a, g*a+ep*q, -g*a+en*r,
+          // spelled out so that the two kernels cannot contract them differently
+          if (!item) {
+            const float* y = XI + (int64_t)s * ldxi;        // s carries neg[b] on the user side
+#pragma unroll
+            for (int c = 0; c < 4; ++c) {
+              const int j = j0 + 32 * c;
+              if (j < p.d) acc[c] = add_ftz(acc[c], __fmaf_rn(eu, u[j], __fmul_rn(g, x[j] - y[j])));
+            }
+          } else if (!(s & 1)) {
+#pragma unroll
+            for (int c = 0; c < 4; ++c) {
+              const int j = j0 + 32 * c;
+              if (j < p.d) acc[c] = add_ftz(acc[c], __fmaf_rn(ep, x[j], __fmul_rn(g, u[j])));
+            }
+          } else {
+#pragma unroll
+            for (int c = 0; c < 4; ++c) {
+              const int j = j0 + 32 * c;
+              if (j < p.d) acc[c] = add_ftz(acc[c], __fmaf_rn(en, x[j], -__fmul_rn(g, u[j])));
+            }
+          }
+        }
+        if (cnt < 32) break;
+      }
+    }
+#pragma unroll
+    for (int c = 0; c < 4; ++c) if (j0 + 32 * c < p.d) dst[j0 + 32 * c] = acc[c];
+  }
+}
+
+// The same machinery for a plain row scatter: Y[idx[b], :] += G[b, :] in ascending b (idx[b] < 0 skipped; they sort first).
+// plan (int32, 2 * n): slot[n] row[n] from slot_rank_kernel over idx.
+__global__ void __launch_bounds__(256) scatter_add_rows_ordered_kernel(const float* __restrict__ G, int64_t ldg, const int* __restrict__ plan, int n, int d,
+                                                                       float* __restrict__ Y, int64_t ldy) {
+  const int lane = threadIdx.x & 31;
+  const int q_first = blockIdx.x * 8 + (threadIdx.x >> 5);
+  if (q_first >= n) return;
+  const int* slotv = plan;
+  const int* rowv = plan + n;
+  const int row = rowv[q_first];
+  if (row < 0 || (q_first > 0 && rowv[q_first - 1] == row)) return;
+  float* dst = Y + (int64_t)row * ldy;
+  for (int jb = 0; jb < d; jb += 128) {
+    const int j0 = jb + lane;
+    float acc[4];
+#pragma unroll
+    for (int c = 0; c < 4; ++c) acc[c] = j0 + 32 * c < d ? dst[j0 + 32 * c] : 0.f;
+    for (int q0 = q_first; q0 < n; q0 += 32) {
+      const int cnt = run_ahead(rowv, q0, n, row);
+      const int s_l = lane < cnt ? slotv[q0 + lane] : 0;
+      for (int k = 0; k < cnt; ++k) {
+        const float* g = G + (int64_t)__shfl_sync(0xffffffffu, s_l, k) * ldg;
+#pragma unroll
+        for (int c = 0; c < 4; ++c) {
+          const int j = j0 + 32 * c;
+          if (j < d) acc[c] = add_ftz(acc[c], g[j]);
+        }
+      }
+      if (cnt < 32) break;
+    }
+#pragma unroll
+    for (int c = 0; c < 4; ++c) if (j0 + 32 * c < d) dst[j0 + 32 * c] = acc[c];
+  }
+}
+
 // feat_reg: loss += c * 0.5 * sum(X^2);  G = (acc ? G : 0) + c * X
 __global__ void __launch_bounds__(256) sqnorm_grad_kernel(const float* X, int64_t ldx, float* G, int64_t ldg, int64_t n, int d,
                                                           float c, int accumulate, float* partial) {
@@ -322,14 +485,10 @@ using namespace llmrec;
 
 extern "C" int64_t llmrec_bpr_work_elems(int32_t n_heads, int32_t B) { return kWorkHdr + (int64_t)n_heads * (7 * (int64_t)B + 8); }
 
-extern "C" int llmrec_bpr_heads_f32(const llmrec_bpr_head* heads, int32_t n_heads,
-                                    const int32_t* users, const int32_t* pos, const int32_t* neg, int32_t B,
-                                    int32_t n_keep, const int32_t* meta, float regs0_over_bs, int32_t d,
-                                    float* out, float* loss_accum, float* work, llmrec_stream_t stream) {
-  LLMREC_REQUIRE_DEVICE();
+static int bpr_params(BprParams& p, const llmrec_bpr_head* heads, int32_t n_heads, const int32_t* users, const int32_t* pos, const int32_t* neg,
+                      int32_t B, int32_t n_keep, const int32_t* meta, float regs0_over_bs, int32_t d, float* out, float* loss_accum, float* work) {
   LLMREC_CHECK_ARG(n_heads >= 1 && n_heads <= kMaxHeads, "bpr: n_heads=%d out of range", n_heads);
   LLMREC_CHECK_ARG(B >= 1 && B <= (1 << 24), "bpr: batch capacity %d unsupported", B);
-  BprParams p{};
   for (int h = 0; h < n_heads; ++h) p.head[h] = heads[h];
   p.n_heads = n_heads; p.users = users; p.pos = pos; p.neg = neg; p.cap = B; p.meta = meta; p.B_host = B; p.n_keep_host = n_keep;
   p.c_emb = regs0_over_bs; p.d = d;
@@ -337,12 +496,93 @@ extern "C" int llmrec_bpr_heads_f32(const llmrec_bpr_head* heads, int32_t n_head
   // the head of `work` holds the per-head tickets + the head counter (zeroed by the caller once; the kernel re-zeroes them)
   static_assert(kMaxHeads + 1 <= kWorkHdr, "ticket block");
   p.counters = reinterpret_cast<unsigned*>(work);
+  return 0;
+}
+
+extern "C" int llmrec_bpr_heads_f32(const llmrec_bpr_head* heads, int32_t n_heads,
+                                    const int32_t* users, const int32_t* pos, const int32_t* neg, int32_t B,
+                                    int32_t n_keep, const int32_t* meta, float regs0_over_bs, int32_t d,
+                                    float* out, float* loss_accum, float* work, llmrec_stream_t stream) {
+  LLMREC_REQUIRE_DEVICE();
+  BprParams p{};
+  if (int rc = bpr_params(p, heads, n_heads, users, pos, neg, B, n_keep, meta, regs0_over_bs, d, out, loss_accum, work)) return rc;
   cudaStream_t st = as_stream(stream);
   dim3 grid((B + 7) / 8, n_heads);
   bpr_forward_kernel<<<grid, kSelThreads, 0, st>>>(p);
   LLMREC_CHECK_LAUNCH("bpr_forward");
   bpr_grad_kernel<<<grid, 256, 0, st>>>(p);
   LLMREC_CHECK_LAUNCH("bpr_grad");
+  return 0;
+}
+
+extern "C" int64_t llmrec_bpr_slot_plan_elems(int32_t B) { return 6 * (int64_t)B; }
+
+extern "C" int llmrec_bpr_slot_plan(const int32_t* users, const int32_t* pos, const int32_t* neg, int32_t B, const int32_t* meta,
+                                    int32_t* plan, llmrec_stream_t stream) {
+  LLMREC_REQUIRE_DEVICE();
+  LLMREC_CHECK_ARG(B >= 1 && 2 * (int64_t)B <= kOrderedMaxSlots, "bpr_slot_plan: batch capacity %d unsupported (the ordered form takes up to %d triplets)",
+                   B, kOrderedMaxSlots / 2);
+  LLMREC_CHECK_ARG(plan, "bpr_slot_plan: plan is NULL");
+  cudaStream_t st = as_stream(stream);
+  slot_rank_kernel<<<(B + 7) / 8, 256, 0, st>>>(users, nullptr, B, meta, plan, plan + B);
+  LLMREC_CHECK_LAUNCH("slot_rank(users)");
+  slot_rank_kernel<<<(2 * B + 7) / 8, 256, 0, st>>>(pos, neg, B, meta, plan + 2 * (size_t)B, plan + 4 * (size_t)B);
+  LLMREC_CHECK_LAUNCH("slot_rank(items)");
+  return 0;
+}
+
+extern "C" int llmrec_bpr_heads_ordered_f32(const llmrec_bpr_head* heads, int32_t n_heads,
+                                            const int32_t* users, const int32_t* pos, const int32_t* neg, int32_t B,
+                                            int32_t n_keep, const int32_t* meta, float regs0_over_bs, int32_t d,
+                                            float* out, float* loss_accum, float* work, const int32_t* plan, llmrec_stream_t stream) {
+  LLMREC_REQUIRE_DEVICE();
+  BprParams p{};
+  if (int rc = bpr_params(p, heads, n_heads, users, pos, neg, B, n_keep, meta, regs0_over_bs, d, out, loss_accum, work)) return rc;
+  LLMREC_CHECK_ARG(2 * (int64_t)B <= kOrderedMaxSlots, "bpr_heads_ordered: batch capacity %d unsupported (the ordered form takes up to %d triplets)",
+                   B, kOrderedMaxSlots / 2);
+  LLMREC_CHECK_ARG(plan, "bpr_heads_ordered: plan is NULL (build it with llmrec_bpr_slot_plan)");
+  // destination buffers: heads that name the same GU (or GI) are folded by one warp in head order; user-side buffers first
+  OrdParams o{};
+  o.plan = plan;
+  int ng = 0;
+  for (int side = 0; side < 2; ++side) {
+    for (int h = 0; h < n_heads; ++h) {
+      if (!heads[h].GU && !heads[h].GI) continue;           // bpr_grad skips such a head altogether
+      float* G = side ? heads[h].GI : heads[h].GU;
+      const int64_t ld = side ? heads[h].ldgi : heads[h].ldgu;
+      if (!G) continue;
+      int g = side ? o.n_user_groups : 0;
+      while (g < ng && o.grp[g].G != G) ++g;
+      if (g == ng) { o.grp[ng].G = G; o.grp[ng].ldg = ld; o.grp[ng].heads = 0u; ++ng; }
+      LLMREC_CHECK_ARG(o.grp[g].ldg == ld, "bpr_heads_ordered: heads that share a gradient buffer must share its leading dimension (head %d)", h);
+      o.grp[g].heads |= 1u << h;
+    }
+    if (!side) o.n_user_groups = ng;
+  }
+  cudaStream_t st = as_stream(stream);
+  bpr_forward_kernel<<<dim3((B + 7) / 8, n_heads), kSelThreads, 0, st>>>(p);
+  LLMREC_CHECK_LAUNCH("bpr_forward");
+  if (ng) {
+    bpr_grad_ordered_kernel<<<dim3((2 * B + 7) / 8, ng), 256, 0, st>>>(p, o);
+    LLMREC_CHECK_LAUNCH("bpr_grad_ordered");
+  }
+  return 0;
+}
+
+extern "C" int64_t llmrec_scatter_add_rows_ordered_scratch(int32_t n) { return 2 * (int64_t)(n > 0 ? n : 0); }
+
+extern "C" int llmrec_scatter_add_rows_ordered_f32(const float* G, int64_t ldg, const int32_t* idx, int32_t n, int32_t d, float* Y, int64_t ldy,
+                                                   int32_t* scratch, int64_t scratch_elems, llmrec_stream_t stream) {
+  LLMREC_REQUIRE_DEVICE();
+  if (n <= 0) return 0;
+  LLMREC_CHECK_ARG(n <= kOrderedMaxSlots, "scatter_add_rows_ordered: %d rows unsupported (the ordered form takes up to %d)", n, kOrderedMaxSlots);
+  LLMREC_CHECK_ARG(scratch && scratch_elems >= 2 * (int64_t)n, "scatter_add_rows_ordered: scratch too small (%lld < %lld int32)", (long long)scratch_elems,
+                   2 * (long long)n);
+  cudaStream_t st = as_stream(stream);
+  slot_rank_kernel<<<(n + 7) / 8, 256, 0, st>>>(idx, nullptr, n, nullptr, scratch, scratch + n);
+  LLMREC_CHECK_LAUNCH("slot_rank(idx)");
+  scatter_add_rows_ordered_kernel<<<(n + 7) / 8, 256, 0, st>>>(G, ldg, scratch, n, d, Y, ldy);
+  LLMREC_CHECK_LAUNCH("scatter_add_rows_ordered");
   return 0;
 }
 

@@ -104,6 +104,8 @@ class ShardedHotPath:
         all-reduce): the scale/softmax after each forward exchange runs on 1/world of the rows, and the item table's AdamW
         state and update are sharded by item (the updated rows are all-gathered instead of the gradient)."""
         self.g, self.cfg, self.group = graph, cfg, group
+        if cfg.deterministic:
+            raise ValueError("deterministic steps are not implemented for the sharded engines (their loss heads and row exchanges scatter with float atomics)")
         self.world = dist.get_world_size(group) if (dist.is_initialized() and not solo) else 1
         self.item_sharded = bool(item_sharded) and self.world > 1 and E_i.shape[0] % self.world == 0
         self.E_u, self.E_i = E_u_local, E_i

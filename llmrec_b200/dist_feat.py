@@ -32,6 +32,8 @@ class ShardedFeatureHotPath:
 
     def __init__(self, graph: ShardedGraph, params, feats_local, cfg: HotPathConfig, user_lo: int, item_lo: int, group=None):
         self.g, self.cfg, self.group, self.p, self.f = graph, cfg, group, params, feats_local
+        if cfg.deterministic:
+            raise ValueError("deterministic steps are not implemented for the sharded engines (their loss heads and row exchanges scatter with float atomics)")
         self.world = dist.get_world_size(group) if dist.is_initialized() else 1
         self.E_u, self.E_i = params["user_id_embedding.weight"], params["item_id_embedding.weight"]
         nu, ni, d, L = self.E_u.shape[0], self.E_i.shape[0], cfg.embed_size, cfg.n_layers

@@ -30,6 +30,12 @@ dUl / dIl instead, and the side-feature gradients already hold their final value
 after a training step: `forward()` (evaluation, MM_Model, the eager mask / MAE branch) fuses every row.  At the netflix shape the two
 fusion families drop from 0.041 + 0.081 ms to 0.008 + 0.011 ms (H100 SXM 80 GB HBM3, 700 W; DESIGN §5).
 
+Deterministic steps (`HotPathConfig.deterministic`, off by default): the loss heads' scatter of row gradients is the one launch of the
+default 3xTF32 / TF32 step whose float adds land in a schedule-dependent order (a batch repeats users and items, and the attribute heads
+share Gprof_u).  When set, the same branch that builds the row sets sorts the batch's slots by (row, slot) (`ops.bpr_slot_plan`, from the
+index buffer alone), and the heads gather each destination row in a fixed order -- heads ascending, batch positions ascending, pos before
+neg (include/llmrec_b200.h) -- so two runs of a step give the same bits, graph or eager, with or without branches.
+
 Live items: Pi[i] is read only by Fu = ui . Pi, and only when item i is a column of ui; GPi[i] = (ui^T GFu)[i] is an empty row, exactly
 zero, when item i has no training edge.  So the projections skip those rows: `_build_live_items` fixes the set of items with a training
 edge once (the non-empty rows of ui^T), copies their rows of the item-side tables into compact tables (`fx`), and zeroes Pi once.  The
@@ -63,6 +69,7 @@ class HotPathConfig:
     batch_size: int = 1024
     aug_sample_rate: float = 0.1      # main.py:218: a batch grows by at most int(batch_size * rate) augmented triplets
     proj_mode: int = 0                # ops.PROJ_MODE
+    deterministic: bool = False       # loss-head row gradients accumulated in a fixed order instead of with float atomics (bit-reproducible steps)
 
 
 PARAM_ORDER = ("image_trans.weight", "image_trans.bias", "text_trans.weight", "text_trans.bias",
@@ -103,6 +110,9 @@ class HotPath:
     def __init__(self, operators, params, feats, cfg: HotPathConfig):
         self.ui, self.iu, self.uiT, self.iuT = operators
         self.cfg = cfg
+        if cfg.deterministic and cfg.proj_mode == 2:
+            raise ValueError("deterministic steps need the tensor-core projections (proj_mode 3xtf32 / tf32): the fp32 SIMT weight gradient "
+                             "adds its row chunks with float atomics")
         self.p = params
         self.feats = feats
         d, L = cfg.embed_size, cfg.n_layers
@@ -134,6 +144,7 @@ class HotPath:
         self.n_heads = (3 + len(self.keys)) if self.has_feats else 1
         self.head_out = torch.zeros(self.n_heads * 4, dtype=torch.float32, device=dev)
         self._bpr_work, self._cap, self._graph = None, 0, None
+        self._slot_plan = None            # cfg.deterministic: the step's slot plan (ops.bpr_slot_plan), sized with _bpr_work
         self.pre_step = None              # optional launches replayed in front of every staged step (device-side batch sampler)
         self.pre_step_undo = None         # undoes the side effect of ONE pre_step (the warm-up step before a capture must not consume a batch)
         self.opt = None
@@ -416,8 +427,8 @@ class HotPath:
         return (c.batch_size + int(c.batch_size * c.aug_sample_rate) + 7) // 8 * 8
 
     def ensure_capacity(self, cap):
-        """Index buffer [4 x cap] (rows users, pos, neg, meta = {B', n_keep}), the per-B' meta table and the BPR work block,
-        sized ONCE for a batch capacity: every captured graph reads these addresses, so they are only ever replaced together
+        """Index buffer [4 x cap] (rows users, pos, neg, meta = {B', n_keep}), the per-B' meta table, the BPR work block and (deterministic
+        steps) the slot plan, sized ONCE for a batch capacity: every captured graph reads these addresses, so they are only ever replaced together
         with the graphs (ADVICE r1: a per-B' work buffer freed under a live graph was a use-after-free)."""
         if getattr(self, "_cap", 0) >= cap:
             return
@@ -430,11 +441,14 @@ class HotPath:
         keep = [int((1 - self.cfg.prune_loss_drop_rate) * b) for b in range(self._cap + 1)]      # main.py:161-162 (double arithmetic)
         self._meta_table = torch.tensor([[b, k] for b, k in enumerate(keep)], dtype=torch.int32).to(dev)
         self._bpr_work = ops.bpr_work(self.n_heads, self._cap, dev)
+        if self.cfg.deterministic:
+            self._slot_plan = torch.zeros(6 * self._cap, dtype=torch.int32, device=dev)
 
-    def loss_and_output_grads(self, users, pos, neg, meta=None, init_done=False):
+    def loss_and_output_grads(self, users, pos, neg, meta=None, init_done=False, plan_done=False):
         """users/pos/neg: int32 CUDA tensors of equal length B' (sampled + augmented triplets) -- or, with `meta` (int32 CUDA
         {B', n_keep}), capacity-sized buffers whose first B' entries are live (the CUDA-graph path).
-        init_done: `_grad_init` already ran for this step (train_step forks it beside the tail of the forward pass)."""
+        init_done: `_grad_init` already ran for this step (train_step forks it beside the tail of the forward pass).
+        plan_done: the slot plan of a deterministic step was already built from these index arrays (train_step's row-set branch)."""
         c = self.cfg
         B = int(users.numel())
         self.ensure_capacity(max(B, self.batch_capacity()))
@@ -448,8 +462,14 @@ class HotPath:
         if not init_done:
             self._grad_init()
         with self._t("bpr"):
-            ops.bpr_heads(heads, users, pos, neg, n_keep, c.regs0 / c.batch_size, self.head_out, self.loss, self._bpr_work, meta=meta)
+            if c.deterministic and not plan_done:
+                self._plan_slots(users, pos, neg, meta)
+            ops.bpr_heads(heads, users, pos, neg, n_keep, c.regs0 / c.batch_size, self.head_out, self.loss, self._bpr_work, meta=meta,
+                          **({"ordered": self._slot_plan} if c.deterministic else {}))
         return self.loss
+
+    def _plan_slots(self, users, pos, neg, meta=None):
+        ops.bpr_slot_plan(users, pos, neg, meta=meta, plan=self._slot_plan)
 
     def _grad_init(self, id_grads=False):
         """First touch of every gradient buffer the loss heads accumulate into: the feat_reg gradient c*X on the image/text blocks (its
@@ -474,10 +494,19 @@ class HotPath:
         if self.opt is None:
             raise RuntimeError("attach an optimizer with set_optimizer() first")
         split = self.has_feats and self.timer is None and (self.branches or self.force_split)
-        demand = self.demand_fuse
-        if demand:
-            # the batch's row sets depend on the indices only: a branch from the start of the step, joined before the fusion
-            self._fork(lambda: self._batch_rows(users, pos, neg, meta), lane=1)
+        demand, det = self.demand_fuse, self.cfg.deterministic
+        if det:
+            self.ensure_capacity(max(int(users.numel()), self.batch_capacity()))     # the slot plan is filled before the heads size anything
+        if demand or det:
+            # the batch's row sets and the slot plan of a deterministic step depend on the indices only: a branch from the start of the step,
+            # joined before the fusion
+            def index_branch():
+                if demand:
+                    self._batch_rows(users, pos, neg, meta)
+                if det:
+                    self._plan_slots(users, pos, neg, meta)
+
+            self._fork(index_branch, lane=1)
         grad_init = lambda: self._grad_init(id_grads=demand)
         if split:
             # the ID layers do not depend on the projections: they run as a branch (through operators with their own long-row scratch)
@@ -503,7 +532,7 @@ class HotPath:
         self._join([1])                                                      # the row sets
         self._fuse_fwd(batch_rows=demand)                                    # joins
         self._join()
-        self.loss_and_output_grads(users, pos, neg, meta, init_done=True)
+        self.loss_and_output_grads(users, pos, neg, meta, init_done=True, plan_done=det)
         if split:
             self._fuse_bwd(batch_rows=demand)
             self._fork(lambda: self._chain_bwd(with_feats=False, opset=ids[2:]), lane=0)    # ID chain

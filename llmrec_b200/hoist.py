@@ -118,6 +118,8 @@ class HoistedHotPath(HotPath):
                  GFu=new(cap, S * d), GFi=new(2 * cap, S * d), Gpu=new(cap, d), Gpi=new(2 * cap, d),
                  U=new(cap, d), I=new(2 * cap, d), gU=new(cap, d), gI=new(2 * cap, d), dU=new(cap, d), dI=new(2 * cap, d),
                  ar=torch.arange(cap, dtype=torch.int32, device=dev), ar2=torch.arange(cap, 2 * cap, dtype=torch.int32, device=dev))
+        if self.cfg.deterministic:                                # rank scratch of the two ordered scatters (they may overlap: one each)
+            c.update(rank_u=torch.zeros(2 * cap, dtype=torch.int32, device=dev), rank_i=torch.zeros(4 * cap, dtype=torch.int32, device=dev))
         self._compact = c
         return c
 
@@ -140,6 +142,11 @@ class HoistedHotPath(HotPath):
         g = self.grads
         creg = cfg.feat_reg_decay / self.ni
         reg_names = ("image_trans", "text_trans")
+        det = cfg.deterministic
+        # deterministic steps: the compact blocks give every triplet rows of its own, so the heads' only shared destination is Gpu (the
+        # attribute heads, folded in head order), and the scatters of dU / dI into the dense tables (a batch repeats users and items)
+        # add in ascending batch position
+        scatter = (lambda G, idx, Y, key: ops.scatter_add_rows_ordered(G, idx, Y, scratch=c[key])) if det else (lambda G, idx, Y, key: ops.scatter_add_rows(G, idx, Y))
 
         # ---- branches: ID layers | first touch of the gradient buffers + feat_reg  ||  main: the batch's side-feature rows ----
         def init_branch():
@@ -155,6 +162,8 @@ class HoistedHotPath(HotPath):
                 for j, name in enumerate(reg_names):
                     G, h, n2 = self.gram[j]
                     ops.feat_reg_gram(p[name + ".weight"], p[name + ".bias"], G, h, n2, creg, g[name + ".weight"], g[name + ".bias"], self.loss)
+            if det:
+                self._plan_slots(c["ar"], c["ar"], c["ar2"], meta)
 
         self._fork(lambda: self._prop_fwd(with_feats=False), lane=0)                          # ID layers (Models.py:169-183)
         self._fork(init_branch, lane=1)
@@ -189,19 +198,20 @@ class HoistedHotPath(HotPath):
             heads.append((c["pu"], blk(c["Fi"], 2 + j), c["Gpu"], blk(c["GFi"], 2 + j), cfg.aug_mf_rate, 0.0))
         n_keep = int((1 - cfg.prune_loss_drop_rate) * cap)
         with self._t("bpr"):
-            ops.bpr_heads(heads, c["ar"], c["ar"], c["ar2"], n_keep, cfg.regs0 / cfg.batch_size, self.head_out, self.loss, self._bpr_work, meta=meta)
+            ops.bpr_heads(heads, c["ar"], c["ar"], c["ar2"], n_keep, cfg.regs0 / cfg.batch_size, self.head_out, self.loss, self._bpr_work, meta=meta,
+                          **({"ordered": self._slot_plan} if det else {}))
         # ---- backward: fusion on the compact rows, ID gradients scattered into the dense chain ----
         dsu = [blk(c["GFu"], 0), blk(c["GFu"], 1), c["Gpu"]] + [blk(c["GFu"], 2 + j) for j in range(len(self.keys))]
         dsi = [blk(c["GFi"], 0), blk(c["GFi"], 1), c["Gpi"]] + [blk(c["GFi"], 2 + j) for j in range(len(self.keys))]
 
         def user_side_bwd():
             ops.fuse_bwd(c["gU"], L + 1, c["dU"], su, coefs, dsu, True)
-            ops.scatter_add_rows(c["dU"], users, self.dUl)                                    # rows past B' carry zero gradients
+            scatter(c["dU"], users, self.dUl, "rank_u")                                       # rows past B' carry zero gradients
 
         with self._t("fuse_bwd"):
             self._fork(user_side_bwd)
             ops.fuse_bwd(c["gI"], L + 1, c["dI"], si, coefs, dsi, True)
-            ops.scatter_add_rows(c["dI"], pn, self.dIl)
+            scatter(c["dI"], pn, self.dIl, "rank_i")
             self._join()
         # ---- branch: the dense ID chain  ||  main: weight / bias gradients from the compact rows ----
         self._fork(lambda: self._chain_bwd(with_feats=False), lane=0)

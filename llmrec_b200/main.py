@@ -72,6 +72,9 @@ class Trainer(object):
         if feat_dtype in ("bf16", "int8") and (args.mask or args.mask_rate > 0):
             raise ValueError(f"--feat_dtype {feat_dtype} cannot be combined with --mask / --mask_rate > 0: the mask branch overwrites rows of the "
                              "feature tables with fp32 column means in place (Trainer._mask_features); use --feat_dtype fp32")
+        if getattr(args, "deterministic", 0) and (args.mask or args.mask_rate > 0 or args.drop_rate > 0):
+            raise ValueError("--deterministic 1 cannot be combined with --mask / --mask_rate > 0 / --drop_rate > 0: that branch accumulates with "
+                             "torch's index_add_ and runs the Decoder backward, whose summation orders are not fixed")
         self.device = torch.device(device)
         self.task_name = "%s_%s_%s" % (datetime.now().strftime("%Y-%m-%d %H:%M:%S"), args.dataset, args.cf_model)
         self.logger = Logger(filename=self.task_name, is_debug=args.debug)

@@ -425,9 +425,26 @@ def bpr_work(n_heads, B, device):
     return torch.zeros(int(N.lib().llmrec_bpr_work_elems(n_heads, B)), dtype=torch.float32, device=device)
 
 
-def bpr_heads(heads, users, pos, neg, n_keep, regs0_over_bs, out, loss, work, meta=None):
+def bpr_slot_plan(users, pos, neg, meta=None, plan=None):
+    """Slot plan of the ordered row gradients (llmrec_bpr_slot_plan): the batch's user slots and pos | neg item slots sorted by (row, slot).
+    It reads the index arrays (and meta[0]) only.  plan: int32 CUDA buffer of llmrec_bpr_slot_plan_elems(B) entries to fill (made when None).
+    Capacities past 65 536 triplets raise."""
+    B = int(users.numel())
+    need = int(N.lib().llmrec_bpr_slot_plan_elems(B))
+    if plan is None:
+        plan = torch.zeros(need, dtype=torch.int32, device=users.device)
+    if _i32(plan, "plan").numel() < need:
+        raise ValueError("bpr_slot_plan: plan buffer too small for this capacity")
+    N.check(N.lib().llmrec_bpr_slot_plan(_p(_i32(users)), _p(_i32(pos)), _p(_i32(neg)), B, _p(meta), _p(plan), _stream()), "bpr_slot_plan")
+    _count(2)
+    return plan
+
+
+def bpr_heads(heads, users, pos, neg, n_keep, regs0_over_bs, out, loss, work, meta=None, ordered=None):
     """heads: list of (XU, XI, GU|None, GI|None, w_mf, w_emb).  See include/llmrec_b200.h.
-    meta: optional int32 CUDA tensor {live B', n_keep}; users/pos/neg/work are then sized for the capacity B."""
+    meta: optional int32 CUDA tensor {live B', n_keep}; users/pos/neg/work are then sized for the capacity B.
+    ordered: a `bpr_slot_plan` of the same index arrays: the row gradients are then accumulated in the fixed order of
+    llmrec_bpr_heads_ordered_f32 (bit-reproducible) instead of with float atomics; loss and `out` are the same either way."""
     arr = (N.BprHead * len(heads))()
     d = int(heads[0][0].shape[1])
     for i, (XU, XI, GU, GI, wmf, wemb) in enumerate(heads):
@@ -437,8 +454,13 @@ def bpr_heads(heads, users, pos, neg, n_keep, regs0_over_bs, out, loss, work, me
     B = int(users.numel())
     if work.numel() < N.lib().llmrec_bpr_work_elems(len(heads), B):
         raise ValueError("bpr_heads: work buffer too small for this capacity")
-    N.check(N.lib().llmrec_bpr_heads_f32(arr, len(heads), _p(_i32(users)), _p(_i32(pos)), _p(_i32(neg)), B, int(n_keep), _p(meta),
-                                          float(regs0_over_bs), d, _p(out), _p(loss), _p(work), _stream()), "bpr_heads")
+    args = (arr, len(heads), _p(_i32(users)), _p(_i32(pos)), _p(_i32(neg)), B, int(n_keep), _p(meta), float(regs0_over_bs), d, _p(out), _p(loss), _p(work))
+    if ordered is not None:
+        if _i32(ordered, "plan").numel() < N.lib().llmrec_bpr_slot_plan_elems(B):
+            raise ValueError("bpr_heads: the slot plan was built for a smaller capacity")
+        N.check(N.lib().llmrec_bpr_heads_ordered_f32(*args, _p(ordered), _stream()), "bpr_heads_ordered")
+    else:
+        N.check(N.lib().llmrec_bpr_heads_f32(*args, _stream()), "bpr_heads")
     _count(2)
 
 
@@ -584,6 +606,18 @@ def gather_rows(X, idx, out):
 def scatter_add_rows(G, idx, Y):
     N.check(N.lib().llmrec_scatter_add_rows_f32(_p(_mat(G)), _ld(G), _p(_i32(idx)), idx.numel(), G.shape[1], _p(_mat(Y)), _ld(Y), _stream()), "scatter_add_rows")
     _count()
+
+
+def scatter_add_rows_ordered(G, idx, Y, scratch=None):
+    """Y[idx[b]] += G[b] one fp32 add at a time in ascending b (idx[b] < 0 skipped): the bit-reproducible form of scatter_add_rows.
+    scratch: int32 CUDA buffer of 2 * len(idx) entries; pass a persistent one under CUDA-graph capture, and one per concurrent call."""
+    n = int(idx.numel())
+    need = int(N.lib().llmrec_scatter_add_rows_ordered_scratch(n))
+    if scratch is None:
+        scratch = torch.empty(max(need, 1), dtype=torch.int32, device=idx.device)
+    N.check(N.lib().llmrec_scatter_add_rows_ordered_f32(_p(_mat(G)), _ld(G), _p(_i32(idx)), n, G.shape[1], _p(_mat(Y)), _ld(Y),
+                                                         _p(_i32(scratch, "scratch")), scratch.numel(), _stream()), "scatter_add_rows_ordered")
+    _count(2)
 
 
 def _scale_col(t):

@@ -85,6 +85,9 @@ _EXTRA = [
                                                                       "int8 quantizes each row once to int8 values and a power-of-two scale "
                                                                       "(every stored value an exact bf16), a quarter of the fp32 bytes; "
                                                                       "the projections are then exact on the rounded tables. Not with the mask branch")),
+    ("deterministic", dict(type=int, default=0, help="1: bit-reproducible training steps -- the loss heads accumulate their row gradients in a fixed "
+                                                     "order (heads, then batch positions, pos before neg) instead of with float atomics, so one "
+                                                     "--seed gives one model. Not with --proj_mode fp32, the mask / dropout branch or the sharded engines")),
 ]
 
 DATASET_ALIASES = {"netflix": "netflix_valid_item", "movielens": "preprocessed_raw_MovieLens", "movieLens": "preprocessed_raw_MovieLens"}
