@@ -612,19 +612,31 @@ class HotPath:
         gi[3, :2].copy_(self._meta_table[B], non_blocking=True)
         return self.replay_staged()
 
-    def _snapshot_state(self):
+    def state_tensors(self):
+        """name -> live tensor, everything one training step hands to the next: "model/<name>", "m/<name>", "v/<name>" per optimized
+        parameter (the reference's parameter names) and "state", AdamW's device-side fp64 step block.  The graph warm-up's undo and
+        the checkpoints (checkpoint.py) both go through this one list."""
         o = self.opt
-        return ([p.clone() for p in o.params], [m.clone() for m in o.m], [v.clone() for v in o.v], o.state.clone())
+        out = {}
+        for sec, tensors in (("model", o.params), ("m", o.m), ("v", o.v)):
+            out.update({sec + "/" + k: t for k, t in zip(self._opt_names, tensors)})
+        out["state"] = o.state
+        return out
 
-    def _restore_state(self, snap):
-        o = self.opt
-        for dst, src in zip(o.params, snap[0]):
-            dst.copy_(src)
-        for dst, src in zip(o.m, snap[1]):
-            dst.copy_(src)
-        for dst, src in zip(o.v, snap[2]):
-            dst.copy_(src)
-        o.state.copy_(snap[3])
+    def load_state(self, src):
+        """Copy `src` (name -> tensor, the keys of `state_tensors`) INTO the live tensors.  In place on purpose: a captured graph, the
+        optimizer's pointer tables and the compact live-item tables hold these addresses, so rebinding a tensor would fork the state.
+        Nothing derived from the parameters outlives a step, so nothing else needs a refresh: the W hi/lo split scratch (keyed by W's
+        address, ops.proj_fwd_group) is rewritten by every projection launch; the hoisted engine's TU / TI / Gram tables and the
+        compact live-item tables are functions of the constant feature tables alone; MM_Model.hot_path keys its engine by the
+        embedding table's address, which a copy keeps; U / I and every activation are recomputed by the next forward."""
+        for k, dst in self.state_tensors().items():
+            dst.copy_(src[k])
+
+    def _snapshot_state(self):
+        return {k: t.clone() for k, t in self.state_tensors().items()}
+
+    _restore_state = load_state
 
     def set_optimizer(self, lr, betas=(0.9, 0.999), eps=1e-8, weight_decay=0.01):
         names = [k for k in PARAM_ORDER if k in self.p and (self.has_feats or k.endswith("embedding.weight"))]

@@ -12,6 +12,8 @@ Changed on purpose (same results, fewer host round trips):
   * the derived `*_final` / `augmented_total_embed_dict` files are NOT written back into the data
     directory (main.py:66,78 side effects);
   * clip_grad_norm_ before zero_grad (main.py:274) is a no-op upstream and is omitted.
+Added (no counterpart upstream): checkpoints -- Trainer.save_checkpoint / load_checkpoint, --save_dir / --save_every / --resume /
+--eval_only (checkpoint.py); without those flags nothing is written and train() is what it was.
 """
 from __future__ import annotations
 
@@ -27,6 +29,7 @@ import numpy as np
 import scipy.sparse as sp
 import torch
 
+from . import checkpoint
 from .Models import Decoder, MM_Model
 from .graph import BipartiteGraph
 from .runtime import get_args, set_args
@@ -75,6 +78,12 @@ class Trainer(object):
         if getattr(args, "deterministic", 0) and (args.mask or args.mask_rate > 0 or args.drop_rate > 0):
             raise ValueError("--deterministic 1 cannot be combined with --mask / --mask_rate > 0 / --drop_rate > 0: that branch accumulates with "
                              "torch's index_add_ and runs the Decoder backward, whose summation orders are not fixed")
+        if getattr(args, "eval_only", 0) and not getattr(args, "resume", None):
+            raise ValueError("--eval_only 1 evaluates a saved model: give it one with --resume PATH")
+        if (getattr(args, "resume", None) or getattr(args, "save_dir", None)) and (args.mask or args.mask_rate > 0 or args.drop_rate > 0):
+            raise ValueError("--save_dir / --resume cannot be combined with --mask / --mask_rate > 0 / --drop_rate > 0: that branch overwrites rows "
+                             "of the feature tables for good (Trainer._mask_features), so the tables are run state there and a checkpoint "
+                             "does not hold them")
         self.device = torch.device(device)
         self.task_name = "%s_%s_%s" % (datetime.now().strftime("%Y-%m-%d %H:%M:%S"), args.dataset, args.cf_model)
         self.logger = Logger(filename=self.task_name, is_debug=args.debug)
@@ -155,6 +164,13 @@ class Trainer(object):
             gi = self.hot.index_buffer(self.hot.batch_capacity())
             self.hot.pre_step = lambda: self.device_sampler.fill(self.hot._gidx, self.hot._meta_table)
             self.hot.pre_step_undo = lambda: self.device_sampler.state[1:2].sub_(1)
+        self.n_interactions = 0
+        self._loop = self._new_loop()                 # where train() stands (what a checkpoint's `loop` section holds)
+        self._resume_loop = None                      # set by load_checkpoint: the next train() continues from it
+        # --resume: after set_seed and after the model and the Decoder were built, so their draws from the CPU generator happen as in
+        # every run and the load then overwrites all RNG streams with the saved ones
+        if getattr(args, "resume", None):
+            self.load_checkpoint(args.resume)
 
     # ---- reference helper API (same names / returns) ----------------------------------------------
     def csr_norm(self, csr_mat, mean_flag=False):
@@ -380,20 +396,90 @@ class Trainer(object):
         u, p, n = self.stage_batch()
         return self._step(u, p, n), int(u.numel())
 
+    # ---- checkpoints (checkpoint.py: format, durable write, validated read) -------------------------------
+    @staticmethod
+    def _new_loop():
+        return dict(epoch=0, batch=0, best_recall=0, stopping_step=0, test_ret=None)
+
+    def _fingerprint(self):
+        """must: what a checkpoint has to agree with to be loadable at all; recorded: the flags an exact resume needs equal."""
+        args = self.args
+        live = checkpoint.engine_tensors(self.hot)
+        must = dict(n_users=int(self.n_users), n_items=int(self.n_items), train_nnz=int(self.ui_graph_raw.nnz), embed_size=int(self.emb_dim),
+                    weight_size=tuple(int(w) for w in self.weight_size),
+                    feat_widths=tuple(int(t.shape[1]) for t in (self.image_feats, self.text_feats, self.user_init_embedding,
+                                                                 *self.item_attribute_embedding.values())),
+                    params={k[len("model/"):]: tuple(t.shape) for k, t in live.items() if k.startswith("model/")})
+        flags = ("seed", "batch_size", "lr", "regs", "model_cat_rate", "user_cat_rate", "item_cat_rate", "aug_mf_rate", "mm_mf_rate",
+                 "prune_loss_drop_rate", "feat_reg_decay", "aug_sample_rate", "proj_mode", "feat_dtype", "hoist_side", "device_sampler",
+                 "host_sampler", "deterministic", "cuda_graph")
+        return dict(must=must, recorded={k: getattr(args, k) for k in flags})
+
+    def save_checkpoint(self, path):
+        """Write the whole run state to `path`, at a step boundary: parameters, AdamW moments and step block, the RNG streams the samplers
+        advance, and where the training loop stands.  Synchronises once, for the device-to-host copies; a training step never does."""
+        live = dict(checkpoint.engine_tensors(self.hot), epoch_stats=self._epoch_stats)
+        if self.device_sampler is not None:
+            live["device_sampler"] = self.device_sampler.state
+        host = checkpoint.to_host(live)
+        model, optim = checkpoint.engine_sections(host, self.hot.opt)
+        lp = self._loop
+        ret = lp["test_ret"]
+        loop = dict(epoch=int(lp["epoch"]), batch=int(lp["batch"]), epoch_stats=host["epoch_stats"], best_recall=float(lp["best_recall"]),
+                    stopping_step=int(lp["stopping_step"]), n_interactions=int(self.n_interactions),
+                    test_ret=None if ret is None else {k: float(v) if np.ndim(v) == 0 else torch.as_tensor(np.asarray(v, dtype=np.float64))
+                                                       for k, v in ret.items()})
+        checkpoint.write(path, model, optim, checkpoint.rng_state(self.device, host.get("device_sampler")), loop, self._fingerprint())
+
+    def load_checkpoint(self, path):
+        """Put the state of `save_checkpoint` back, IN PLACE (HotPath.load_state): before the first step or after a CUDA graph has been
+        captured and replayed.  The file is validated as a whole first; a load that raises leaves this Trainer as it was.  The next
+        train() continues from the saved epoch and batch.  A recorded flag that differs from this run's is logged; the continuation is
+        exact only when none does."""
+        ck, saved, diffs = checkpoint.read(path, self._fingerprint(), checkpoint.engine_tensors(self.hot))
+        if diffs:
+            self.logger.logging("checkpoint %s was written with other flags (saved -> this run): %s" % (path, ", ".join(diffs)))
+        self.hot.load_state(saved)
+        checkpoint.set_rng_state(ck["rng"], self.device, self.device_sampler)
+        lp = ck["loop"]
+        self._epoch_stats.copy_(lp["epoch_stats"])
+        self.n_interactions = lp["n_interactions"]
+        ret = lp["test_ret"]
+        self._loop = self._resume_loop = dict(
+            epoch=lp["epoch"], batch=lp["batch"], best_recall=lp["best_recall"], stopping_step=lp["stopping_step"],
+            test_ret=None if ret is None else {k: v.numpy() if isinstance(v, torch.Tensor) else v for k, v in ret.items()})
+
+    def evaluate(self):
+        """--eval_only 1: no training step; the metrics of the loaded model on the test users, logged like an epoch's."""
+        ret = self.test(list(self.data_generator.test_set.keys()), is_val=False)
+        r, p, h, n = ret["recall"], ret["precision"], ret["hit_ratio"], ret["ndcg"]
+        self.logger.logging("recall=[%.5f, %.5f, %.5f, %.5f], precision=[%.5f, %.5f, %.5f, %.5f], hit=[%.5f, %.5f, %.5f, %.5f], "
+                            "ndcg=[%.5f, %.5f, %.5f, %.5f]" % (r[0], r[1], r[2], r[-1], p[0], p[1], p[2], p[-1], h[0], h[1], h[2], h[-1],
+                                                               n[0], n[1], n[2], n[-1]))
+        return ret
+
     # ---- training loop (main.py:189-326) -----------------------------------------------------------------
     def train(self):
+        """Starts at epoch 0, or where the checkpoint loaded last stands: in the middle of an epoch its remaining batches run on top of
+        the saved loss accumulators, so the epoch's log line is the uninterrupted one, and early stopping keeps its counters."""
         args, dg = self.args, self.data_generator
         run_time = datetime.strftime(datetime.now(), "%Y_%m_%d__%H_%M_%S")
         training_time_list = []
-        stopping_step, best_recall, test_ret = 0, 0, None
-        for epoch in range(args.epoch):
+        lp = self._loop = self._resume_loop or self._new_loop()
+        self._resume_loop = None
+        save_dir = getattr(args, "save_dir", None)
+        save_every = max(int(getattr(args, "save_every", 1)), 1)
+        stopping_step, best_recall, test_ret = lp["stopping_step"], lp["best_recall"], lp["test_ret"]
+        for epoch in range(lp["epoch"], args.epoch):
             t1 = time()
             n_batch = dg.n_train // args.batch_size + 1
-            self._epoch_stats.zero_()
-            self.n_interactions = 0
+            if lp["batch"] == 0:
+                self._epoch_stats.zero_()
+                self.n_interactions = 0
             self.model_mm.train()
-            for _ in range(n_batch):
+            for k in range(lp["batch"], n_batch):
                 self.n_interactions += max(self.train_next_batch()[1], 0)
+                lp["batch"] = k + 1
             loss, mf_loss, emb_loss, n_dev = (float(x) for x in self._epoch_stats.tolist())      # the one sync per epoch
             self.n_interactions += int(n_dev)
             reg_loss, contrastive_loss = 0.0, 0.0
@@ -417,18 +503,25 @@ class Trainer(object):
                     "precision=[%.5f, %.5f, %.5f, %.5f], hit=[%.5f, %.5f, %.5f, %.5f], ndcg=[%.5f, %.5f, %.5f, %.5f]" % (
                         epoch, t2 - t1, t3 - t2, loss, mf_loss, emb_loss, reg_loss, r[0], r[1], r[2], r[-1], p[0], p[1], p[2], p[-1],
                         h[0], h[1], h[2], h[-1], n[0], n[1], n[2], n[-1]))
+            lp.update(epoch=epoch + 1, batch=0)                # a checkpoint written from here on continues with the next epoch
             if ret["recall"][1] > best_recall:
                 best_recall = ret["recall"][1]
                 test_ret = self.test(users_to_test, is_val=False)
                 self.logger.logging("Test_Recall@%d: %.5f,  precision=[%.5f], ndcg=[%.5f]" % (
                     eval(args.Ks)[1], test_ret["recall"][1], test_ret["precision"][1], test_ret["ndcg"][1]))
                 stopping_step = 0
+                lp.update(best_recall=best_recall, test_ret=test_ret, stopping_step=0)
+                if save_dir:
+                    self.save_checkpoint(os.path.join(save_dir, "best.pt"))      # the parameters that scored it
             elif stopping_step < args.early_stopping_patience:
                 stopping_step += 1
+                lp["stopping_step"] = stopping_step
                 self.logger.logging("#####Early stopping steps: %d #####" % stopping_step)
             else:
                 self.logger.logging("#####Early stop! #####")
                 break
+            if save_dir and (epoch + 1) % save_every == 0:
+                self.save_checkpoint(os.path.join(save_dir, "last.pt"))
         self.logger.logging(str(test_ret))
         return best_recall, run_time
 
@@ -441,7 +534,9 @@ def main(argv=None):
     gen = Data(path=ddir, batch_size=args.batch_size, sampler=args.host_sampler)
     batch_test.init(gen, args)
     config = dict(n_users=gen.n_users, n_items=gen.n_items)
-    trainer = Trainer(data_config=config, data_generator=gen)
+    trainer = Trainer(data_config=config, data_generator=gen)         # --resume loads here, after set_seed and the model's own draws
+    if args.eval_only:
+        return trainer.evaluate()
     return trainer.train()
 
 

@@ -25,8 +25,8 @@ _FLOAT = {
     "lr": (0.0001, "AdamW learning rate"),
     "de_lr": (0.0002, "learning rate of the (unused) decoder optimiser"),
     "weight_decay": (1e-4, "unused: AdamW runs with torch's default 0.01"),
-    "drop_rate": (0.0, "feature dropout (only 0 is supported here)"),
-    "mask_rate": (0.0, "share of nodes whose features are masked (mask branch, not supported here)"),
+    "drop_rate": (0.0, "dropout on the projected side features (> 0 runs the eager mask / dropout branch, Trainer._train_batch_masked)"),
+    "mask_rate": (0.0, "share of nodes whose features are overwritten with the column mean (> 0 runs the eager mask / dropout branch)"),
     "user_cat_rate": (2.8, "fusion weight of the normalised user-profile term"),
     "item_cat_rate": (0.005, "fusion weight of each normalised item-attribute term"),
     "model_cat_rate": (0.02, "fusion weight of the normalised image and text terms"),
@@ -48,7 +48,7 @@ _OPTIONAL_TEXT = {                     # nargs="?": python-literal strings are e
     "mess_dropout": ("[0.1, 0.1]", "unused by LLMRec"),
     "norm_type": ("sym", "unused by LLMRec"),
     "Ks": ("[10, 20, 50]", "cut-offs of recall / precision / hit / ndcg"),
-    "test_flag": ("part", "part = top-K metrics; full (with AUC) is not supported here"),
+    "test_flag": ("part", "part = top-K metrics; full = the same plus the per-user ROC-AUC over every candidate"),
     "cf_model": ("lightgcn", "name used in the log file name"),
 }
 _TEXT = {
@@ -88,6 +88,12 @@ _EXTRA = [
     ("deterministic", dict(type=int, default=0, help="1: bit-reproducible training steps -- the loss heads accumulate their row gradients in a fixed "
                                                      "order (heads, then batch positions, pos before neg) instead of with float atomics, so one "
                                                      "--seed gives one model. Not with --proj_mode fp32, the mask / dropout branch or the sharded engines")),
+    ("save_dir", dict(default=None, help="directory for checkpoints: last.pt after every --save_every epochs (after the evaluation), best.pt whenever "
+                                         "recall@Ks[1] improves. Nothing is written without it. Not with the mask / dropout branch")),
+    ("save_every", dict(type=int, default=1, help="epochs between two writes of last.pt (with --save_dir)")),
+    ("resume", dict(default=None, help="checkpoint to continue from: parameters, AdamW state, RNG streams and the position in the training loop are "
+                                       "put back before the first step, so training goes on as if it had never stopped")),
+    ("eval_only", dict(type=int, default=0, help="1: run no training step, evaluate the model of --resume once on the test users")),
 ]
 
 DATASET_ALIASES = {"netflix": "netflix_valid_item", "movielens": "preprocessed_raw_MovieLens", "movieLens": "preprocessed_raw_MovieLens"}
