@@ -1,0 +1,146 @@
+"""bench_recommend.py -- recommendation throughput (Trainer.recommend / recommend.top_k, --candidates_out) on one H100.
+
+    python bench_recommend.py [--reps 3] [--syn_users 131072] [--syn_histories 8192] [--syn_scale 1.0]
+
+Three legs per workload, each timed end to end on the host clock between device synchronises (median of --reps calls after one
+warm-up call) and reported in users/s:
+  known      trained users scored from U with their training items excluded (exclude="train"), K = 10
+  fold_in    held-out histories folded in (HotPath.fold_in) and scored, exclude="train", K = 10
+  candidates the --candidates_out file: every user's top-10 over the whole catalog, nothing excluded, pickled to a temporary file
+Every call includes the full eval forward a recommendation starts with.
+Workloads: the netflix shape of bench.py (Trainer with side features, held-out histories = a user's training row plus its test items),
+and the 10M x 1M x 200M synthetic of dist_bench (ID-only single-GPU engine, d = 128, L = 2; histories = a training row plus two random
+items, folded in as unknown users; the known and candidates legs score the first --syn_users users).
+One JSON line on stdout with the card's name and power limit; a summary on stderr.  Needs a CUDA device (no fallback).
+"""
+from __future__ import annotations
+
+import argparse
+import json
+import os
+import sys
+import tempfile
+import time
+import types
+
+REPO = os.path.dirname(os.path.abspath(__file__))
+if REPO not in sys.path:
+    sys.path.insert(0, REPO)
+
+import bench  # noqa: E402
+from bench_feat_dtype import card  # noqa: E402
+
+
+def _timed(fn, reps):
+    import torch
+    fn()
+    torch.cuda.synchronize()
+    ts = []
+    for _ in range(reps):
+        t0 = time.perf_counter()
+        fn()
+        torch.cuda.synchronize()
+        ts.append(time.perf_counter() - t0)
+    return sorted(ts)[len(ts) // 2], min(ts), max(ts)
+
+
+def _leg(name, n_users, fn, reps):
+    med, lo, hi = _timed(fn, reps)
+    out = {"users": n_users, "s_per_call": round(med, 5), "s_min": round(lo, 5), "s_max": round(hi, 5), "users_per_s": round(n_users / med, 1)}
+    sys.stderr.write(f"  {name:10s} {n_users:9d} users  {med * 1e3:9.2f} ms/call  {n_users / med:12.0f} users/s\n")
+    return out
+
+
+def netflix(a, tmp):
+    import numpy as np
+    tr, gen, args = bench.make_trainer("netflix", types.SimpleNamespace(proj_mode=a.proj_mode, host_sampler="native", graph=1))
+    for _ in range(5):
+        tr.train_next_batch()                                     # a model some steps in: U / I stale on all but the last batch's rows
+    nu = tr.n_users
+    rp, col = tr.graph.rowptr_u.cpu().numpy(), tr.graph.col_u.cpu().numpy()
+    users = np.array(sorted(int(u) for u in gen.test_set.keys()))
+    hist = [col[rp[u]:rp[u + 1]].tolist() + list(gen.test_set[int(u)]) for u in users]
+    path = os.path.join(tmp, "candidate_indices")
+    res = {"workload": bench.workload_string("netflix"),
+           "known": _leg("known", nu, lambda: tr.recommend(K=10, exclude="train"), a.reps),
+           "fold_in": _leg("fold_in", len(hist), lambda: tr.recommend(users=users, K=10, exclude="train", histories=hist), a.reps),
+           "candidates": _leg("candidates", nu, lambda: tr.write_candidates(path, 10), a.reps)}
+    del tr, gen
+    return res
+
+
+def synthetic(a, tmp):
+    import numpy as np
+    import torch
+    from llmrec_b200 import dist_bench, recommend
+    from llmrec_b200.dist import ShardedGraph, synthetic_shard
+    from llmrec_b200.engine import HotPath, HotPathConfig
+    from llmrec_b200.ops import CsrOperator
+    dev = torch.device("cuda", 0)
+    nu, ni, ne, d, L = dist_bench.syn_sizes(a.syn_scale)
+    ul, it, _, _ = synthetic_shard(nu, ni, ne, 0, 1, dev, seed=0)
+    g = ShardedGraph(ul, it, nu, ni, solo=True)
+    del ul, it
+    iu = CsrOperator(g.rowptr_i, g.col_i, ni, nu, rs=g.si, plan=g.iu_raw.plan)                # iu = diag(si) R^T (one rank: no all-reduce)
+    gen = torch.Generator(device=dev).manual_seed(0)
+    params = {"user_id_embedding.weight": torch.randn(nu, d, device=dev, generator=gen) * 0.1,
+              "item_id_embedding.weight": torch.randn(ni, d, device=dev, generator=gen) * 0.1}
+    hp = HotPath((g.ui, iu, g.uiT_raw, g.iuT), params, None, HotPathConfig(embed_size=d, n_layers=L))
+    rng = np.random.default_rng(0)
+    hu = rng.choice(nu, a.syn_histories, replace=False)
+    rp = g.rowptr_u.cpu().numpy()
+    col = g.col_u.cpu().numpy()
+    hist = [col[rp[u]:rp[u + 1]].tolist() + rng.integers(0, ni, 2).tolist() for u in hu]
+    n = min(a.syn_users, nu)
+    users = np.arange(n)
+    path = os.path.join(tmp, "candidate_indices_synthetic")
+
+    def known():
+        hp.forward()
+        recommend.top_k(hp, g.rowptr_u, g.col_u, users=users, K=10, exclude="train", mode=a.score_mode)
+
+    def fold():
+        hp.forward()
+        recommend.top_k(hp, g.rowptr_u, g.col_u, K=10, exclude="train", histories=hist, mode=a.score_mode)
+
+    def cand():
+        hp.forward()
+        ids, _ = recommend.top_k(hp, g.rowptr_u, g.col_u, users=users, K=10, exclude="none", mode=a.score_mode)
+        recommend.write_candidates(path, ids)
+
+    res = {"workload": f"synthetic {nu}x{ni}, {g.nnz} training edges, d={d}, L={L}, ID-only engine",
+           "known": _leg("known", n, known, a.reps), "fold_in": _leg("fold_in", len(hist), fold, a.reps),
+           "candidates": _leg("candidates", n, cand, a.reps)}
+    del hp, g, params
+    torch.cuda.empty_cache()
+    return res
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--reps", type=int, default=3, help="timed calls per leg (the median is reported), after one warm-up call")
+    ap.add_argument("--proj_mode", default="3xtf32", choices=["3xtf32", "tf32", "fp32"])
+    ap.add_argument("--syn_users", type=int, default=131072, help="synthetic workload: users of the known and candidates legs")
+    ap.add_argument("--syn_histories", type=int, default=8192, help="synthetic workload: histories of the fold-in leg")
+    ap.add_argument("--syn_scale", type=float, default=1.0, help="size factor of the 10M x 1M x 200M synthetic graph")
+    ap.add_argument("--workloads", default="netflix,synthetic")
+    a = ap.parse_args()
+    import torch
+    from llmrec_b200 import ops
+    if not torch.cuda.is_available():
+        raise SystemExit("bench_recommend.py needs a CUDA (H100) device")
+    a.score_mode = ops.SCORE_MODE.get(a.proj_mode, 0)
+    name, limit = card()
+    result = {"metric": "recommend_users_per_sec", "gpu": name, "power_limit": limit, "proj_mode": a.proj_mode, "K": 10,
+              "timing": f"host clock between device synchronises, median of {a.reps} calls after one warm-up; each call runs the full eval forward",
+              "workloads": {}}
+    with tempfile.TemporaryDirectory(prefix="llmrec_recommend_") as tmp:
+        for wl in a.workloads.split(","):
+            sys.stderr.write(f"{wl}:\n")
+            result["workloads"][wl] = netflix(a, tmp) if wl == "netflix" else synthetic(a, tmp)
+            torch.cuda.empty_cache()
+    print(json.dumps(result), flush=True)
+
+
+if __name__ == "__main__":
+    main()

@@ -49,6 +49,7 @@ import contextlib
 import os
 from dataclasses import dataclass
 
+import numpy as np
 import torch
 
 from . import ops
@@ -326,11 +327,15 @@ class HotPath:
         return (dict(rows=self.batch_u.list, count=self.batch_u.count, max_rows=mu),
                 dict(rows=self.batch_i.list, count=self.batch_i.count, max_rows=mi))
 
+    def _side_coefs(self):
+        """fusion weights of the side terms, in the order of the side lists (img, txt, profile, attributes; Models.py:185-197)"""
+        c = self.cfg
+        return [c.model_cat_rate, c.model_cat_rate, c.user_cat_rate] + [c.item_cat_rate] * len(self.keys) if self.has_feats else []
+
     def _fuse_fwd(self, batch_rows=False):
         """batch_rows: U / I on the batch's rows only (train_step); the other rows keep whatever they held."""
-        c = self.cfg
         if self.has_feats:
-            coefs = [c.model_cat_rate, c.model_cat_rate, c.user_cat_rate] + [c.item_cat_rate] * len(self.keys)
+            coefs = self._side_coefs()
             su = [self.blk(self.Fu, 0), self.blk(self.Fu, 1), self.prof_u] + [self.blk(self.Fu, 2 + j) for j in range(len(self.keys))]
             si = [self.blk(self.Fi, 0), self.blk(self.Fi, 1), self.prof_i] + [self.blk(self.Fi, 2 + j) for j in range(len(self.keys))]
         else:
@@ -341,6 +346,73 @@ class HotPath:
             ops.fuse_fwd(self.Il, si, coefs, self.I, **ki)
             self._join()
         self._fuse_args = (coefs, su, si)
+
+    # ---- fold-in: the user side of the forward for interaction histories given at call time -----------------------------------
+    def fold_in(self, rowptr, col, known=None):
+        """-> U_new [m x d]: the fused representation of m users whose histories are the rows of an int CSR over item ids (rowptr[m+1],
+        col; `graph.history_matrix` rejects ids outside [0, n_items) and collapses repeats).  known: optional int[m], the trained user id
+        of each row or -1.  Reads the item side of the last full `forward()` (Pi, prof_i, Il) and the parameters; writes no buffer a
+        training step reads.
+
+        Every user-side quantity of the forward is the user's row of ui = diag(su) R times an item-side tensor (Fu = ui.Pi,
+        prof_u = ui.prof_i, Ul[l] = [softmax] ui.Il[l-1]), so with R the new rows and su their (deg + 1e-8)^-1/2 these are ONE SpMM
+        launch with S + 1 + L segments, followed by the fusion of the m rows.  Layer 0 is E_u[known] for a trained user; an unknown user
+        has no ID embedding, and its layer 0 is a zero row (it enters the mean of the L + 1 layers as 0)."""
+        from .graph import history_matrix, inv_sqrt_degree
+        R = history_matrix(rowptr, col, self.ni)
+        m, d, L, dev = R.shape[0], self.d, self.L, self.E_u.device
+        kn = np.full(m, -1, dtype=np.int32) if known is None else \
+            (known.detach().cpu().numpy() if hasattr(known, "detach") else np.asarray(known)).astype(np.int64).reshape(-1)
+        if kn.size != m or (m and (kn.min() < -1 or kn.max() >= self.nu)):
+            raise ValueError(f"fold_in: known must hold one trained user id in [0, {self.nu}) or -1 per history ({m})")
+        if m == 0:
+            return torch.empty(0, d, dtype=torch.float32, device=dev)
+        t = lambda a, dt: torch.from_numpy(np.ascontiguousarray(a.astype(dt))).to(dev)
+        op = ops.CsrOperator(t(R.indptr, np.int32), t(R.indices, np.int32), m, self.ni, rs=t(inv_sqrt_degree(R), np.float32),
+                             tile_nnz=getattr(self.ui.plan, "tile_nnz", 0))       # pieces cut as the training operator cuts them
+        new = lambda *s: torch.empty(*s, dtype=torch.float32, device=dev)
+        Ul = [new(m, d) for _ in range(L + 1)]
+        Fu, prof_u = (new(m, self.S * d), new(m, d)) if self.has_feats else (None, None)
+        if self.has_feats:
+            self._fold_in_items(np.unique(R.indices))
+        op.apply(self._fold_in_segs(Fu, prof_u, Ul))
+        ops.gather_rows(self.E_u, t(kn, np.int32), Ul[0])                      # known -> E_u row, -1 -> zeros
+        su = [self.blk(Fu, 0), self.blk(Fu, 1), prof_u] + [self.blk(Fu, 2 + j) for j in range(len(self.keys))] if self.has_feats else []
+        U = new(m, d)
+        ops.fuse_fwd(Ul, su, self._side_coefs(), U)                                                            # :185-197
+        return U
+
+    def _fold_in_segs(self, Fu, prof_u, Ul):
+        """The segments of the one fold-in launch: Pi's S blocks -> Fu, prof_i -> prof_u, Il[l-1] -> Ul[l] (softmax on l = L)."""
+        segs = []
+        if self.has_feats:
+            segs += [(self.blk(self.Pi, s), self.blk(Fu, s), None, False) for s in range(self.S)]              # :153,156,162
+            segs.append((self.prof_i, prof_u, None, False))                                                     # :167
+        segs += [(self.Il[l - 1], Ul[l], None, l == self.L) for l in range(1, self.L + 1)]                    # :174,178
+        return segs
+
+    def _fold_in_items(self, items):
+        """Make Pi hold X.W^T + b on every item of `items` (sorted ids) before a fold-in.  The forward projects the live items only, and
+        Pi's edgeless rows are zero; a history given at call time may hold such an item.  Those rows are projected here with the
+        grouped kernels and a row map into Pi's edgeless rows, which no training launch reads (no ui column points there)."""
+        if self.live_i is None:
+            return
+        if getattr(self, "_edgeless", None) is None:
+            # once: the edgeless item ids and their rows of the item-side tables (the tables' own dtype), as _build_live_items does
+            dead = torch.nonzero(self._live_pos < 0).flatten()
+            f = self.feats
+            self._edgeless = (dead.cpu().numpy(), dead.to(torch.int32).contiguous(),
+                              dict(image=f["image"][dead].contiguous(), text=f["text"][dead].contiguous(),
+                                   item={k: v[dead].contiguous() for k, v in f["item"].items()}))
+        dead_np, dead, x = self._edgeless
+        if dead_np.size == 0 or not np.isin(items, dead_np, assume_unique=True).any():
+            return
+        p = self.p
+        probs = [(x["image"], p["image_trans.weight"], p["image_trans.bias"], self.blk(self.Pi, 0), dead),
+                 (x["text"], p["text_trans.weight"], p["text_trans.bias"], self.blk(self.Pi, 1), dead)]
+        probs += [(x["item"][k], p["item_trans.weight"], p["item_trans.bias"], self.blk(self.Pi, 2 + j), dead) for j, k in enumerate(self.keys)]
+        probs.sort(key=lambda t: -t[0].shape[1])
+        ops.proj_fwd_group(probs, self.d, self.cfg.proj_mode)
 
     # ---- backward: expects gU, gI and (GFu, GFi, Gprof_u, Gprof_i, GP_usr_direct) filled ---------------
     def backward(self, gp_usr_direct=None, batch_rows=False):

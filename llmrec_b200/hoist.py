@@ -107,6 +107,16 @@ class HoistedHotPath(HotPath):
         self._fuse_fwd()
         return self.U, self.I
 
+    def _fold_in_items(self, items):
+        """fold_in reads Pi = X.W^T + b, which this engine never materialises (its forward projects the propagated tables): one grouped
+        projection of the full item-side tables per call, into the engine's Pi, which no hoisted step reads."""
+        p, f = self.p, self.feats
+        probs = [(f["image"], p["image_trans.weight"], p["image_trans.bias"], self.blk(self.Pi, 0)),
+                 (f["text"], p["text_trans.weight"], p["text_trans.bias"], self.blk(self.Pi, 1))]
+        probs += [(f["item"][k], p["item_trans.weight"], p["item_trans.bias"], self.blk(self.Pi, 2 + j)) for j, k in enumerate(self.keys)]
+        probs.sort(key=lambda t: -t[0].shape[1])
+        ops.proj_fwd_group(probs, self.d, self.cfg.proj_mode)
+
     # ---- compact buffers of a training step ---------------------------------------------------------------------------
     def _ensure_compact(self, cap):
         c = self._compact

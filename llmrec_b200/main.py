@@ -29,9 +29,9 @@ import numpy as np
 import scipy.sparse as sp
 import torch
 
-from . import checkpoint
+from . import checkpoint, ops, recommend
 from .Models import Decoder, MM_Model
-from .graph import BipartiteGraph
+from .graph import BipartiteGraph, histories_csr
 from .runtime import get_args, set_args
 from .utility import batch_test
 from .utility.load_data import Data
@@ -458,6 +458,42 @@ class Trainer(object):
                                                                n[0], n[1], n[2], n[-1]))
         return ret
 
+    # ---- recommendations (recommend.py) ---------------------------------------------------------------------------------
+    def _current_model(self):
+        """The engine after a full eval forward: a training step leaves U / I current on its batch's rows only, and every item-side
+        tensor one parameter update behind.  Launches nothing else and changes no run state."""
+        if self.masked_mode:
+            raise ValueError("recommendations need a fixed model: with --mask / --mask_rate > 0 / --drop_rate > 0 every forward rewrites rows of "
+                             "the feature tables (Trainer._mask_features)")
+        recommend.check_engine(self.hot)
+        with torch.no_grad():
+            self.hot.forward()
+        return self.hot
+
+    def recommend(self, users=None, K=10, exclude="train", histories=None):
+        """-> (ids int64 [m x K], scores fp32 [m x K]) on the device: each row's K best items, ties to the lowest item id, padded with
+        -1 / -inf when fewer than K items are left.
+        users: trained user ids (default every user).  histories: item-id lists or a (rowptr, col) pair, folded in with the trained item
+        side (HotPath.fold_in); `users` then names each history's trained id (or -1) and may be omitted.  exclude: "train" masks a
+        trained user's training items and a history's own items; "none" masks nothing (the reference's candidate lists).  K: 1..64 and
+        at most n_items.  --proj_mode picks the scoring mode."""
+        recommend.check_k(K, self.n_items)
+        hot = self._current_model()
+        mode = ops.SCORE_MODE.get(getattr(self.args, "proj_mode", "3xtf32"), 0)
+        return recommend.top_k(hot, self.graph.rowptr_u, self.graph.col_u, users=users, K=K, exclude=exclude, histories=histories, mode=mode)
+
+    def fold_in(self, histories, known=None):
+        """-> U_new [m x d]: the fused user representations of item-id histories (lists or a (rowptr, col) pair) under the current
+        parameters; known: each history's trained user id or -1 (layer 0 = that user's ID embedding, or zero)."""
+        R = histories_csr(histories, self.n_items)
+        return self._current_model().fold_in(R.indptr, R.indices, known=known)
+
+    def write_candidates(self, path, K=10):
+        """--candidates_out: the top-K of every user over the whole catalog, nothing excluded (torch.topk(U . I^T, k=K) of the reference's
+        stage 1), pickled as a CPU int64 tensor [n_users x K] to `path` (atomically)."""
+        ids, _ = self.recommend(K=K, exclude="none")
+        return recommend.write_candidates(path, ids)
+
     # ---- training loop (main.py:189-326) -----------------------------------------------------------------
     def train(self):
         """Starts at epoch 0, or where the checkpoint loaded last stands: in the middle of an epoch its remaining batches run on top of
@@ -534,10 +570,16 @@ def main(argv=None):
     gen = Data(path=ddir, batch_size=args.batch_size, sampler=args.host_sampler)
     batch_test.init(gen, args)
     config = dict(n_users=gen.n_users, n_items=gen.n_items)
+    if args.candidates_out:                                           # before any training: a bad K or flag mix fails at once
+        recommend.check_k(args.candidates_k, gen.n_items)
     trainer = Trainer(data_config=config, data_generator=gen)         # --resume loads here, after set_seed and the model's own draws
-    if args.eval_only:
-        return trainer.evaluate()
-    return trainer.train()
+    if args.candidates_out and trainer.masked_mode:
+        raise ValueError("--candidates_out needs a fixed model: not with --mask / --mask_rate > 0 / --drop_rate > 0")
+    ret = trainer.evaluate() if args.eval_only else trainer.train()
+    if args.candidates_out:                                           # from the model in memory when the run ends
+        trainer.write_candidates(args.candidates_out, args.candidates_k)
+        trainer.logger.logging("candidates: top-%d of %d users written to %s" % (args.candidates_k, trainer.n_users, args.candidates_out))
+    return ret
 
 
 if __name__ == "__main__":

@@ -94,6 +94,10 @@ _EXTRA = [
     ("resume", dict(default=None, help="checkpoint to continue from: parameters, AdamW state, RNG streams and the position in the training loop are "
                                        "put back before the first step, so training goes on as if it had never stopped")),
     ("eval_only", dict(type=int, default=0, help="1: run no training step, evaluate the model of --resume once on the test users")),
+    ("candidates_out", dict(default=None, help="when the run ends (after training, or after --eval_only 1), write every user's top --candidates_k "
+                                               "items over the whole catalog, nothing excluded, as the pickled CPU int64 tensor [n_users x K] "
+                                               "the augmentation stage reads (data/<dataset>/candidate_indices). Not with the mask / dropout branch")),
+    ("candidates_k", dict(type=int, default=10, help="list length of --candidates_out (1..64, at most n_items)")),
 ]
 
 DATASET_ALIASES = {"netflix": "netflix_valid_item", "movielens": "preprocessed_raw_MovieLens", "movieLens": "preprocessed_raw_MovieLens"}
