@@ -417,6 +417,23 @@ int llmrec_device_sample_batch(const int32_t* exist_users, int32_t n_exist, int3
                                const int32_t* meta_table, int32_t cap, uint64_t* state, int32_t* out, uint32_t* key_scratch,
                                llmrec_stream_t stream);
 
+/* Device-side batch sampler ON the reference's streams (`--device_sampler 2`): one launch draws exactly the batch of
+ * llmrec_host_sample_batch (same arguments, same users / pos / neg / augmented triplets / B', both streams left in the same state) into the
+ * [4 x cap] index buffer of llmrec_device_sample_batch.  train_col: the rows in the host sampler's order (the positive indexes them);
+ * train_col_sorted: the same rows sorted ascending (negative rejection).  All pointers DEVICE.
+ * state: int32[LLMREC_REF_SAMPLER_STATE_ELEMS] = { CPython `random` key[624], pos, numpy global MT19937 key[624], pos, error, pad }.
+ * error != 0 (set by a call, or found on entry): the host sampler's return code (2 no train item, 3 no possible negative, 4 uid missing
+ * from the augmentation tables; 5 a rejection loop passed 2^24 draws); both streams keep their state before the failing call, and every
+ * call writes a batch of user 0 / item 0 with B' = batch until the host clears the word.
+ * work: int32[llmrec_device_sample_batch_ref_work(...)] scratch (unused when it fits in shared memory). */
+#define LLMREC_REF_SAMPLER_STATE_ELEMS 1252
+int64_t llmrec_device_sample_batch_ref_work(int32_t n_exist, int32_t batch, int32_t users_pool_branch, int32_t aug_pool_branch);
+int llmrec_device_sample_batch_ref(const int32_t* exist_users, int32_t n_exist, int32_t batch, int32_t users_pool_branch,
+                                   const int32_t* train_rowptr, const int32_t* train_col, const int32_t* train_col_sorted,
+                                   int32_t n_items, int32_t n_aug, int32_t aug_pool_branch, const int32_t* aug_pos, const int32_t* aug_neg,
+                                   int32_t n_aug_table, int32_t aug_limit, const int32_t* meta_table, int32_t cap,
+                                   int32_t* state, int32_t* out, int32_t* work, int64_t work_elems, llmrec_stream_t stream);
+
 /* Row helpers of the sharded (multi-GPU) path: epilogue of an item-side propagation applied AFTER the cross-rank
  * sum of per-rank partials, and gather / scatter-add of batch rows by index (idx < 0 = row not owned: zeros / skipped). */
 int llmrec_row_scale_softmax_f32(const float* X, int64_t ldx, const float* scale, float* Y, int64_t ldy, int64_t n, int32_t d,

@@ -151,6 +151,10 @@ SIGNATURES = {
                                            C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]),
     "llmrec_device_sample_batch": (C.c_int, [c_i32p, C.c_int32, C.c_int32, c_i32p, c_i32p, C.c_int32, C.c_int32, c_i32p, c_i32p, C.c_int32, C.c_int32,
                                              c_i32p, C.c_int32, C.c_void_p, c_i32p, C.c_void_p, c_stream]),
+    "llmrec_device_sample_batch_ref_work": (C.c_int64, [C.c_int32, C.c_int32, C.c_int32, C.c_int32]),
+    "llmrec_device_sample_batch_ref": (C.c_int, [c_i32p, C.c_int32, C.c_int32, C.c_int32, c_i32p, c_i32p, c_i32p, C.c_int32, C.c_int32, C.c_int32,
+                                                 c_i32p, c_i32p, C.c_int32, C.c_int32, c_i32p, C.c_int32, c_i32p, c_i32p, c_i32p, C.c_int64,
+                                                 c_stream]),
     "llmrec_row_scale_softmax_f32": (C.c_int, [c_f32p, C.c_int64, c_f32p, c_f32p, C.c_int64, C.c_int64, C.c_int32, C.c_int32, c_stream]),
     "llmrec_gather_rows_f32": (C.c_int, [c_f32p, C.c_int64, c_i32p, C.c_int32, C.c_int32, c_f32p, C.c_int64, c_stream]),
     "llmrec_scatter_add_rows_f32": (C.c_int, [c_f32p, C.c_int64, c_i32p, C.c_int32, C.c_int32, c_f32p, C.c_int64, c_stream]),

@@ -148,6 +148,8 @@ class HotPath:
         self._slot_plan = None            # cfg.deterministic: the step's slot plan (ops.bpr_slot_plan), sized with _bpr_work
         self.pre_step = None              # optional launches replayed in front of every staged step (device-side batch sampler)
         self.pre_step_undo = None         # undoes the side effect of ONE pre_step (the warm-up step before a capture must not consume a batch)
+        self.pre_step_save = None         # called before the warm-up's pre_step: keeps what pre_step_undo puts back
+        self.post_step = None             # optional launches after every staged step (joins what pre_step forked)
         self.opt = None
         self.timer = None
         # independent launches of a step run as BRANCHES: a side stream forked from / joined into the current one with events, so the
@@ -655,9 +657,13 @@ class HotPath:
                 # one eager step at full capacity sizes every lazily allocated scratch buffer; its parameter update is undone
                 snap = self._snapshot_state()
                 self._gidx[3, :2].copy_(self._meta_table[cap])
+                if self.pre_step_save is not None:
+                    self.pre_step_save()
                 if self.pre_step is not None:
                     self.pre_step()
                 self.train_step(u, p, n, meta)
+                if self.post_step is not None:
+                    self.post_step()
                 self._restore_state(snap)
                 if self.pre_step is not None and self.pre_step_undo is not None:
                     self.pre_step_undo()
@@ -669,6 +675,8 @@ class HotPath:
                 if self.pre_step is not None:
                     self.pre_step()
                 self.train_step(u, p, n, meta)
+                if self.post_step is not None:
+                    self.post_step()
             self._graph = g
         self._graph.replay()
         return self.loss

@@ -153,8 +153,23 @@ class Trainer(object):
         self.use_graph = bool(getattr(args, "cuda_graph", 1))
         self._epoch_stats = torch.zeros(4, dtype=torch.float32, device=self.device)          # total, mf, emb, interactions (device-side sampler)
         # --device_sampler 1 (SURVEY.md 8f-1): batches are drawn ON the GPU into the engine's index buffer, in front of every step
+        # --device_sampler 2: the same place, drawing the host sampler's exact batches from device copies of `random` / `np.random`
         self.device_sampler = None
-        if getattr(args, "device_sampler", 0) and not self.masked_mode:
+        self.ref_sampler = getattr(args, "device_sampler", 0) == 2 and not self.masked_mode
+        if self.ref_sampler:
+            from .device_sampler import ReferenceDeviceSampler
+            from .host_native import BatchSampler
+            rowptr, col = data_generator.csr("train")
+            col_sorted = data_generator.csr("train", sorted_rows=True)[1]
+            aug_pos, aug_neg = BatchSampler.aug_tables(self.augmented_sample_dict, data_generator.n_users, self.n_items)
+            ds = self.device_sampler = ReferenceDeviceSampler(data_generator.exist_users, rowptr, col, col_sorted, data_generator.n_items,
+                                                              data_generator.batch_size, aug_pos, aug_neg, self.n_items, args.aug_sample_rate,
+                                                              self.device)
+            # batch t + 1 is drawn beside step t (on the step's own stream with LLMREC_BRANCHES=0); the graph warm-up hands its batch back
+            ds.attach(self.hot.index_buffer(self.hot.batch_capacity()), self.hot._meta_table, side_stream=self.hot.branches)
+            self.hot.pre_step, self.hot.post_step = ds.step_begin, ds.step_end
+            self.hot.pre_step_save, self.hot.pre_step_undo = ds.save, ds.undo
+        elif getattr(args, "device_sampler", 0) and not self.masked_mode:
             from .device_sampler import DeviceSampler
             from .host_native import BatchSampler
             rowptr, col = data_generator.csr("train", sorted_rows=True)
@@ -383,12 +398,16 @@ class Trainer(object):
         With the device-side sampler B' is only known on the device (-1 here; Trainer.train reads the epoch total once)."""
         if self.device_sampler is not None:
             hp = self.hot
+            if self.ref_sampler:
+                self.device_sampler.host_is_current = False
             if self.use_graph:
                 loss = hp.replay_staged()
             else:
                 hp.pre_step()
                 gi = hp._gidx
                 loss = hp.train_step(gi[0], gi[1], gi[2], gi[3])
+                if hp.post_step is not None:
+                    hp.post_step()
             self._epoch_stats[0:1] += loss
             self._epoch_stats[1:3] += hp.head_out[0:2]
             self._epoch_stats[3:4] += hp._gidx[3, 0:1].float()
@@ -419,7 +438,9 @@ class Trainer(object):
         """Write the whole run state to `path`, at a step boundary: parameters, AdamW moments and step block, the RNG streams the samplers
         advance, and where the training loop stands.  Synchronises once, for the device-to-host copies; a training step never does."""
         live = dict(checkpoint.engine_tensors(self.hot), epoch_stats=self._epoch_stats)
-        if self.device_sampler is not None:
+        if self.ref_sampler:
+            self.device_sampler.sync_to_host()                        # the file holds `random` / `np.random` as a host-sampled run has them
+        elif self.device_sampler is not None:
             live["device_sampler"] = self.device_sampler.state
         host = checkpoint.to_host(live)
         model, optim = checkpoint.engine_sections(host, self.hot.opt)
@@ -440,7 +461,9 @@ class Trainer(object):
         if diffs:
             self.logger.logging("checkpoint %s was written with other flags (saved -> this run): %s" % (path, ", ".join(diffs)))
         self.hot.load_state(saved)
-        checkpoint.set_rng_state(ck["rng"], self.device, self.device_sampler)
+        checkpoint.set_rng_state(ck["rng"], self.device, None if self.ref_sampler else self.device_sampler)
+        if self.ref_sampler:
+            self.device_sampler.upload_from_host()                    # in place, also under a captured graph
         lp = ck["loop"]
         self._epoch_stats.copy_(lp["epoch_stats"])
         self.n_interactions = lp["n_interactions"]
@@ -506,6 +529,8 @@ class Trainer(object):
         save_dir = getattr(args, "save_dir", None)
         save_every = max(int(getattr(args, "save_every", 1)), 1)
         stopping_step, best_recall, test_ret = lp["stopping_step"], lp["best_recall"], lp["test_ret"]
+        if self.ref_sampler and self.device_sampler.host_is_current:
+            self.device_sampler.upload_from_host()                    # from `random` / `np.random` as they stand now, like the host sampler
         for epoch in range(lp["epoch"], args.epoch):
             t1 = time()
             n_batch = dg.n_train // args.batch_size + 1
@@ -517,6 +542,8 @@ class Trainer(object):
                 self.n_interactions += max(self.train_next_batch()[1], 0)
                 lp["batch"] = k + 1
             loss, mf_loss, emb_loss, n_dev = (float(x) for x in self._epoch_stats.tolist())      # the one sync per epoch
+            if self.ref_sampler:
+                self.device_sampler.check()                           # a draw that failed on the device raises here
             self.n_interactions += int(n_dev)
             reg_loss, contrastive_loss = 0.0, 0.0
             if math.isnan(loss):
@@ -558,6 +585,8 @@ class Trainer(object):
                 break
             if save_dir and (epoch + 1) % save_every == 0:
                 self.save_checkpoint(os.path.join(save_dir, "last.pt"))
+        if self.ref_sampler:
+            self.device_sampler.sync_to_host()                        # `random` / `np.random` end where a host-sampled run leaves them
         self.logger.logging(str(test_ret))
         return best_recall, run_time
 

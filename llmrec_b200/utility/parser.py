@@ -78,7 +78,7 @@ _EXTRA = [
     ("hoist_side", dict(type=int, default=0, help="1: precompute the propagation of the constant side features once (ui.X, iu.ui.X) and project only the "
                                                    "batch's rows per step (SURVEY.md 8f-3); same results within the golden tolerances; off automatically "
                                                    "when drop_rate > 0 or the mask branch is on")),
-    ("device_sampler", dict(type=int, default=0, help="1: draw the batches on the GPU (non-parity RNG stream, SURVEY.md 8f-1); 0 replays the reference's host sampling")),
+    ("device_sampler", dict(type=int, default=0, choices=[0, 1, 2], help="0: the reference's batches, drawn on the host (default); 1: batches drawn on the GPU from their own RNG stream (same distributions, other batches, SURVEY.md 8f-1); 2: the reference's exact batches, drawn on the GPU from device copies of `random` / `np.random`")),
     ("feat_dtype", dict(default="fp32", choices=["fp32", "bf16", "int8"], help="element type the side-feature tables (image, text, user profile, "
                                                                       "attributes) are kept in: bf16 rounds them once (round-to-nearest-even) "
                                                                       "when the model is built and halves their memory and projection reads; "
