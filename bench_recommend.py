@@ -1,16 +1,21 @@
-"""bench_recommend.py -- recommendation throughput (Trainer.recommend / recommend.top_k, --candidates_out) on one H100.
+"""bench_recommend.py -- recommendation throughput (Trainer.recommend / recommend.top_k, --candidates_out, item fold-in and item-to-item
+neighbours) on one H100.
 
-    python bench_recommend.py [--reps 3] [--syn_users 131072] [--syn_histories 8192] [--syn_scale 1.0]
+    python bench_recommend.py [--reps 3] [--syn_users 131072] [--syn_histories 8192] [--syn_items 65536] [--syn_scale 1.0]
 
-Three legs per workload, each timed end to end on the host clock between device synchronises (median of --reps calls after one
-warm-up call) and reported in users/s:
-  known      trained users scored from U with their training items excluded (exclude="train"), K = 10
-  fold_in    held-out histories folded in (HotPath.fold_in) and scored, exclude="train", K = 10
-  candidates the --candidates_out file: every user's top-10 over the whole catalog, nothing excluded, pickled to a temporary file
+Five legs per workload, each timed end to end on the host clock between device synchronises (median of --reps calls after one
+warm-up call):
+  known         trained users scored from U with their training items excluded (exclude="train"), K = 10; users/s
+  fold_in       held-out histories folded in (HotPath.fold_in) and scored, exclude="train", K = 10; users/s
+  candidates    the --candidates_out file: every user's top-10 over the whole catalog, nothing excluded, pickled to a temporary file;
+                users/s
+  fold_in_items trained items' user lists folded in as new items (HotPath.fold_in_items, no ID embedding); items/s
+  similar       item-to-item neighbours (recommend.similar_items) of trained items over the trained catalog, K = 10; queries/s
 Every call includes the full eval forward a recommendation starts with.
-Workloads: the netflix shape of bench.py (Trainer with side features, held-out histories = a user's training row plus its test items),
-and the 10M x 1M x 200M synthetic of dist_bench (ID-only single-GPU engine, d = 128, L = 2; histories = a training row plus two random
-items, folded in as unknown users; the known and candidates legs score the first --syn_users users).
+Workloads: the netflix shape of bench.py (Trainer with side features, held-out histories = a user's training row plus its test items;
+every item's user list and every item as a query), and the 10M x 1M x 200M synthetic of dist_bench (ID-only single-GPU engine,
+d = 128, L = 2; histories = a training row plus two random items, folded in as unknown users; the known and candidates legs score the
+first --syn_users users; the item legs take --syn_items random items).
 One JSON line on stdout with the card's name and power limit; a summary on stderr.  Needs a CUDA device (no fallback).
 """
 from __future__ import annotations
@@ -44,10 +49,10 @@ def _timed(fn, reps):
     return sorted(ts)[len(ts) // 2], min(ts), max(ts)
 
 
-def _leg(name, n_users, fn, reps):
+def _leg(name, n_users, fn, reps, unit="users"):
     med, lo, hi = _timed(fn, reps)
-    out = {"users": n_users, "s_per_call": round(med, 5), "s_min": round(lo, 5), "s_max": round(hi, 5), "users_per_s": round(n_users / med, 1)}
-    sys.stderr.write(f"  {name:10s} {n_users:9d} users  {med * 1e3:9.2f} ms/call  {n_users / med:12.0f} users/s\n")
+    out = {unit: n_users, "s_per_call": round(med, 5), "s_min": round(lo, 5), "s_max": round(hi, 5), unit + "_per_s": round(n_users / med, 1)}
+    sys.stderr.write(f"  {name:13s} {n_users:9d} {unit:7s}  {med * 1e3:9.2f} ms/call  {n_users / med:12.0f} {unit}/s\n")
     return out
 
 
@@ -65,6 +70,10 @@ def netflix(a, tmp):
            "known": _leg("known", nu, lambda: tr.recommend(K=10, exclude="train"), a.reps),
            "fold_in": _leg("fold_in", len(hist), lambda: tr.recommend(users=users, K=10, exclude="train", histories=hist), a.reps),
            "candidates": _leg("candidates", nu, lambda: tr.write_candidates(path, 10), a.reps)}
+    ni = tr.n_items
+    irp, icol = tr.graph.rowptr_i.cpu().numpy(), tr.graph.col_i.cpu().numpy()
+    res["fold_in_items"] = _leg("fold_in_items", ni, lambda: tr.fold_in_items((irp, icol)), a.reps, unit="items")
+    res["similar"] = _leg("similar", ni, lambda: tr.similar_items(np.arange(ni), K=10), a.reps, unit="queries")
     del tr, gen
     return res
 
@@ -108,9 +117,25 @@ def synthetic(a, tmp):
         ids, _ = recommend.top_k(hp, g.rowptr_u, g.col_u, users=users, K=10, exclude="none", mode=a.score_mode)
         recommend.write_candidates(path, ids)
 
+    items = np.sort(rng.choice(ni, min(a.syn_items, ni), replace=False))
+    irp, icol = g.rowptr_i.cpu().numpy(), g.col_i.cpu().numpy()
+    lists = [icol[irp[i]:irp[i + 1]] for i in items]
+    item_rp = np.concatenate([[0], np.cumsum([x.size for x in lists])])
+    item_col = np.concatenate(lists)
+
+    def fold_items():
+        hp.forward()
+        hp.fold_in_items(item_rp, item_col)
+
+    def similar():
+        hp.forward()
+        recommend.similar_items(hp, items, K=10, mode=a.score_mode)
+
     res = {"workload": f"synthetic {nu}x{ni}, {g.nnz} training edges, d={d}, L={L}, ID-only engine",
            "known": _leg("known", n, known, a.reps), "fold_in": _leg("fold_in", len(hist), fold, a.reps),
-           "candidates": _leg("candidates", n, cand, a.reps)}
+           "candidates": _leg("candidates", n, cand, a.reps),
+           "fold_in_items": _leg("fold_in_items", items.size, fold_items, a.reps, unit="items"),
+           "similar": _leg("similar", items.size, similar, a.reps, unit="queries")}
     del hp, g, params
     torch.cuda.empty_cache()
     return res
@@ -122,6 +147,7 @@ def main():
     ap.add_argument("--proj_mode", default="3xtf32", choices=["3xtf32", "tf32", "fp32"])
     ap.add_argument("--syn_users", type=int, default=131072, help="synthetic workload: users of the known and candidates legs")
     ap.add_argument("--syn_histories", type=int, default=8192, help="synthetic workload: histories of the fold-in leg")
+    ap.add_argument("--syn_items", type=int, default=65536, help="synthetic workload: items of the fold_in_items and similar legs")
     ap.add_argument("--syn_scale", type=float, default=1.0, help="size factor of the 10M x 1M x 200M synthetic graph")
     ap.add_argument("--workloads", default="netflix,synthetic")
     a = ap.parse_args()

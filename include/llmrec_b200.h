@@ -447,6 +447,9 @@ int llmrec_scatter_add_rows_f32(const float* G, int64_t ldg, const int32_t* idx,
 int llmrec_scatter_add_rows_ordered_f32(const float* G, int64_t ldg, const int32_t* idx, int32_t n, int32_t d, float* Y, int64_t ldy,
                                         int32_t* scratch, int64_t scratch_elems, llmrec_stream_t stream);
 int64_t llmrec_scatter_add_rows_ordered_scratch(int32_t n);
+/* Y[r, :] = X[r, :] / max(||X[r, :]||_2, 1e-12) for r < n (F.normalize(X, dim=1)): the unit rows of item-to-item cosine neighbours.
+ * X == Y (in place) is allowed. */
+int llmrec_row_normalize_f32(const float* X, int64_t ldx, float* Y, int64_t ldy, int64_t n, int32_t d, llmrec_stream_t stream);
 
 /* ---------------------------------------------------------------------------------------------
  * Hoisted side-feature mode (SURVEY.md 8f-3; Models.py:145-167 with dropout p = 0 and the mask branch off):

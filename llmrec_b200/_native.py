@@ -160,6 +160,7 @@ SIGNATURES = {
     "llmrec_scatter_add_rows_f32": (C.c_int, [c_f32p, C.c_int64, c_i32p, C.c_int32, C.c_int32, c_f32p, C.c_int64, c_stream]),
     "llmrec_scatter_add_rows_ordered_f32": (C.c_int, [c_f32p, C.c_int64, c_i32p, C.c_int32, C.c_int32, c_f32p, C.c_int64, c_i32p, C.c_int64, c_stream]),
     "llmrec_scatter_add_rows_ordered_scratch": (C.c_int64, [C.c_int32]),
+    "llmrec_row_normalize_f32": (C.c_int, [c_f32p, C.c_int64, c_f32p, C.c_int64, C.c_int64, C.c_int32, c_stream]),
     "llmrec_rank1_add_f32": (C.c_int, [C.POINTER(Rank1Block), C.c_int32, c_stream]),
     "llmrec_scaled_colsum_f32": (C.c_int, [C.POINTER(ColsumTerm), C.c_int32, C.c_int32, c_f32p, C.c_int32, c_f32p, c_stream]),
     "llmrec_scaled_colsum_scratch": (C.c_int64, [C.c_int32]),

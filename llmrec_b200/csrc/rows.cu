@@ -26,6 +26,20 @@ __global__ void __launch_bounds__(256) row_scale_softmax_kernel(const float* __r
   const float inv = 1.0f / t;
   for (int j = lane; j < d; j += 32) y[j] = expf(s * x[j] - m) * inv;
 }
+// Y[r,:] = X[r,:] / max(||X[r,:]||_2, 1e-12)  (F.normalize; item-to-item cosine).  One warp per row; X == Y is fine: every lane
+// rewrites only the elements it read.
+__global__ void __launch_bounds__(256) row_normalize_kernel(const float* X, int64_t ldx, float* Y, int64_t ldy, int64_t n, int d) {
+  const int lane = threadIdx.x & 31;
+  const int64_t row = (blockIdx.x * (int64_t)(blockDim.x >> 5)) + (threadIdx.x >> 5);
+  if (row >= n) return;
+  const float* x = X + row * ldx;
+  float* y = Y + row * ldy;
+  float ss = 0.f;
+  for (int j = lane; j < d; j += 32) ss = fmaf(x[j], x[j], ss);
+  ss = warp_sum(ss);
+  const float inv = 1.0f / fmaxf(sqrtf(ss), 1e-12f);
+  for (int j = lane; j < d; j += 32) y[j] = x[j] * inv;
+}
 // out[b,:] = idx[b] >= 0 ? X[idx[b],:] : 0
 __global__ void __launch_bounds__(256) gather_rows_kernel(const float* __restrict__ X, int64_t ldx, const int* __restrict__ idx, int n, int d,
                                                           float* __restrict__ out, int64_t ldo) {
@@ -160,6 +174,14 @@ extern "C" int llmrec_row_scale_softmax_f32(const float* X, int64_t ldx, const f
   if (n <= 0) return 0;
   row_scale_softmax_kernel<<<(unsigned)((n + 7) / 8), 256, 0, as_stream(stream)>>>(X, ldx, scale, Y, ldy, n, d, softmax);
   LLMREC_CHECK_LAUNCH("row_scale_softmax");
+  return 0;
+}
+extern "C" int llmrec_row_normalize_f32(const float* X, int64_t ldx, float* Y, int64_t ldy, int64_t n, int32_t d, llmrec_stream_t stream) {
+  LLMREC_REQUIRE_DEVICE();
+  if (n <= 0) return 0;
+  LLMREC_CHECK_ARG(X && Y && d > 0 && ldx >= d && ldy >= d, "row_normalize: need X, Y, d > 0 and leading dimensions >= d");
+  row_normalize_kernel<<<(unsigned)((n + 7) / 8), 256, 0, as_stream(stream)>>>(X, ldx, Y, ldy, n, d);
+  LLMREC_CHECK_LAUNCH("row_normalize");
   return 0;
 }
 extern "C" int llmrec_gather_rows_f32(const float* X, int64_t ldx, const int32_t* idx, int32_t n, int32_t d, float* out, int64_t ldo,

@@ -78,6 +78,15 @@ PARAM_ORDER = ("image_trans.weight", "image_trans.bias", "text_trans.weight", "t
                "user_id_embedding.weight", "item_id_embedding.weight")
 
 
+def _known_ids(known, m, n, msg):
+    """The `known` argument of a fold-in: None (every row -1) or one id in [0, n) or -1 per row -> int64[m]; else ValueError(msg)."""
+    kn = np.full(m, -1, dtype=np.int64) if known is None else \
+        (known.detach().cpu().numpy() if hasattr(known, "detach") else np.asarray(known)).astype(np.int64).reshape(-1)
+    if kn.size != m or (m and (kn.min() < -1 or kn.max() >= n)):
+        raise ValueError(msg.format(n=n, m=m))
+    return kn
+
+
 class KernelTimer:
     """CUDA-event timer per kernel family on the current stream (bench.py's roofline leg)."""
 
@@ -363,10 +372,7 @@ class HotPath:
         from .graph import history_matrix, inv_sqrt_degree
         R = history_matrix(rowptr, col, self.ni)
         m, d, L, dev = R.shape[0], self.d, self.L, self.E_u.device
-        kn = np.full(m, -1, dtype=np.int32) if known is None else \
-            (known.detach().cpu().numpy() if hasattr(known, "detach") else np.asarray(known)).astype(np.int64).reshape(-1)
-        if kn.size != m or (m and (kn.min() < -1 or kn.max() >= self.nu)):
-            raise ValueError(f"fold_in: known must hold one trained user id in [0, {self.nu}) or -1 per history ({m})")
+        kn = _known_ids(known, m, self.nu, "fold_in: known must hold one trained user id in [0, {n}) or -1 per history ({m})")
         if m == 0:
             return torch.empty(0, d, dtype=torch.float32, device=dev)
         t = lambda a, dt: torch.from_numpy(np.ascontiguousarray(a.astype(dt))).to(dev)
@@ -415,6 +421,50 @@ class HotPath:
         probs += [(x["item"][k], p["item_trans.weight"], p["item_trans.bias"], self.blk(self.Pi, 2 + j), dead) for j, k in enumerate(self.keys)]
         probs.sort(key=lambda t: -t[0].shape[1])
         ops.proj_fwd_group(probs, self.d, self.cfg.proj_mode)
+
+    # ---- item fold-in: the item side of the forward for items added after training -------------------------------------------
+    def fold_in_items(self, rowptr, col, known=None):
+        """-> I_new [m x d]: the fused representation of m items whose interactions are the rows of an int CSR over trained user ids
+        (rowptr[m+1], col; `graph.history_matrix` rejects ids outside [0, n_users) and collapses repeats).  known: optional int[m], the
+        trained item id of each row or -1.  Reads the user side of the last full `forward()` (Fu, P_usr, Ul) and the parameters; writes
+        no buffer a training step reads.
+
+        The mirror of `fold_in`: every item-side quantity of the forward is the item's row of iu = diag(si) R^T times a user-side
+        tensor (Fi = iu.Fu, prof_i = iu.P_usr, Il[l] = [softmax] iu.Ul[l]), so with R^T the new rows and si their (deg + 1e-8)^-1/2 these
+        are ONE SpMM launch with S + 1 + L segments, followed by the fusion of the m rows.  Layer 0 is E_i[known] for a trained item and
+        a zero row for a new one.  The item's own side features enter no term of its row (they reach items only through two hops)."""
+        from .graph import history_matrix, inv_sqrt_degree
+        R = history_matrix(rowptr, col, self.nu, what="new items", unit="user id")
+        m, d, L, dev = R.shape[0], self.d, self.L, self.E_i.device
+        kn = _known_ids(known, m, self.ni, "fold_in_items: known must hold one trained item id in [0, {n}) or -1 per item ({m})")
+        if m == 0:
+            return torch.empty(0, d, dtype=torch.float32, device=dev)
+        t = lambda a, dt: torch.from_numpy(np.ascontiguousarray(a.astype(dt))).to(dev)
+        op = ops.CsrOperator(t(R.indptr, np.int32), t(R.indices, np.int32), m, self.nu, rs=t(inv_sqrt_degree(R), np.float32),
+                             tile_nnz=getattr(self.iu.plan, "tile_nnz", 0))       # pieces cut as the training operator cuts them
+        new = lambda *s: torch.empty(*s, dtype=torch.float32, device=dev)
+        Il = [new(m, d) for _ in range(L + 1)]
+        Fi, prof_i = (new(m, self.S * d), new(m, d)) if self.has_feats else (None, None)
+        if self.has_feats:
+            self._fold_in_profiles()
+        op.apply(self._fold_in_items_segs(Fi, prof_i, Il))
+        ops.gather_rows(self.E_i, t(kn, np.int32), Il[0])                      # known -> E_i row, -1 -> zeros
+        si = [self.blk(Fi, 0), self.blk(Fi, 1), prof_i] + [self.blk(Fi, 2 + j) for j in range(len(self.keys))] if self.has_feats else []
+        I = new(m, d)
+        ops.fuse_fwd(Il, si, self._side_coefs(), I)                                                            # :185-197
+        return I
+
+    def _fold_in_items_segs(self, Fi, prof_i, Il):
+        """The segments of the one item fold-in launch: Fu's S blocks -> Fi, P_usr -> prof_i, Ul[l] -> Il[l] (softmax on l = L)."""
+        segs = []
+        if self.has_feats:
+            segs += [(self.blk(self.Fu, s), self.blk(Fi, s), None, False) for s in range(self.S)]              # :154,157,163
+            segs.append((self.P_usr, prof_i, None, False))                                                      # :166
+        segs += [(self.Ul[l], Il[l], None, l == self.L) for l in range(1, self.L + 1)]                        # :175,180
+        return segs
+
+    def _fold_in_profiles(self):
+        """Make P_usr hold X_usr.W_u^T + b_u before an item fold-in.  The forward of this engine projects every user row, so it does."""
 
     # ---- backward: expects gU, gI and (GFu, GFi, Gprof_u, Gprof_i, GP_usr_direct) filled ---------------
     def backward(self, gp_usr_direct=None, batch_rows=False):

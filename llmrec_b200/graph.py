@@ -30,36 +30,37 @@ def inv_sqrt_degree(mat: sp.spmatrix) -> np.ndarray:
     return s
 
 
-def history_matrix(rowptr, col, n_items: int) -> sp.csr_matrix:
+def history_matrix(rowptr, col, n_items: int, what: str = "histories", unit: str = "item id") -> sp.csr_matrix:
     """m interaction histories given at call time (int CSR over item ids: rowptr[m+1], col[nnz]; arrays, lists or tensors on any
     device) -> the binary [m x n_items] CSR with sorted rows, a repeated id within a row collapsed as BipartiteGraph does for R.
-    An id outside [0, n_items) raises ValueError."""
+    An id outside [0, n_items) raises ValueError.  The same holds for the user lists of new items (columns = user ids); `what` and
+    `unit` name the input in the error messages."""
     as_np = lambda a: (a.detach().cpu().numpy() if hasattr(a, "detach") else np.asarray(a)).astype(np.int64).reshape(-1)
     rp, c = as_np(rowptr), as_np(col)
     if rp.size < 1 or rp[0] != 0 or np.any(np.diff(rp) < 0) or rp[-1] != c.size:
-        raise ValueError(f"histories: rowptr must start at 0, never decrease and end at len(col) = {c.size}")
+        raise ValueError(f"{what}: rowptr must start at 0, never decrease and end at len(col) = {c.size}")
     if c.size and (c.min() < 0 or c.max() >= n_items):
         bad = int(c[(c < 0) | (c >= n_items)][0])
-        raise ValueError(f"histories: item id {bad} is outside [0, {n_items})")
+        raise ValueError(f"{what}: {unit} {bad} is outside [0, {n_items})")
     m = rp.size - 1
     R = sp.csr_matrix((np.ones(c.size, dtype=np.float32), c, rp), shape=(m, n_items))
     R.sum_duplicates()
     R.sort_indices()
     R.data[:] = 1.0
     if R.nnz >= 2 ** 31:
-        raise ValueError("histories too large for int32 CSR")
+        raise ValueError(f"{what} too large for int32 CSR")
     return R
 
 
-def histories_csr(histories, n_items: int) -> sp.csr_matrix:
+def histories_csr(histories, n_items: int, what: str = "histories", unit: str = "item id") -> sp.csr_matrix:
     """`history_matrix` of either form a caller may hold: a (rowptr, col) pair (a tuple of two arrays / tensors), or a sequence of
     item-id lists, one per history."""
     if isinstance(histories, tuple) and len(histories) == 2 and all(hasattr(a, "shape") for a in histories):
-        return history_matrix(histories[0], histories[1], n_items)
+        return history_matrix(histories[0], histories[1], n_items, what, unit)
     rows = [np.asarray(list(h), dtype=np.int64).reshape(-1) for h in histories]
     rp = np.zeros(len(rows) + 1, dtype=np.int64)
     rp[1:] = np.cumsum([r.size for r in rows])
-    return history_matrix(rp, np.concatenate(rows) if rows else np.zeros(0, np.int64), n_items)
+    return history_matrix(rp, np.concatenate(rows) if rows else np.zeros(0, np.int64), n_items, what, unit)
 
 
 class BipartiteGraph:

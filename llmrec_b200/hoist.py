@@ -117,6 +117,13 @@ class HoistedHotPath(HotPath):
         probs.sort(key=lambda t: -t[0].shape[1])
         ops.proj_fwd_group(probs, self.d, self.cfg.proj_mode)
 
+    def _fold_in_profiles(self):
+        """fold_in_items reads P_usr = X_usr.W_u^T + b_u, which this engine never materialises (its prof_u / prof_i come from TU / TI):
+        one projection of the user table per call, into the engine's P_usr, which no hoisted step reads.  Its Fu, which fold_in_items
+        also reads, is written by the forward (TU.W^T + cu b^T)."""
+        p = self.p
+        ops.proj_fwd_group([(self.feats["user"], p["user_trans.weight"], p["user_trans.bias"], self.P_usr)], self.d, self.cfg.proj_mode)
+
     # ---- compact buffers of a training step ---------------------------------------------------------------------------
     def _ensure_compact(self, cap):
         c = self._compact

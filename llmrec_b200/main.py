@@ -493,23 +493,46 @@ class Trainer(object):
             self.hot.forward()
         return self.hot
 
-    def recommend(self, users=None, K=10, exclude="train", histories=None):
+    def recommend(self, users=None, K=10, exclude="train", histories=None, new_items=None):
         """-> (ids int64 [m x K], scores fp32 [m x K]) on the device: each row's K best items, ties to the lowest item id, padded with
         -1 / -inf when fewer than K items are left.
         users: trained user ids (default every user).  histories: item-id lists or a (rowptr, col) pair, folded in with the trained item
-        side (HotPath.fold_in); `users` then names each history's trained id (or -1) and may be omitted.  exclude: "train" masks a
-        trained user's training items and a history's own items; "none" masks nothing (the reference's candidate lists).  K: 1..64 and
-        at most n_items.  --proj_mode picks the scoring mode."""
-        recommend.check_k(K, self.n_items)
+        side (HotPath.fold_in); `users` then names each history's trained id (or -1) and may be omitted.  new_items: the user lists of m
+        items added after training (user-id lists or a (rowptr, col) pair), folded in with the trained user side (HotPath.fold_in_items)
+        and scored after the trained catalog as ids n_items + j.  exclude: "train" masks a trained user's training items and a history's
+        own items, and every new item whose list names the user (a history: its trained id); "none" masks nothing (the reference's
+        candidate lists).  K: 1..64 and at most the catalog size.  --proj_mode picks the scoring mode."""
+        Rn = recommend.new_items_csr(new_items, self.n_users)
+        recommend.check_k(K, self.n_items + (0 if Rn is None else Rn.shape[0]))
         hot = self._current_model()
         mode = ops.SCORE_MODE.get(getattr(self.args, "proj_mode", "3xtf32"), 0)
-        return recommend.top_k(hot, self.graph.rowptr_u, self.graph.col_u, users=users, K=K, exclude=exclude, histories=histories, mode=mode)
+        return recommend.top_k(hot, self.graph.rowptr_u, self.graph.col_u, users=users, K=K, exclude=exclude, histories=histories, mode=mode,
+                               new_items=Rn)
 
     def fold_in(self, histories, known=None):
         """-> U_new [m x d]: the fused user representations of item-id histories (lists or a (rowptr, col) pair) under the current
         parameters; known: each history's trained user id or -1 (layer 0 = that user's ID embedding, or zero)."""
         R = histories_csr(histories, self.n_items)
         return self._current_model().fold_in(R.indptr, R.indices, known=known)
+
+    def fold_in_items(self, user_lists, known=None):
+        """-> I_new [m x d]: the fused item representations of items given by the trained users who interacted with each (user-id lists
+        or a (rowptr, col) pair) under the current parameters; known: each item's trained id or -1 (layer 0 = that item's ID embedding,
+        or zero).  No feature rows are needed: an item's own side features do not enter its row."""
+        R = recommend.new_items_csr(user_lists, self.n_users)
+        if R is None:
+            raise ValueError("fold_in_items: give one user-id list per item")
+        return self._current_model().fold_in_items(R.indptr, R.indices, known=known)
+
+    def similar_items(self, items, K=10, new_items=None):
+        """-> (ids int64 [q x K], cosines fp32 [q x K]) on the device: each query item's K nearest items by cosine of the fused item rows,
+        never the query itself, ties to the lowest id, padded with -1 / -inf.  items: trained ids, or n_items + j for the j-th of
+        `new_items` (user lists of items added after training, as for `recommend`).  K: 1..64 and below the catalog size."""
+        Rn = recommend.new_items_csr(new_items, self.n_users)
+        recommend.check_k(K, self.n_items + (0 if Rn is None else Rn.shape[0]) - 1, "the catalog size - 1")
+        hot = self._current_model()
+        mode = ops.SCORE_MODE.get(getattr(self.args, "proj_mode", "3xtf32"), 0)
+        return recommend.similar_items(hot, items, K=K, new_items=Rn, mode=mode)
 
     def write_candidates(self, path, K=10):
         """--candidates_out: the top-K of every user over the whole catalog, nothing excluded (torch.topk(U . I^T, k=K) of the reference's

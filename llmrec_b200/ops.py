@@ -597,6 +597,16 @@ def row_scale_softmax(X, scale, out, softmax):
     return out
 
 
+def row_normalize(X, out=None):
+    """out = X / max(||X||_2, 1e-12) row by row (F.normalize(X, dim=1)); out may be X."""
+    out = torch.empty((X.shape[0], X.shape[1]), dtype=torch.float32, device=X.device) if out is None else out
+    if tuple(out.shape) != tuple(X.shape):
+        raise ValueError(f"row_normalize: out {tuple(out.shape)} differs from X {tuple(X.shape)}")
+    N.check(N.lib().llmrec_row_normalize_f32(_p(_mat(X)), _ld(X), _p(_mat(out)), _ld(out), X.shape[0], X.shape[1], _stream()), "row_normalize")
+    _count()
+    return out
+
+
 def gather_rows(X, idx, out):
     N.check(N.lib().llmrec_gather_rows_f32(_p(_mat(X)), _ld(X), _p(_i32(idx)), idx.numel(), X.shape[1], _p(_mat(out)), _ld(out), _stream()), "gather_rows")
     _count()
