@@ -26,32 +26,21 @@ class _HotPathFn(torch.autograd.Function):
         hp.forward()
         hp._version = getattr(hp, "_version", 0) + 1
         ctx.hp, ctx.version = hp, hp._version
-        v = hp.side_views()
-        outs = [hp.U, hp.I, v["img_i"], v["txt_i"], v["img_u"], v["txt_u"], v["p_usr"], v["prof_u"], v["prof_i"]]
-        outs += [v["att_u"][k] for k in hp.keys] + [v["att_i"][k] for k in hp.keys]
-        return tuple(o.clone() for o in outs)
+        return tuple(o.clone() for o, _ in hp.outputs())
 
     @staticmethod
     def backward(ctx, *g):
         hp = ctx.hp
         if ctx.version != hp._version:
             raise RuntimeError("MM_Model.forward was called again before backward; the fused path keeps one live forward")
-        K = len(hp.keys)
-
-        def put(dst, src):
-            if src is None:
+        direct = None
+        for (_, dst), src in zip(hp.outputs(), g):
+            if dst is None:                                       # p_usr: its gradient is added in the backward chain
+                direct = src.contiguous() if src is not None else None
+            elif src is None:
                 dst.zero_()
             else:
                 dst.copy_(src)
-
-        put(hp.gU, g[0]); put(hp.gI, g[1])
-        put(hp.blk(hp.GFi, 0), g[2]); put(hp.blk(hp.GFi, 1), g[3])
-        put(hp.blk(hp.GFu, 0), g[4]); put(hp.blk(hp.GFu, 1), g[5])
-        put(hp.Gprof_u, g[7]); put(hp.Gprof_i, g[8])
-        for j in range(K):
-            put(hp.blk(hp.GFu, 2 + j), g[9 + j])
-            put(hp.blk(hp.GFi, 2 + j), g[9 + K + j])
-        direct = g[6].contiguous() if g[6] is not None else None
         grads = hp.backward(gp_usr_direct=direct)
         return (None,) + tuple(grads[n].clone() for n in PARAM_ORDER)
 

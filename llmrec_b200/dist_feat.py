@@ -24,6 +24,7 @@ import torch.distributed as dist
 from . import ops
 from .dist import ShardedGraph, owner_local_index, shard_bounds
 from .engine import HotPathConfig, PARAM_ORDER
+from .sides import SideLayout
 
 
 class ShardedFeatureHotPath:
@@ -40,7 +41,8 @@ class ShardedFeatureHotPath:
         self.nu, self.ni, self.d, self.L = nu, ni, d, L
         self.lo, self.hi = int(user_lo), int(user_lo) + nu
         self.keys = list(feats_local["item"].keys())
-        S = self.S = 2 + len(self.keys)
+        self.sides = SideLayout(self.keys, d)
+        S = self.S = self.sides.S
         self.ilo, self.ihi = int(item_lo), int(item_lo) + feats_local["image"].shape[0]
         self.even_items = self.world > 1 and ni % self.world == 0 and (self.ihi - self.ilo) * self.world == ni
         dev = self.E_i.device
@@ -69,7 +71,7 @@ class ShardedFeatureHotPath:
         self.opt.lr = lr
 
     def blk(self, buf, s):
-        return buf[:, s * self.d:(s + 1) * self.d]
+        return self.sides.blk(buf, s)
 
     # -- collectives ---------------------------------------------------------------------------------------------------------
     def _allreduce(self, t):
@@ -96,15 +98,9 @@ class ShardedFeatureHotPath:
 
     # -- forward (Models.py:145-197) --------------------------------------------------------------------------------------------
     def forward(self):
-        g, p, f, d, S, L, m = self.g, self.p, self.f, self.d, self.S, self.L, self.cfg.proj_mode
-        own = self.Pi[self.ilo:self.ihi]
-        probs = [(f["image"], p["image_trans.weight"], p["image_trans.bias"], self.blk(own, 0)),
-                 (f["text"], p["text_trans.weight"], p["text_trans.bias"], self.blk(own, 1))]
-        probs += [(f["item"][k], p["item_trans.weight"], p["item_trans.bias"], self.blk(own, 2 + j)) for j, k in enumerate(self.keys)]
-        probs.append((f["user"], p["user_trans.weight"], p["user_trans.bias"], self.P_usr))
-        probs = [t for t in probs if t[0].shape[0] > 0]
-        probs.sort(key=lambda t: -t[0].shape[1])
-        ops.proj_fwd_group(probs, d, m)                                                                   # :145-150, this rank's rows
+        g, sd, d, S, L, m = self.g, self.sides, self.d, self.S, self.L, self.cfg.proj_mode
+        probs = sd.proj_problems(self.f, self.p, self.Pi[self.ilo:self.ihi], self.P_usr)
+        ops.proj_fwd_group([t for t in probs if t[0].shape[0] > 0], d, m)                                  # :145-150, this rank's rows
         self._gather_item_rows(self.Pi)
         g.ui.apply([(self.blk(self.Pi, s), self.blk(self.Fu, s), None, False) for s in range(S)] + [(self.Il[0], self.Ul[1], None, L == 1)])
         self._item_sum(g.iu_raw, [(self.blk(self.Fu, s), self.blk(self.part_w, s)) for s in range(S)], self.part_w, self.Fi)   # :154,157,163
@@ -118,10 +114,7 @@ class ShardedFeatureHotPath:
             self._item_sum(g.iu_raw, [(self.Ul[l], self.part)], self.part, self.Il[l], l == L)
             if l < L:
                 g.ui.apply([(self.Il[l], self.Ul[l + 1], None, l + 1 == L)])
-        c = self.cfg
-        coefs = [c.model_cat_rate, c.model_cat_rate, c.user_cat_rate] + [c.item_cat_rate] * len(self.keys)
-        su = [self.blk(self.Fu, 0), self.blk(self.Fu, 1), self.prof_u] + [self.blk(self.Fu, 2 + j) for j in range(len(self.keys))]
-        si = [self.blk(self.Fi, 0), self.blk(self.Fi, 1), self.prof_i] + [self.blk(self.Fi, 2 + j) for j in range(len(self.keys))]
+        coefs, su, si = sd.coefs(self.cfg), sd.fused(self.Fu, self.prof_u), sd.fused(self.Fi, self.prof_i)
         ops.fuse_fwd(self.Ul, su, coefs, self.U)                                                           # :185-197
         ops.fuse_fwd(self.Il, si, coefs, self.I)
         self._fuse_args = (coefs, su, si)
@@ -146,15 +139,11 @@ class ShardedFeatureHotPath:
         self._allreduce(self.Ub4)
         for t in (self.loss, self.loss_local, self.gUb4, self.gU, self.gI, self.GFu, self.GFi, self.Gprof_u, self.Gprof_i):
             t.zero_()
-        creg = c.feat_reg_decay / self.ni
-        d2 = 2 * d
-        ops.sqnorm_grad(self.Fu[:, :d2], self.GFu[:, :d2], creg, False, self.loss_local)                   # this rank's users only
-        ops.sqnorm_grad(self.Fi[:, :d2], self.GFi[:, :d2], creg, False, self.loss)                         # replicated
-        heads = [(ub(0), self.I, gb(0), self.gI, 1.0, 1.0),
-                 (ub(1), self.blk(self.Fi, 0), gb(1), self.blk(self.GFi, 0), c.mm_mf_rate, 0.0),
-                 (ub(2), self.blk(self.Fi, 1), gb(2), self.blk(self.GFi, 1), c.mm_mf_rate, 0.0)]
-        for j in range(len(self.keys)):
-            heads.append((ub(3), self.blk(self.Fi, 2 + j), gb(3), self.blk(self.GFi, 2 + j), c.aug_mf_rate, 0.0))
+        creg, sd = c.feat_reg_decay / self.ni, self.sides
+        ops.sqnorm_grad(sd.reg(self.Fu), sd.reg(self.GFu), creg, False, self.loss_local)                   # this rank's users only
+        ops.sqnorm_grad(sd.reg(self.Fi), sd.reg(self.GFi), creg, False, self.loss)                         # replicated
+        # the gathered user rows: U | img_u | txt_u | prof_u, so blocks 0 and 1 of Ub4[:, d:] are the image and text rows
+        heads = [(ub(0), self.I, gb(0), self.gI, 1.0, 1.0)] + sd.heads(c, self.Ub4[:, d:], ub(3), self.gUb4[:, d:], gb(3), self.Fi, self.GFi)
         ops.bpr_heads(heads, self.arange, pos, neg, n_keep, c.regs0 / c.batch_size, self.head_out, self.loss, self.work)
         for s, dst in enumerate((self.gU, self.blk(self.GFu, 0), self.blk(self.GFu, 1), self.Gprof_u)):   # user-row grads to their owners
             ops.scatter_add_rows(gb(s), local, dst)
@@ -165,11 +154,9 @@ class ShardedFeatureHotPath:
     # -- backward ---------------------------------------------------------------------------------------------------------------
     def backward(self):
         g, d, S, L, m = self.g, self.d, self.S, self.L, self.cfg.proj_mode
-        G, f = self.grads, self.f
+        G, sd = self.grads, self.sides
         coefs, su, si = self._fuse_args
-        nk = len(self.keys)
-        dsu = [self.blk(self.GFu, 0), self.blk(self.GFu, 1), self.Gprof_u] + [self.blk(self.GFu, 2 + j) for j in range(nk)]
-        dsi = [self.blk(self.GFi, 0), self.blk(self.GFi, 1), self.Gprof_i] + [self.blk(self.GFi, 2 + j) for j in range(nk)]
+        dsu, dsi = sd.fused(self.GFu, self.Gprof_u), sd.fused(self.GFi, self.Gprof_i)
         dUl = G["user_id_embedding.weight"]
         ops.fuse_bwd(self.gU, L + 1, dUl, su, coefs, dsu, True)
         ops.fuse_bwd(self.gI, L + 1, self.dIl, si, coefs, dsi, True)
@@ -196,31 +183,19 @@ class ShardedFeatureHotPath:
                 self._allreduce(self.part_w)                                                               # = GPi (all item rows)
             g_cur = dst
         G["item_id_embedding.weight"].copy_(g_cur)
-        # weight gradients: this rank's item rows / user rows, then one all-reduce per tensor
-        own = self.part_w[self.ilo:self.ihi]
-        probs = [(f["item"][k], self.blk(own, 2 + j), G["item_trans.weight"], G["item_trans.bias"], j > 0) for j, k in enumerate(self.keys)]
-        probs.append((f["user"], self.GP_usr, G["user_trans.weight"], G["user_trans.bias"], False))
-        probs.append((f["text"], self.blk(own, 1), G["text_trans.weight"], G["text_trans.bias"], False))
-        probs.append((f["image"], self.blk(own, 0), G["image_trans.weight"], G["image_trans.bias"], False))
+        # weight gradients: this rank's item rows / user rows, then one all-reduce per tensor.  A rank holds rows of every item table
+        # or of none, so dropping the empty tables keeps each dW's first problem the one that does not accumulate
+        probs = sd.wgrad_problems(self.f, G, self.part_w[self.ilo:self.ihi], self.GP_usr)
         live = [t for t in probs if t[0].shape[0] > 0]
         for name in ("image_trans", "text_trans", "user_trans", "item_trans"):
             if not any(t[2] is G[name + ".weight"] for t in live):                                        # a rank without rows of that table
                 G[name + ".weight"].zero_(); G[name + ".bias"].zero_()
         if live:
-            ops.proj_wgrad_group(self._fix_accumulate(live), d, m)
+            ops.proj_wgrad_group(live, d, m)
         for name in ("image_trans", "text_trans", "user_trans", "item_trans"):
             self._allreduce(G[name + ".weight"])
             self._allreduce(G[name + ".bias"])
         return G
-
-    @staticmethod
-    def _fix_accumulate(probs):
-        """accumulate flags must be False for the first problem writing a given dW and True for the later ones."""
-        seen, out = set(), []
-        for X, dY, dW, db, _ in probs:
-            out.append((X, dY, dW, db, id(dW) in seen))
-            seen.add(id(dW))
-        return out
 
     def train_step(self, users, pos, neg):
         self.forward()

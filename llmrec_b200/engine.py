@@ -53,6 +53,7 @@ import numpy as np
 import torch
 
 from . import ops
+from .sides import SideLayout
 
 
 @dataclass
@@ -133,14 +134,14 @@ class HotPath:
         new = lambda *s: torch.empty(*s, dtype=torch.float32, device=dev)
         self.has_feats = feats is not None
         self.keys = list(feats["item"].keys()) if self.has_feats else []
-        S = self.S = (2 + len(self.keys)) if self.has_feats else 0
+        self.sides = SideLayout(self.keys, d) if self.has_feats else None
+        S = self.S = self.sides.S if self.has_feats else 0
         self.fx = feats                                                    # what the projection kernels read
         if self.has_feats:
             self.Pi, self.Fu, self.Fi = new(ni, S * d), new(nu, S * d), new(ni, S * d)
             self.P_usr, self.prof_i, self.prof_u = new(nu, d), new(ni, d), new(nu, d)
             self.GPi, self.GFu, self.GFi = new(ni, S * d), new(nu, S * d), new(ni, S * d)
             self.GP_usr, self.Gprof_i, self.Gprof_u = new(nu, d), new(ni, d), new(nu, d)
-            self.names = ["img", "txt"] + ["att:" + k for k in self.keys]
         self.Ul = [self.E_u] + [new(nu, d) for _ in range(L)]
         self.Il = [self.E_i] + [new(ni, d) for _ in range(L)]
         self.U, self.I = new(nu, d), new(ni, d)
@@ -251,15 +252,26 @@ class HotPath:
         d = self.d
         return buf[:, s * d:(s + 1) * d]
 
-    def side_views(self):
-        """name -> tensor views in the order of the reference's return tuple (Models.py:199)."""
+    def side_views(self, grads=False):
+        """name -> tensor views of the side outputs of the reference's return tuple (Models.py:199); att_i / att_u: key -> view.
+        grads: their gradient buffers instead (p_usr has none: its gradient enters `backward` as gp_usr_direct)."""
         if not self.has_feats:
             return {}
-        v = dict(img_i=self.blk(self.Fi, 0), txt_i=self.blk(self.Fi, 1), img_u=self.blk(self.Fu, 0), txt_u=self.blk(self.Fu, 1),
-                 p_usr=self.P_usr, prof_u=self.prof_u, prof_i=self.prof_i,
-                 att_i={k: self.blk(self.Fi, 2 + j) for j, k in enumerate(self.keys)},
-                 att_u={k: self.blk(self.Fu, 2 + j) for j, k in enumerate(self.keys)})
-        return v
+        Fu, Fi, P_usr, prof_u, prof_i = ((self.GFu, self.GFi, None, self.Gprof_u, self.Gprof_i) if grads else
+                                         (self.Fu, self.Fi, self.P_usr, self.prof_u, self.prof_i))
+        b, att = self.blk, self.sides.att
+        return dict(img_i=b(Fi, 0), txt_i=b(Fi, 1), img_u=b(Fu, 0), txt_u=b(Fu, 1), p_usr=P_usr, prof_u=prof_u, prof_i=prof_i,
+                    att_i=dict(zip(self.keys, att(Fi))), att_u=dict(zip(self.keys, att(Fu))))
+
+    def outputs(self):
+        """(output, gradient buffer) pairs in the order of the reference's return tuple (Models.py:199): U, I, img_i, txt_i, img_u,
+        txt_u, p_usr, prof_u, prof_i, att_u per key, att_i per key."""
+        out = [(self.U, self.gU), (self.I, self.gI)]
+        if self.has_feats:
+            v, g = self.side_views(), self.side_views(grads=True)
+            out += [(v[n], g[n]) for n in ("img_i", "txt_i", "img_u", "txt_u", "p_usr", "prof_u", "prof_i")]
+            out += [(v[a][k], g[a][k]) for a in ("att_u", "att_i") for k in self.keys]
+        return out
 
     # ---- forward -------------------------------------------------------------------------------
     def forward(self):
@@ -269,17 +281,9 @@ class HotPath:
         return self.U, self.I
 
     def _proj_fwd(self):
-        d, m = self.d, self.cfg.proj_mode
-        p, f = self.p, self.fx
         if self.has_feats:
-            with self._t("proj_fwd"):                                                                                # Models.py:145-150
-                rows = () if self.live_i is None else (self.live_i,)                                  # compact item tables -> Pi[live_i]
-                probs = [(f["image"], p["image_trans.weight"], p["image_trans.bias"], self.blk(self.Pi, 0), *rows),
-                         (f["text"], p["text_trans.weight"], p["text_trans.bias"], self.blk(self.Pi, 1), *rows)]
-                probs += [(f["item"][k], p["item_trans.weight"], p["item_trans.bias"], self.blk(self.Pi, 2 + j), *rows) for j, k in enumerate(self.keys)]
-                probs.append((f["user"], p["user_trans.weight"], p["user_trans.bias"], self.P_usr))
-                probs.sort(key=lambda t: -t[0].shape[1])                       # long-K tiles first
-                ops.proj_fwd_group(probs, d, m)
+            with self._t("proj_fwd"):                                                    # compact item tables -> Pi[live_i]
+                ops.proj_fwd_group(self.sides.proj_problems(self.fx, self.p, self.Pi, self.P_usr, self.live_i), self.d, self.cfg.proj_mode)
 
     def _prop_fwd(self, with_feats=None, after_sides=None, with_ids=True, opset=None):
         """with_feats=False: the ID layers only (the hoisted mode propagates no side-feature operand); with_ids=False: the side-feature
@@ -339,18 +343,14 @@ class HotPath:
                 dict(rows=self.batch_i.list, count=self.batch_i.count, max_rows=mi))
 
     def _side_coefs(self):
-        """fusion weights of the side terms, in the order of the side lists (img, txt, profile, attributes; Models.py:185-197)"""
-        c = self.cfg
-        return [c.model_cat_rate, c.model_cat_rate, c.user_cat_rate] + [c.item_cat_rate] * len(self.keys) if self.has_feats else []
+        """fusion weights of the side terms (SideLayout.coefs; none without side features)"""
+        return self.sides.coefs(self.cfg) if self.has_feats else []
 
     def _fuse_fwd(self, batch_rows=False):
         """batch_rows: U / I on the batch's rows only (train_step); the other rows keep whatever they held."""
+        coefs, su, si = self._side_coefs(), [], []
         if self.has_feats:
-            coefs = self._side_coefs()
-            su = [self.blk(self.Fu, 0), self.blk(self.Fu, 1), self.prof_u] + [self.blk(self.Fu, 2 + j) for j in range(len(self.keys))]
-            si = [self.blk(self.Fi, 0), self.blk(self.Fi, 1), self.prof_i] + [self.blk(self.Fi, 2 + j) for j in range(len(self.keys))]
-        else:
-            coefs, su, si = [], [], []
+            su, si = self.sides.fused(self.Fu, self.prof_u), self.sides.fused(self.Fi, self.prof_i)
         ku, ki = self._rows_kw(batch_rows)
         with self._t("fuse_fwd"):
             self._fork(lambda: ops.fuse_fwd(self.Ul, su, coefs, self.U, **ku))                                         # :185-197
@@ -358,7 +358,7 @@ class HotPath:
             self._join()
         self._fuse_args = (coefs, su, si)
 
-    # ---- fold-in: the user side of the forward for interaction histories given at call time -----------------------------------
+    # ---- fold-in: one side of the forward for rows given at call time ----------------------------------------------------------
     def fold_in(self, rowptr, col, known=None):
         """-> U_new [m x d]: the fused representation of m users whose histories are the rows of an int CSR over item ids (rowptr[m+1],
         col; `graph.history_matrix` rejects ids outside [0, n_items) and collapses repeats).  known: optional int[m], the trained user id
@@ -369,60 +369,11 @@ class HotPath:
         prof_u = ui.prof_i, Ul[l] = [softmax] ui.Il[l-1]), so with R the new rows and su their (deg + 1e-8)^-1/2 these are ONE SpMM
         launch with S + 1 + L segments, followed by the fusion of the m rows.  Layer 0 is E_u[known] for a trained user; an unknown user
         has no ID embedding, and its layer 0 is a zero row (it enters the mean of the L + 1 layers as 0)."""
-        from .graph import history_matrix, inv_sqrt_degree
+        from .graph import history_matrix
         R = history_matrix(rowptr, col, self.ni)
-        m, d, L, dev = R.shape[0], self.d, self.L, self.E_u.device
-        kn = _known_ids(known, m, self.nu, "fold_in: known must hold one trained user id in [0, {n}) or -1 per history ({m})")
-        if m == 0:
-            return torch.empty(0, d, dtype=torch.float32, device=dev)
-        t = lambda a, dt: torch.from_numpy(np.ascontiguousarray(a.astype(dt))).to(dev)
-        op = ops.CsrOperator(t(R.indptr, np.int32), t(R.indices, np.int32), m, self.ni, rs=t(inv_sqrt_degree(R), np.float32),
-                             tile_nnz=getattr(self.ui.plan, "tile_nnz", 0))       # pieces cut as the training operator cuts them
-        new = lambda *s: torch.empty(*s, dtype=torch.float32, device=dev)
-        Ul = [new(m, d) for _ in range(L + 1)]
-        Fu, prof_u = (new(m, self.S * d), new(m, d)) if self.has_feats else (None, None)
-        if self.has_feats:
-            self._fold_in_items(np.unique(R.indices))
-        op.apply(self._fold_in_segs(Fu, prof_u, Ul))
-        ops.gather_rows(self.E_u, t(kn, np.int32), Ul[0])                      # known -> E_u row, -1 -> zeros
-        su = [self.blk(Fu, 0), self.blk(Fu, 1), prof_u] + [self.blk(Fu, 2 + j) for j in range(len(self.keys))] if self.has_feats else []
-        U = new(m, d)
-        ops.fuse_fwd(Ul, su, self._side_coefs(), U)                                                            # :185-197
-        return U
+        kn = _known_ids(known, R.shape[0], self.nu, "fold_in: known must hold one trained user id in [0, {n}) or -1 per history ({m})")
+        return self._fold_in(True, R, kn)
 
-    def _fold_in_segs(self, Fu, prof_u, Ul):
-        """The segments of the one fold-in launch: Pi's S blocks -> Fu, prof_i -> prof_u, Il[l-1] -> Ul[l] (softmax on l = L)."""
-        segs = []
-        if self.has_feats:
-            segs += [(self.blk(self.Pi, s), self.blk(Fu, s), None, False) for s in range(self.S)]              # :153,156,162
-            segs.append((self.prof_i, prof_u, None, False))                                                     # :167
-        segs += [(self.Il[l - 1], Ul[l], None, l == self.L) for l in range(1, self.L + 1)]                    # :174,178
-        return segs
-
-    def _fold_in_items(self, items):
-        """Make Pi hold X.W^T + b on every item of `items` (sorted ids) before a fold-in.  The forward projects the live items only, and
-        Pi's edgeless rows are zero; a history given at call time may hold such an item.  Those rows are projected here with the
-        grouped kernels and a row map into Pi's edgeless rows, which no training launch reads (no ui column points there)."""
-        if self.live_i is None:
-            return
-        if getattr(self, "_edgeless", None) is None:
-            # once: the edgeless item ids and their rows of the item-side tables (the tables' own dtype), as _build_live_items does
-            dead = torch.nonzero(self._live_pos < 0).flatten()
-            f = self.feats
-            self._edgeless = (dead.cpu().numpy(), dead.to(torch.int32).contiguous(),
-                              dict(image=f["image"][dead].contiguous(), text=f["text"][dead].contiguous(),
-                                   item={k: v[dead].contiguous() for k, v in f["item"].items()}))
-        dead_np, dead, x = self._edgeless
-        if dead_np.size == 0 or not np.isin(items, dead_np, assume_unique=True).any():
-            return
-        p = self.p
-        probs = [(x["image"], p["image_trans.weight"], p["image_trans.bias"], self.blk(self.Pi, 0), dead),
-                 (x["text"], p["text_trans.weight"], p["text_trans.bias"], self.blk(self.Pi, 1), dead)]
-        probs += [(x["item"][k], p["item_trans.weight"], p["item_trans.bias"], self.blk(self.Pi, 2 + j), dead) for j, k in enumerate(self.keys)]
-        probs.sort(key=lambda t: -t[0].shape[1])
-        ops.proj_fwd_group(probs, self.d, self.cfg.proj_mode)
-
-    # ---- item fold-in: the item side of the forward for items added after training -------------------------------------------
     def fold_in_items(self, rowptr, col, known=None):
         """-> I_new [m x d]: the fused representation of m items whose interactions are the rows of an int CSR over trained user ids
         (rowptr[m+1], col; `graph.history_matrix` rejects ids outside [0, n_users) and collapses repeats).  known: optional int[m], the
@@ -433,38 +384,58 @@ class HotPath:
         tensor (Fi = iu.Fu, prof_i = iu.P_usr, Il[l] = [softmax] iu.Ul[l]), so with R^T the new rows and si their (deg + 1e-8)^-1/2 these
         are ONE SpMM launch with S + 1 + L segments, followed by the fusion of the m rows.  Layer 0 is E_i[known] for a trained item and
         a zero row for a new one.  The item's own side features enter no term of its row (they reach items only through two hops)."""
-        from .graph import history_matrix, inv_sqrt_degree
+        from .graph import history_matrix
         R = history_matrix(rowptr, col, self.nu, what="new items", unit="user id")
-        m, d, L, dev = R.shape[0], self.d, self.L, self.E_i.device
-        kn = _known_ids(known, m, self.ni, "fold_in_items: known must hold one trained item id in [0, {n}) or -1 per item ({m})")
+        kn = _known_ids(known, R.shape[0], self.ni, "fold_in_items: known must hold one trained item id in [0, {n}) or -1 per item ({m})")
+        return self._fold_in(False, R, kn)
+
+    def _fold_in(self, users, R, kn):
+        """The fold-in of m new rows of one side (users: R's rows are users over item ids, else items over user ids) with layer-0 ids
+        kn: the segments of the one launch are the other side's S blocks, its profile and its ID layers (softmax on l = L)."""
+        from .graph import inv_sqrt_degree
+        m, d, L, dev = R.shape[0], self.d, self.L, self.E_u.device
         if m == 0:
             return torch.empty(0, d, dtype=torch.float32, device=dev)
+        train_op, E = (self.ui, self.E_u) if users else (self.iu, self.E_i)
         t = lambda a, dt: torch.from_numpy(np.ascontiguousarray(a.astype(dt))).to(dev)
-        op = ops.CsrOperator(t(R.indptr, np.int32), t(R.indices, np.int32), m, self.nu, rs=t(inv_sqrt_degree(R), np.float32),
-                             tile_nnz=getattr(self.iu.plan, "tile_nnz", 0))       # pieces cut as the training operator cuts them
+        op = ops.CsrOperator(t(R.indptr, np.int32), t(R.indices, np.int32), m, R.shape[1], rs=t(inv_sqrt_degree(R), np.float32),
+                             tile_nnz=getattr(train_op.plan, "tile_nnz", 0))       # pieces cut as the training operator cuts them
         new = lambda *s: torch.empty(*s, dtype=torch.float32, device=dev)
-        Il = [new(m, d) for _ in range(L + 1)]
-        Fi, prof_i = (new(m, self.S * d), new(m, d)) if self.has_feats else (None, None)
+        layers = [new(m, d) for _ in range(L + 1)]
+        self._fold_in_sources(users, R)
+        segs, sides = [], []
         if self.has_feats:
-            self._fold_in_profiles()
-        op.apply(self._fold_in_items_segs(Fi, prof_i, Il))
-        ops.gather_rows(self.E_i, t(kn, np.int32), Il[0])                      # known -> E_i row, -1 -> zeros
-        si = [self.blk(Fi, 0), self.blk(Fi, 1), prof_i] + [self.blk(Fi, 2 + j) for j in range(len(self.keys))] if self.has_feats else []
-        I = new(m, d)
-        ops.fuse_fwd(Il, si, self._side_coefs(), I)                                                            # :185-197
-        return I
+            F, prof = new(m, self.S * d), new(m, d)
+            src_F, src_prof = (self.Pi, self.prof_i) if users else (self.Fu, self.P_usr)                   # :153-157,162-163,166-167
+            segs += [(self.blk(src_F, s), self.blk(F, s), None, False) for s in range(self.S)]
+            segs.append((src_prof, prof, None, False))
+            sides = self.sides.fused(F, prof)
+        src_layers = self.Il[:L] if users else self.Ul[1:]                                                    # :174-180
+        segs += [(src_layers[l - 1], layers[l], None, l == L) for l in range(1, L + 1)]
+        op.apply(segs)
+        ops.gather_rows(E, t(kn, np.int32), layers[0])                          # known -> E row, -1 -> zeros
+        out = new(m, d)
+        ops.fuse_fwd(layers, sides, self._side_coefs(), out)                                                                # :185-197
+        return out
 
-    def _fold_in_items_segs(self, Fi, prof_i, Il):
-        """The segments of the one item fold-in launch: Fu's S blocks -> Fi, P_usr -> prof_i, Ul[l] -> Il[l] (softmax on l = L)."""
-        segs = []
-        if self.has_feats:
-            segs += [(self.blk(self.Fu, s), self.blk(Fi, s), None, False) for s in range(self.S)]              # :154,157,163
-            segs.append((self.P_usr, prof_i, None, False))                                                      # :166
-        segs += [(self.Ul[l], Il[l], None, l == self.L) for l in range(1, self.L + 1)]                        # :175,180
-        return segs
-
-    def _fold_in_profiles(self):
-        """Make P_usr hold X_usr.W_u^T + b_u before an item fold-in.  The forward of this engine projects every user row, so it does."""
+    def _fold_in_sources(self, users, R):
+        """Bring what a fold-in reads up to date: Pi on the items of R (users), or P_usr (items).  This engine's forward projects
+        every user row, but the live items only, leaving Pi's edgeless rows zero, and a history given at call time may hold such an
+        item.  Those rows are projected here with the grouped kernels and a row map into Pi's edgeless rows, which no training launch
+        reads (no ui column points there)."""
+        if not users or self.live_i is None:
+            return
+        if getattr(self, "_edgeless", None) is None:
+            # once: the edgeless item ids and their rows of the item-side tables (the tables' own dtype), as _build_live_items does
+            dead = torch.nonzero(self._live_pos < 0).flatten()
+            f = self.feats
+            self._edgeless = (dead.cpu().numpy(), dead.to(torch.int32).contiguous(),
+                              dict(image=f["image"][dead].contiguous(), text=f["text"][dead].contiguous(),
+                                   item={k: v[dead].contiguous() for k, v in f["item"].items()}))
+        dead_np, dead, x = self._edgeless
+        if dead_np.size == 0 or not np.isin(np.unique(R.indices), dead_np, assume_unique=True).any():
+            return
+        ops.proj_fwd_group(self.sides.proj_problems(x, self.p, Pi=self.Pi, rows=dead), self.d, self.cfg.proj_mode)
 
     # ---- backward: expects gU, gI and (GFu, GFi, Gprof_u, Gprof_i, GP_usr_direct) filled ---------------
     def backward(self, gp_usr_direct=None, batch_rows=False):
@@ -478,11 +449,9 @@ class HotPath:
         exact zero to GFu / GFi / Gprof_*; `_grad_init(id_grads=True)` has zeroed dUl / dIl instead."""
         L = self.L
         coefs, su, si = self._fuse_args
+        dsu, dsi = [], []
         if self.has_feats:
-            dsu = [self.blk(self.GFu, 0), self.blk(self.GFu, 1), self.Gprof_u] + [self.blk(self.GFu, 2 + j) for j in range(len(self.keys))]
-            dsi = [self.blk(self.GFi, 0), self.blk(self.GFi, 1), self.Gprof_i] + [self.blk(self.GFi, 2 + j) for j in range(len(self.keys))]
-        else:
-            dsu, dsi = [], []
+            dsu, dsi = self.sides.fused(self.GFu, self.Gprof_u), self.sides.fused(self.GFi, self.Gprof_i)
         ku, ki = self._rows_kw(batch_rows)
         with self._t("fuse_bwd"):
             self._fork(lambda: ops.fuse_bwd(self.gU, L + 1, self.dUl, su, coefs, dsu, True, **ku))
@@ -532,16 +501,10 @@ class HotPath:
             g_cur_I = dst
 
     def _wgrad(self):
-        d, m = self.d, self.cfg.proj_mode
         if self.has_feats:
-            f, g = self.fx, self.grads
-            with self._t("proj_wgrad"):
-                rows = () if self.live_i is None else (self.live_i,)                                  # compact row r <-> GPi[live_i[r]]
-                probs = [(f["item"][k], self.blk(self.GPi, 2 + j), g["item_trans.weight"], g["item_trans.bias"], j > 0, *rows) for j, k in enumerate(self.keys)]
-                probs.append((f["user"], self.GP_usr, g["user_trans.weight"], g["user_trans.bias"], False))
-                probs.append((f["text"], self.blk(self.GPi, 1), g["text_trans.weight"], g["text_trans.bias"], False, *rows))
-                probs.append((f["image"], self.blk(self.GPi, 0), g["image_trans.weight"], g["image_trans.bias"], False, *rows))
-                ops.proj_wgrad_group(probs, d, m)
+            with self._t("proj_wgrad"):                                                  # compact row r <-> GPi[live_i[r]]
+                probs = self.sides.wgrad_problems(self.fx, self.grads, self.GPi, self.GP_usr, self.live_i)
+                ops.proj_wgrad_group(probs, self.d, self.cfg.proj_mode)
 
     # ---- losses + their gradients w.r.t. the forward outputs ---------------------------------------------
     def batch_capacity(self):
@@ -579,10 +542,7 @@ class HotPath:
         n_keep = int((1 - c.prune_loss_drop_rate) * B)                     # main.py:161-162 (double arithmetic)
         heads = [(self.U, self.I, self.gU, self.gI, 1.0, 1.0)]                                                        # main.py:232-235
         if self.has_feats:
-            heads.append((self.blk(self.Fu, 0), self.blk(self.Fi, 0), self.blk(self.GFu, 0), self.blk(self.GFi, 0), c.mm_mf_rate, 0.0))  # :238-241
-            heads.append((self.blk(self.Fu, 1), self.blk(self.Fi, 1), self.blk(self.GFu, 1), self.blk(self.GFi, 1), c.mm_mf_rate, 0.0))  # :242-246
-            for j in range(len(self.keys)):                                                                            # :248-254
-                heads.append((self.prof_u, self.blk(self.Fi, 2 + j), self.Gprof_u, self.blk(self.GFi, 2 + j), c.aug_mf_rate, 0.0))
+            heads += self.sides.heads(c, self.Fu, self.prof_u, self.GFu, self.Gprof_u, self.Fi, self.GFi)
         if not init_done:
             self._grad_init()
         with self._t("bpr"):
@@ -602,12 +562,11 @@ class HotPath:
         c = self.cfg
         regions = [(self.gU, None, 0.0), (self.gI, None, 0.0)]
         if self.has_feats:
-            creg = c.feat_reg_decay / self.ni
-            d2 = 2 * self.d
-            regions += [(self.GFu[:, :d2], self.Fu[:, :d2], creg), (self.GFi[:, :d2], self.Fi[:, :d2], creg),
+            creg, sd = c.feat_reg_decay / self.ni, self.sides
+            regions += [(sd.reg(self.GFu), sd.reg(self.Fu), creg), (sd.reg(self.GFi), sd.reg(self.Fi), creg),
                         (self.Gprof_u, None, 0.0), (self.Gprof_i, None, 0.0)]
-            if self.S > 2:
-                regions += [(self.GFu[:, d2:], None, 0.0), (self.GFi[:, d2:], None, 0.0)]
+            if self.keys:
+                regions += [(sd.unreg(self.GFu), None, 0.0), (sd.unreg(self.GFi), None, 0.0)]
         if id_grads:          # last: the loss's partial sums keep their slots, so its fixed-order reduction gives the same bits
             regions += [(self.dUl, None, 0.0), (self.dIl, None, 0.0)]
         with self._t("grad_init"):

@@ -45,17 +45,15 @@ class HoistedHotPath(HotPath):
 
     # ---- one-time precompute --------------------------------------------------------------------------------------
     def _build_tables(self, gs):
-        f, dev = self.feats, self.E_u.device
-        names = ["image", "text"] + ["item:" + k for k in self.keys] + ["user"]
-        raw = [f["image"], f["text"]] + [f["item"][k] for k in self.keys] + [f["user"]]
-        w_of = ["image_trans", "text_trans"] + ["item_trans"] * len(self.keys) + ["user_trans"]
+        dev, sd = self.E_u.device, self.sides
+        raw = sd.tables(self.feats)
         # the logical widths come from the weights (an int8 table's rows are wider: values, padding and the row scale)
-        widths = [int(self.p[w + ".weight"].shape[1]) for w in w_of]
+        widths = [int(self.p[w + ".weight"].shape[1]) for w in sd.weights]
         wide = lambda X, w: feat_int8.dequantize(X, w) if X.dtype == torch.int8 else X.float()
         self.col0 = [0]
         for w in widths:
             self.col0.append(self.col0[-1] + w)
-        self.names_s, self.widths = names, widths
+        self.widths = widths
         Kc = self.col0[-1] + 32                                   # + one 32-column pad block holding the scale columns
         self.Kc = Kc
         TU = torch.zeros(self.nu, Kc, dtype=torch.float32, device=dev)
@@ -74,14 +72,13 @@ class HoistedHotPath(HotPath):
         self.TU, self.TI, self.sc = TU, TI, sc
         # Gram matrices of the image / text tables over BOTH sides (feat_reg touches img_i, txt_i, img_u, txt_u): one-time fp64 products
         self.gram = []
-        for j in range(2):
+        for j in range(len(sd.reg_weights)):
             c0, w = self.col0[j], widths[j]
             A, Bm = TU[:, c0:c0 + w].double(), TI[:, c0:c0 + w].double()
             G = (A.t() @ A + Bm.t() @ Bm).float().contiguous()
             h = (A.t() @ TU[:, sc].double() + Bm.t() @ TI[:, sc].double()).float().contiguous()
             n2 = float((TU[:, sc].double() ** 2).sum() + (TI[:, sc].double() ** 2).sum())
             self.gram.append((G, h, n2))
-        self.w_names = ["image_trans", "text_trans"] + ["item_trans"] * len(self.keys) + ["user_trans"]
 
     def _tab(self, T, j):
         return T[:, self.col0[j]:self.col0[j] + self.widths[j]]
@@ -91,12 +88,11 @@ class HoistedHotPath(HotPath):
         d, m, p, S = self.d, self.cfg.proj_mode, self.p, self.S
         probs, r1 = [], []
         for j in range(S):
-            W = p[self.w_names[j] + ".weight"]
+            W, b = self.sides.param(p, j)
             probs.append((self._tab(self.TU, j), W, None, self.blk(self.Fu, j)))
             probs.append((self._tab(self.TI, j), W, None, self.blk(self.Fi, j)))
-            b = p[self.w_names[j] + ".bias"]
             r1 += [(self.blk(self.Fu, j), self.TU[:, self.sc], b), (self.blk(self.Fi, j), self.TI[:, self.sc], b)]
-        Wu, bu = p["user_trans.weight"], p["user_trans.bias"]
+        Wu, bu = self.sides.param(p, S)
         probs += [(self._tab(self.TU, S), Wu, None, self.prof_u), (self._tab(self.TI, S), Wu, None, self.prof_i)]
         r1 += [(self.prof_u, self.TU[:, self.sc + 1], bu), (self.prof_i, self.TI[:, self.sc + 1], bu)]
         probs.sort(key=lambda t: -t[0].shape[1])
@@ -107,22 +103,14 @@ class HoistedHotPath(HotPath):
         self._fuse_fwd()
         return self.U, self.I
 
-    def _fold_in_items(self, items):
-        """fold_in reads Pi = X.W^T + b, which this engine never materialises (its forward projects the propagated tables): one grouped
-        projection of the full item-side tables per call, into the engine's Pi, which no hoisted step reads."""
-        p, f = self.p, self.feats
-        probs = [(f["image"], p["image_trans.weight"], p["image_trans.bias"], self.blk(self.Pi, 0)),
-                 (f["text"], p["text_trans.weight"], p["text_trans.bias"], self.blk(self.Pi, 1))]
-        probs += [(f["item"][k], p["item_trans.weight"], p["item_trans.bias"], self.blk(self.Pi, 2 + j)) for j, k in enumerate(self.keys)]
-        probs.sort(key=lambda t: -t[0].shape[1])
+    def _fold_in_sources(self, users, R):
+        """fold_in reads Pi = X.W^T + b and fold_in_items P_usr = X_usr.W_u^T + b_u, which this engine never materialises (its forward
+        projects the propagated tables): one grouped projection per call, of the full item-side tables into the engine's Pi or of
+        the user table into its P_usr, which no hoisted step reads.  Fu, which fold_in_items also reads, is written by the forward
+        (TU.W^T + cu b^T)."""
+        sd, f, p = self.sides, self.feats, self.p
+        probs = sd.proj_problems(f, p, Pi=self.Pi) if users else sd.proj_problems(f, p, P_usr=self.P_usr)
         ops.proj_fwd_group(probs, self.d, self.cfg.proj_mode)
-
-    def _fold_in_profiles(self):
-        """fold_in_items reads P_usr = X_usr.W_u^T + b_u, which this engine never materialises (its prof_u / prof_i come from TU / TI):
-        one projection of the user table per call, into the engine's P_usr, which no hoisted step reads.  Its Fu, which fold_in_items
-        also reads, is written by the forward (TU.W^T + cu b^T)."""
-        p = self.p
-        ops.proj_fwd_group([(self.feats["user"], p["user_trans.weight"], p["user_trans.bias"], self.P_usr)], self.d, self.cfg.proj_mode)
 
     # ---- compact buffers of a training step ---------------------------------------------------------------------------
     def _ensure_compact(self, cap):
@@ -145,7 +133,7 @@ class HoistedHotPath(HotPath):
         pos and neg must be the two halves of ONE contiguous [2 x cap] block (engine index buffer rows 1-2, or a fresh cat)."""
         if self.opt is None:
             raise RuntimeError("attach an optimizer with set_optimizer() first")
-        cfg, d, S, L, p, m = self.cfg, self.d, self.S, self.L, self.p, self.cfg.proj_mode
+        cfg, d, S, L, p, m, sd = self.cfg, self.d, self.S, self.L, self.p, self.cfg.proj_mode, self.sides
         cap = int(users.numel())
         self.ensure_capacity(max(cap, self.batch_capacity()) if meta is None else cap)
         c = self._ensure_compact(cap)
@@ -154,11 +142,11 @@ class HoistedHotPath(HotPath):
         else:
             pn = c.setdefault("pn", torch.empty(2 * cap, dtype=torch.int32, device=users.device))
             pn[:cap].copy_(pos); pn[cap:].copy_(neg)
-        blk = lambda buf, s: buf[:, s * d:(s + 1) * d]
+        blk = self.blk
         tab = lambda X, j: X[:, self.col0[j]:self.col0[j] + self.widths[j]]
         g = self.grads
         creg = cfg.feat_reg_decay / self.ni
-        reg_names = ("image_trans", "text_trans")
+        reg_names = sd.reg_weights
         det = cfg.deterministic
         # deterministic steps: the compact blocks give every triplet rows of its own, so the heads' only shared destination is Gpu (the
         # attribute heads, folded in head order), and the scatters of dU / dI into the dense tables (a batch repeats users and items)
@@ -189,10 +177,10 @@ class HoistedHotPath(HotPath):
             ops.gather_rows(self.TI, pn, c["Xi"])
         probs, r1 = [], []
         for j in range(S):
-            W, b = p[self.w_names[j] + ".weight"], p[self.w_names[j] + ".bias"]
+            W, b = sd.param(p, j)
             probs += [(tab(c["Xu"], j), W, None, blk(c["Fu"], j)), (tab(c["Xi"], j), W, None, blk(c["Fi"], j))]
             r1 += [(blk(c["Fu"], j), c["Xu"][:, self.sc], b), (blk(c["Fi"], j), c["Xi"][:, self.sc], b)]
-        Wu, bu = p["user_trans.weight"], p["user_trans.bias"]
+        Wu, bu = sd.param(p, S)
         probs += [(tab(c["Xu"], S), Wu, None, c["pu"]), (tab(c["Xi"], S), Wu, None, c["pi"])]
         r1 += [(c["pu"], c["Xu"][:, self.sc + 1], bu), (c["pi"], c["Xi"][:, self.sc + 1], bu)]
         probs.sort(key=lambda t: -t[0].shape[1])
@@ -200,26 +188,19 @@ class HoistedHotPath(HotPath):
             ops.proj_fwd_group(probs, d, m)                                                   # Models.py:145-167 on the batch's rows
             ops.rank1_add(r1)
         self._join()
-        coefs = [cfg.model_cat_rate, cfg.model_cat_rate, cfg.user_cat_rate] + [cfg.item_cat_rate] * len(self.keys)
-        su = [blk(c["Fu"], 0), blk(c["Fu"], 1), c["pu"]] + [blk(c["Fu"], 2 + j) for j in range(len(self.keys))]
-        si = [blk(c["Fi"], 0), blk(c["Fi"], 1), c["pi"]] + [blk(c["Fi"], 2 + j) for j in range(len(self.keys))]
+        coefs, su, si = sd.coefs(cfg), sd.fused(c["Fu"], c["pu"]), sd.fused(c["Fi"], c["pi"])
         with self._t("fuse_fwd"):
             self._fork(lambda: ops.fuse_fwd(self.Ul, su, coefs, c["U"], rows=users, compact=True))   # :185-197 on the batch's rows
             ops.fuse_fwd(self.Il, si, coefs, c["I"], rows=pn, compact=True)
             self._join()
         # ---- losses + output gradients ----
-        heads = [(c["U"], c["I"], c["gU"], c["gI"], 1.0, 1.0),                                                         # main.py:232-235
-                 (blk(c["Fu"], 0), blk(c["Fi"], 0), blk(c["GFu"], 0), blk(c["GFi"], 0), cfg.mm_mf_rate, 0.0),        # :238-241
-                 (blk(c["Fu"], 1), blk(c["Fi"], 1), blk(c["GFu"], 1), blk(c["GFi"], 1), cfg.mm_mf_rate, 0.0)]        # :242-246
-        for j in range(len(self.keys)):                                                                               # :248-254
-            heads.append((c["pu"], blk(c["Fi"], 2 + j), c["Gpu"], blk(c["GFi"], 2 + j), cfg.aug_mf_rate, 0.0))
+        heads = [(c["U"], c["I"], c["gU"], c["gI"], 1.0, 1.0)] + sd.heads(cfg, c["Fu"], c["pu"], c["GFu"], c["Gpu"], c["Fi"], c["GFi"])
         n_keep = int((1 - cfg.prune_loss_drop_rate) * cap)
         with self._t("bpr"):
             ops.bpr_heads(heads, c["ar"], c["ar"], c["ar2"], n_keep, cfg.regs0 / cfg.batch_size, self.head_out, self.loss, self._bpr_work, meta=meta,
                           **({"ordered": self._slot_plan} if det else {}))
         # ---- backward: fusion on the compact rows, ID gradients scattered into the dense chain ----
-        dsu = [blk(c["GFu"], 0), blk(c["GFu"], 1), c["Gpu"]] + [blk(c["GFu"], 2 + j) for j in range(len(self.keys))]
-        dsi = [blk(c["GFi"], 0), blk(c["GFi"], 1), c["Gpi"]] + [blk(c["GFi"], 2 + j) for j in range(len(self.keys))]
+        dsu, dsi = sd.fused(c["GFu"], c["Gpu"]), sd.fused(c["GFi"], c["Gpi"])
 
         def user_side_bwd():
             ops.fuse_bwd(c["gU"], L + 1, c["dU"], su, coefs, dsu, True)
@@ -235,7 +216,7 @@ class HoistedHotPath(HotPath):
         wg, seen = [], set(reg_names)                             # image / text gradients already hold the feat_reg term
         bias_terms = {}
         for j in list(range(S)) + [S]:
-            name = self.w_names[j] if j < S else "user_trans"
+            name = sd.weights[j]
             dYu, dYi = (blk(c["GFu"], j), blk(c["GFi"], j)) if j < S else (c["Gpu"], c["Gpi"])
             scol = self.sc if j < S else self.sc + 1
             wg.append((tab(c["Xu"], j), dYu, g[name + ".weight"], None, name in seen)); seen.add(name)

@@ -279,9 +279,8 @@ class Trainer(object):
         if args.drop_rate > 0:
             # nn.Dropout in training mode on each projection, reference order image, text, user, item keys (Models.py:145-150); the mask of a
             # contiguous [n x d] tensor is drawn from the CUDA generator exactly as nn.Dropout would on the projection itself
-            d = hp.d
-            blocks = [hp.blk(hp.Pi, 0), hp.blk(hp.Pi, 1), hp.P_usr] + [hp.blk(hp.Pi, 2 + j) for j in range(len(hp.keys))]
-            drop = [torch.nn.functional.dropout(torch.ones(b.shape[0], d, device=self.device), p=args.drop_rate, training=True) for b in blocks]
+            blocks = hp.sides.fused(hp.Pi, hp.P_usr)
+            drop = [torch.nn.functional.dropout(torch.ones(b.shape[0], hp.d, device=self.device), p=args.drop_rate, training=True) for b in blocks]
             for b, mk in zip(blocks, drop):
                 b.mul_(mk)
         hp._prop_fwd()
@@ -302,14 +301,13 @@ class Trainer(object):
                 att = att + crit(dec_i[j], raw_i, alpha=args.alpha_l)
             (args.att_re_rate * att).backward()
             self.decoder.zero_grad(set_to_none=True)                      # de_optimizer is never stepped upstream
-            for j, k in enumerate(keys):
-                hp.blk(hp.GFi, 2 + j).index_add_(0, i_mask, leaf[k].grad)
+            for k, g in hp.side_views(grads=True)["att_i"].items():
+                g.index_add_(0, i_mask, leaf[k].grad)
             hp.loss.add_(args.att_re_rate * att.detach())
         hp._fuse_bwd()
         hp._chain_bwd()
         if drop is not None:                                              # backward of the dropout: the same masks on the projection gradients
-            gblocks = [hp.blk(hp.GPi, 0), hp.blk(hp.GPi, 1), hp.GP_usr] + [hp.blk(hp.GPi, 2 + j) for j in range(len(hp.keys))]
-            for b, mk in zip(gblocks, drop):
+            for b, mk in zip(hp.sides.fused(hp.GPi, hp.GP_usr), drop):
                 b.mul_(mk)
         hp._wgrad()
         hp.opt.step([hp.grads[k] for k in hp._opt_names])

@@ -4,6 +4,8 @@ from __future__ import annotations
 import json
 import os
 
+from .sides import SideLayout
+
 REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
@@ -34,8 +36,9 @@ def step_bytes(hp, nnz):
     if hp.has_feats:
         f, p = hp.feats, hp.p
         nl = getattr(hp, "n_live", ni)         # the item-side problems read the live items' rows only (engine.HotPath._build_live_items)
+        w = SideLayout(hp.keys, d).weights                   # the S item-side blocks, then the user profile
         k = lambda name: int(p[name + ".weight"].shape[1])      # logical widths from the weights (an int8 row also holds its scale)
-        gemms = [(nl, k("image_trans")), (nl, k("text_trans"))] + [(nl, k("item_trans"))] * len(f["item"]) + [(nu, k("user_trans"))]
+        gemms = [(nl, k(name)) for name in w[:-1]] + [(nu, k(w[-1]))]
         xb = f["image"].element_size()
         out["proj_fwd"] = out["proj_wgrad"] = sum(proj_bytes(n, k, d, xb) for n, k in gemms)
     sp = lambda M, N, segs: spmm_bytes(nnz, M, N, d, segs)
