@@ -408,7 +408,10 @@ int llmrec_host_sample_batch(uint32_t* py_key, int32_t* py_pos, uint32_t* np_key
 /* Device-side batch sampler (SURVEY.md 8f-1; utility/load_data.py:157-195 + main.py:216-224 on the GPU): ONE kernel fills the [4 x cap]
  * int32 index buffer of a training step -- rows users / pos / neg and the meta row {B', n_keep} looked up in meta_table[2*B' ..] -- from
  * DEVICE copies of exist_users, the train CSR (rows SORTED ascending) and the augmented-edge tables (ids < 0 or >= aug_limit are dropped,
- * as upstream's filter does; INT32_MIN = uid missing).  state = device uint64[2] {seed, step}; the kernel advances `step`, so the launch
+ * as upstream's filter does; INT32_MIN = uid missing, and a missing uid or one >= n_aug_table is dropped too, where upstream raises
+ * KeyError).  PRECONDITION, not checked here: every exist user has 1 <= deg < n_items (a train item to be the positive and an item left to
+ * be the negative) and every train row is sorted ascending; DeviceSampler checks both on the host.  The negative is never a train item.
+ * state = device uint64[2] {seed, step}; the kernel advances `step`, so the launch
  * can live inside a captured CUDA graph.  NOT bit-compatible with the reference's host RNG streams (that is llmrec_host_sample_batch, the
  * default): same distributions, counter-based generator.  key_scratch: uint32[max(n_exist, batch)]. */
 int llmrec_device_sample_batch(const int32_t* exist_users, int32_t n_exist, int32_t batch,

@@ -5,8 +5,12 @@
 // host_sampler.cu, the default); here a counter-based generator (splitmix64 over {seed, step, lane}) gives the same DISTRIBUTIONS:
 //   users   a uniformly random batch_size-subset of exist_users (the batch_size smallest of n_exist random keys, radix-selected),
 //           or batch_size independent draws when batch_size > n_exist (load_data.py:158-161)
-//   pos     uniform over the user's train items; neg: uniform over items, rejected while it is a train item of the user (:166-187)
-//   aug     n_aug = int(batch * rate) distinct batch positions; (u, aug_pos[u], aug_neg[u]) appended when both ids are in [0, aug_limit)
+//   pos     uniform over the user's train items; neg: uniform over items, rejected while it is a train item of the user (:166-187);
+//           after 2^16 rejected candidates the r-th non-member, r uniform in [0, n_items - deg), so neg is never a train item
+//   aug     n_aug = min(int(batch * rate), batch) distinct batch positions (the n_aug smallest of batch random keys, ties to the lower
+//           position); (u, aug_pos[u], aug_neg[u]) appended in position order when both ids are in [0, aug_limit).  A uid outside
+//           [0, n_aug_table) or with an INT32_MIN entry (missing from augmented_sample_dict) is DROPPED, where upstream raises KeyError
+// Precondition (checked on the host by DeviceSampler): every exist user has 1 <= deg < n_items and every train row is sorted ascending.
 // One CTA of 1024 threads (a batch is ~1e3 triplets); deterministic for a given {seed, step}; the step counter lives on the device.
 #include "common.cuh"
 
@@ -107,7 +111,7 @@ __global__ void __launch_bounds__(1024) device_sample_kernel(const SampleParams 
   __shared__ int hist[256];
   __shared__ int redi[32];
   __shared__ unsigned s_prefix;
-  __shared__ int s_want, s_kept;
+  __shared__ int s_want;
   const int tid = threadIdx.x;
   const unsigned long long seed = p.state[0], step = p.state[1];
   const unsigned long long base = splitmix64(seed ^ splitmix64(step));
@@ -131,12 +135,22 @@ __global__ void __launch_bounds__(1024) device_sample_kernel(const SampleParams 
     const int u = users[b];
     const int e0 = p.rowptr[u], deg = p.rowptr[u + 1] - e0;
     pos[b] = deg > 0 ? p.col[e0 + g.below(deg)] : 0;
-    int c = 0;
-    for (int tries = 0; tries < (1 << 16); ++tries) {
+    int c = 0; bool found = false;
+    for (int tries = 0; tries < (1 << 16) && !found; ++tries) {
       c = g.below(p.n_items);
       int lo = e0, hi = e0 + deg; bool hit = false;                   // train rows are sorted ascending
       while (lo < hi) { const int m = (lo + hi) >> 1; const int x = p.col[m]; if (x == c) { hit = true; break; } if (x < c) lo = m + 1; else hi = m; }
-      if (!hit) break;
+      found = !hit;
+    }
+    if (!found && deg < p.n_items) {
+      // 2^16 candidates were all train items (a user holding nearly every item): draw the r-th non-member directly, still uniform
+      // over the n_items - deg non-members.  Walk the sorted row: every distinct member at or below the running candidate pushes it up.
+      c = g.below(p.n_items - deg);
+      for (int j = e0; j < e0 + deg; ++j) {
+        const int x = p.col[j];
+        if (x > c) break;
+        if (j == e0 || x != p.col[j - 1]) ++c;
+      }
     }
     neg[b] = c;
   }
@@ -148,19 +162,19 @@ __global__ void __launch_bounds__(1024) device_sample_kernel(const SampleParams 
     unsigned T; int r;
     const int n_aug = p.n_aug < B ? p.n_aug : B;
     radix_select(key2, B, n_aug - 1, T, r, hist, &s_prefix, &s_want);
-    if (tid == 0) s_kept = 0;
+    // pass 1: the selection as radix_select defines it (key2 < T, or == T and among the first r ties in position order) writes
+    // keys[i] = 0 for a selected position whose table entries are valid, 0xffffffff otherwise; the users are already emitted, so the key
+    // scratch (>= batch entries) is free
+    for (int i = tid; i < B; i += blockDim.x) p.keys[i] = 0xffffffffu;
     __syncthreads();
-    // selected AND valid -> second ordered pass over the validity flag (a key of 0 selects, 0xffffffff rejects)
-    auto ok_key = [&](int i) {
-      const unsigned k = key2(i);
-      // tie handling of the selection is position-ordered; recompute "selected" cheaply: k < T, or k == T (rare: 32-bit keys) -> accept ties
-      const bool sel = k < T || k == T;
+    ordered_emit(key2, B, T, r, [&](int i, int) {
       const int u = users[i];
       const bool in = u >= 0 && u < p.n_aug_table;
       const int ap = in ? p.aug_pos[u] : -1, an = in ? p.aug_neg[u] : -1;
-      return (sel && ap >= 0 && an >= 0 && ap < p.aug_limit && an < p.aug_limit) ? 0u : 0xffffffffu;
-    };
-    kept = ordered_emit(ok_key, B, 1u, 0, [&](int i, int slot) {
+      if (ap >= 0 && an >= 0 && ap < p.aug_limit && an < p.aug_limit) p.keys[i] = 0u;
+    }, redi);
+    // pass 2: the flagged positions appended in position order
+    kept = ordered_emit([&](int i) { return p.keys[i]; }, B, 1u, 0, [&](int i, int slot) {
       if (B + slot < p.cap) { const int u = users[i]; users[B + slot] = u; pos[B + slot] = p.aug_pos[u]; neg[B + slot] = p.aug_neg[u]; }
     }, redi);
     if (B + kept > p.cap) kept = p.cap - B;

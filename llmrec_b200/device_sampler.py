@@ -15,6 +15,9 @@ from . import ops
 
 class DeviceSampler:
     def __init__(self, exist_users, train_rowptr, train_col_sorted, n_items, batch_size, aug_pos, aug_neg, aug_limit, aug_rate, device, seed=0):
+        """Raises what the host sampler raises when an exist user has no train item or no possible negative, and ValueError when a train
+        row is not sorted ascending: the kernel assumes all three (its binary search and its negative draw)."""
+        check_device_sampler_inputs(exist_users, train_rowptr, train_col_sorted, n_items)
         dev = torch.device(device)
         t = lambda a: torch.from_numpy(np.ascontiguousarray(a, dtype=np.int32)).to(dev)
         self.exist, self.rowptr, self.col = t(exist_users), t(train_rowptr), t(train_col_sorted)
@@ -35,6 +38,26 @@ class DeviceSampler:
             self.aug_pos.numel() if self.n_aug else 0, self.aug_limit, C.c_void_p(meta_table.data_ptr()), cap, C.c_void_p(self.state.data_ptr()),
             C.c_void_p(index_buffer.data_ptr()), C.c_void_p(self.keys.data_ptr()), C.c_void_p(torch.cuda.current_stream().cuda_stream)), "device_sample_batch")
         ops._count()
+
+
+def check_device_sampler_inputs(exist_users, train_rowptr, train_col_sorted, n_items):
+    """The precondition of llmrec_device_sample_batch: every exist user has 1 <= deg < n_items, and every train row is sorted ascending."""
+    rowptr = np.asarray(train_rowptr, dtype=np.int64)
+    col = np.asarray(train_col_sorted)
+    exist = np.asarray(exist_users, dtype=np.int64)
+    deg = rowptr[exist + 1] - rowptr[exist]
+    if (deg <= 0).any():
+        raise_sampler_error(2)
+    if (deg >= int(n_items)).any():
+        raise_sampler_error(3)
+    down = np.flatnonzero(col[1:] < col[:-1]) + 1                     # positions whose item is below the one before it
+    starts = np.zeros(len(col) + 1, dtype=bool)
+    starts[rowptr[:-1][rowptr[:-1] < len(col)]] = True
+    if (~starts[down]).any():
+        j = int(down[~starts[down]][0])
+        u = int(np.searchsorted(rowptr, j, side="right") - 1)
+        raise ValueError(f"device sampler: train row {u} is not sorted ascending (items {int(col[j - 1])}, {int(col[j])}); "
+                         "the kernel's binary search needs sorted rows")
 
 
 STATE_ELEMS = 1252                      # LLMREC_REF_SAMPLER_STATE_ELEMS: random key[624], pos, numpy key[624], pos, error, pad
