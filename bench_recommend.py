@@ -2,8 +2,9 @@
 neighbours) on one H100.
 
     python bench_recommend.py [--reps 3] [--syn_users 131072] [--syn_histories 8192] [--syn_items 65536] [--syn_scale 1.0]
+                              [--pairs 1048576] [--legs rerank,score_pairs]
 
-Five legs per workload, each timed end to end on the host clock between device synchronises (median of --reps calls after one
+Seven legs per workload, each timed end to end on the host clock between device synchronises (median of --reps calls after one
 warm-up call):
   known         trained users scored from U with their training items excluded (exclude="train"), K = 10; users/s
   fold_in       held-out histories folded in (HotPath.fold_in) and scored, exclude="train", K = 10; users/s
@@ -11,7 +12,13 @@ warm-up call):
                 users/s
   fold_in_items trained items' user lists folded in as new items (HotPath.fold_in_items, no ID embedding); items/s
   similar       item-to-item neighbours (recommend.similar_items) of trained items over the trained catalog, K = 10; queries/s
-Every call includes the full eval forward a recommendation starts with.
+  rerank        every user (synthetic: --syn_users users) re-ranks --rerank_c random candidates (netflix 100, synthetic 200), K = 10,
+                nothing excluded (Trainer.rerank / recommend.rerank); queries/s and candidates/s
+  score_pairs   --pairs random (trained user, trained item) pairs scored (Trainer.score / recommend.score_pairs); pairs/s
+Every call includes the full eval forward a recommendation starts with.  The rerank and score_pairs legs also time their kernel alone
+(llmrec_rerank_f32 / llmrec_score_pairs_f32 between CUDA events, median of 5 windows of 20 launches) and report it as GB/s of gathered
+rows: 4*d bytes per candidate row plus 4 per id (pairs: two rows and two ids), against the size of I (L2-resident at netflix,
+HBM-resident at the synthetic shape).
 Workloads: the netflix shape of bench.py (Trainer with side features, held-out histories = a user's training row plus its test items;
 every item's user list and every item as a query), and the 10M x 1M x 200M synthetic of dist_bench (ID-only single-GPU engine,
 d = 128, L = 2; histories = a training row plus two random items, folded in as unknown users; the known and candidates legs score the
@@ -49,11 +56,73 @@ def _timed(fn, reps):
     return sorted(ts)[len(ts) // 2], min(ts), max(ts)
 
 
+ONLY = set()               # --legs: the legs to run (empty: all)
+
+
 def _leg(name, n_users, fn, reps, unit="users"):
+    if ONLY and name not in ONLY:
+        return None
     med, lo, hi = _timed(fn, reps)
     out = {unit: n_users, "s_per_call": round(med, 5), "s_min": round(lo, 5), "s_max": round(hi, 5), unit + "_per_s": round(n_users / med, 1)}
     sys.stderr.write(f"  {name:13s} {n_users:9d} {unit:7s}  {med * 1e3:9.2f} ms/call  {n_users / med:12.0f} {unit}/s\n")
     return out
+
+
+def _kernel(fn, reps=20, windows=5):
+    """median seconds per launch of `fn` between CUDA events"""
+    import torch
+    fn()
+    torch.cuda.synchronize()
+    ts = []
+    for _ in range(windows):
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record()
+        for _ in range(reps):
+            fn()
+        e1.record()
+        torch.cuda.synchronize()
+        ts.append(e0.elapsed_time(e1) / 1e3 / reps)
+    return sorted(ts)[len(ts) // 2]
+
+
+def _serving_legs(U, I, e2e_rerank, e2e_pairs, n_q, c, n_pairs, reps, seed=0):
+    """The rerank and score_pairs legs: end to end (`e2e_*`, given the candidates / pairs) and the kernel alone on U / I"""
+    import torch
+    from llmrec_b200 import ops
+    dev, d = U.device, int(U.shape[1])
+    g = torch.Generator(device=dev).manual_seed(seed)
+    cand = torch.randint(0, I.shape[0], (n_q, c), device=dev, generator=g, dtype=torch.int32)
+    qrow = torch.arange(n_q, dtype=torch.int32, device=dev)
+    rp = torch.arange(n_q + 1, dtype=torch.int32, device=dev) * c
+    col = cand.reshape(-1).contiguous()
+    pu = torch.randint(0, U.shape[0], (n_pairs,), device=dev, generator=g, dtype=torch.int32)
+    pi = torch.randint(0, I.shape[0], (n_pairs,), device=dev, generator=g, dtype=torch.int32)
+    i_mb = I.shape[0] * d * 4 / 1e6
+    if ONLY and "rerank" not in ONLY and "score_pairs" not in ONLY:
+        return {}
+    rr = _leg("rerank", n_q, lambda: e2e_rerank(cand), reps, unit="queries")
+    if rr is None:
+        return {"score_pairs": _pairs_legs(U, I, e2e_pairs, pu, pi, reps)}
+    rr["candidates_per_s"] = round(n_q * c / rr["s_per_call"], 1)
+    k = _kernel(lambda: ops.rerank(U, I, qrow, rp, col, None, None, 10))
+    rr.update(candidates_per_query=c, kernel_s=round(k, 7), kernel_queries_per_s=round(n_q / k, 1),
+              kernel_candidates_per_s=round(n_q * c / k, 1), kernel_GB_per_s=round(n_q * c * (4 * d + 4) / k / 1e9, 1), I_MB=round(i_mb, 1))
+    sys.stderr.write(f"  {'rerank kernel':13s} {n_q:9d} queries  {k * 1e3:9.3f} ms       {n_q * c / k:12.0f} cand/s  "
+                     f"{rr['kernel_GB_per_s']:7.1f} GB/s (I: {i_mb:.1f} MB)\n")
+    return {"rerank": rr, "score_pairs": _pairs_legs(U, I, e2e_pairs, pu, pi, reps)}
+
+
+def _pairs_legs(U, I, e2e_pairs, pu, pi, reps):
+    from llmrec_b200 import ops
+    n_pairs, d = int(pu.numel()), int(U.shape[1])
+    sp_ = _leg("score_pairs", n_pairs, lambda: e2e_pairs(pu, pi), reps, unit="pairs")
+    if sp_ is None:
+        return None
+    k = _kernel(lambda: ops.score_pairs(U, I, pu, pi))
+    sp_.update(kernel_s=round(k, 7), kernel_pairs_per_s=round(n_pairs / k, 1), kernel_GB_per_s=round(n_pairs * (8 * d + 8) / k / 1e9, 1))
+    sys.stderr.write(f"  {'pairs kernel':13s} {n_pairs:9d} pairs    {k * 1e3:9.3f} ms       {n_pairs / k:12.0f} pairs/s "
+                     f"{sp_['kernel_GB_per_s']:7.1f} GB/s\n")
+    return sp_
 
 
 def netflix(a, tmp):
@@ -74,6 +143,8 @@ def netflix(a, tmp):
     irp, icol = tr.graph.rowptr_i.cpu().numpy(), tr.graph.col_i.cpu().numpy()
     res["fold_in_items"] = _leg("fold_in_items", ni, lambda: tr.fold_in_items((irp, icol)), a.reps, unit="items")
     res["similar"] = _leg("similar", ni, lambda: tr.similar_items(np.arange(ni), K=10), a.reps, unit="queries")
+    hp = tr._current_model()
+    res.update(_serving_legs(hp.U, hp.I, lambda cand: tr.rerank(cand, K=10), lambda u, i: tr.score(u, i), nu, 100, a.pairs, a.reps))
     del tr, gen
     return res
 
@@ -131,11 +202,21 @@ def synthetic(a, tmp):
         hp.forward()
         recommend.similar_items(hp, items, K=10, mode=a.score_mode)
 
+    def rr(cand):
+        hp.forward()
+        recommend.rerank(hp, g.rowptr_u, g.col_u, cand, users=users, K=10)
+
+    def pairs(u, i):
+        hp.forward()
+        recommend.score_pairs(hp, u, i)
+
     res = {"workload": f"synthetic {nu}x{ni}, {g.nnz} training edges, d={d}, L={L}, ID-only engine",
            "known": _leg("known", n, known, a.reps), "fold_in": _leg("fold_in", len(hist), fold, a.reps),
            "candidates": _leg("candidates", n, cand, a.reps),
            "fold_in_items": _leg("fold_in_items", items.size, fold_items, a.reps, unit="items"),
            "similar": _leg("similar", items.size, similar, a.reps, unit="queries")}
+    hp.forward()
+    res.update(_serving_legs(hp.U, hp.I, rr, pairs, n, 200, a.pairs, a.reps))
     del hp, g, params
     torch.cuda.empty_cache()
     return res
@@ -149,13 +230,16 @@ def main():
     ap.add_argument("--syn_histories", type=int, default=8192, help="synthetic workload: histories of the fold-in leg")
     ap.add_argument("--syn_items", type=int, default=65536, help="synthetic workload: items of the fold_in_items and similar legs")
     ap.add_argument("--syn_scale", type=float, default=1.0, help="size factor of the 10M x 1M x 200M synthetic graph")
+    ap.add_argument("--pairs", type=int, default=1 << 20, help="pairs of the score_pairs legs")
     ap.add_argument("--workloads", default="netflix,synthetic")
+    ap.add_argument("--legs", default="", help="comma-separated subset of the legs to run (default: all)")
     a = ap.parse_args()
     import torch
     from llmrec_b200 import ops
     if not torch.cuda.is_available():
         raise SystemExit("bench_recommend.py needs a CUDA (H100) device")
     a.score_mode = ops.SCORE_MODE.get(a.proj_mode, 0)
+    ONLY.update(x for x in a.legs.split(",") if x)
     name, limit = card()
     result = {"metric": "recommend_users_per_sec", "gpu": name, "power_limit": limit, "proj_mode": a.proj_mode, "K": 10,
               "timing": f"host clock between device synchronises, median of {a.reps} calls after one warm-up; each call runs the full eval forward",

@@ -380,6 +380,29 @@ int llmrec_user_auc_f32(const float* U, int64_t ldu, const float* I, int64_t ldi
                         const int32_t* mask_rowptr, const int32_t* mask_col, const int32_t* truth_rowptr, const int32_t* truth_col,
                         float* out_auc, llmrec_stream_t stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * Scores of given pairs and re-ranking of given candidate lists (no full-catalog pass).  One score is
+ * the sequential fp32 FMA chain a = 0; for j in 0..d-1: a = fmaf(U[u][j], I[i][j], a) -- the order of
+ * both llmrec_score_topk_f32 modes' returned scores, so the same (u, i) gets the same bits.  Any d >= 1,
+ * any leading dimensions.  Exact fp32 on the SIMT cores: each candidate row is read once per query.
+ *
+ * score_pairs: out[p] = <U[qrow[p]], I[item[p]]> for p < n (a negative id gives NaN; ids are otherwise
+ *   rows of U / I).  out fp32[n].
+ * rerank: query r (< m) scores every candidate cand_col[cand_rowptr[r] .. cand_rowptr[r+1]) against
+ *   U[qrow[r]], drops ids outside [0, n_catalog) (-1 = padding), drops ids of mask row qrow[r] (mask_rowptr
+ *   NULL: no mask; rows SORTED ASCENDING, as for score_topk), keeps one copy of a repeated id and writes the K
+ *   best by (score desc, id asc) to out_idx int32 [m x K] / out_val fp32 [m x K].  A NaN score ranks after
+ *   every number; a real candidate, even at -inf or NaN, ranks before padding; fewer than K survivors are
+ *   padded with -1 / -inf.  K is 1..LLMREC_RERANK_MAX_K (the selection width); rows may be any length
+ *   (a long row is streamed with a running top-K in shared memory).  No scratch, no host sync.
+ * --------------------------------------------------------------------------------------------- */
+#define LLMREC_RERANK_MAX_K 1024
+int llmrec_score_pairs_f32(const float* U, int64_t ldu, const float* I, int64_t ldi, const int32_t* qrow, const int32_t* item,
+                           int32_t n, int32_t d, float* out, llmrec_stream_t stream);
+int llmrec_rerank_f32(const float* U, int64_t ldu, const float* I, int64_t ldi, const int32_t* qrow, int32_t m,
+                      const int32_t* cand_rowptr, const int32_t* cand_col, const int32_t* mask_rowptr, const int32_t* mask_col,
+                      int32_t n_catalog, int32_t d, int32_t K, int32_t* out_idx, float* out_val, llmrec_stream_t stream);
+
 /* Host-side (CPU, no GPU needed) BPR item sampler, bit-identical to Data.sample()'s numpy draws
  * (utility/load_data.py:166-187): hand over numpy's legacy MT19937 state (np.random.get_state()), get the
  * positives / rejection-sampled negatives for `users` and the advanced state back.  All pointers HOST. */

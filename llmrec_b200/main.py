@@ -532,6 +532,33 @@ class Trainer(object):
         mode = ops.SCORE_MODE.get(getattr(self.args, "proj_mode", "3xtf32"), 0)
         return recommend.similar_items(hot, items, K=K, new_items=Rn, mode=mode)
 
+    def score(self, users, items, new_items=None):
+        """-> fp32 [n] on the device: the model's score <U[users[p]], I[items[p]]> of each (user, item) pair, by the exact fp32 chain of the
+        scores `recommend` returns (the same pair gets the same bits; --proj_mode does not change them).  users: trained ids; items:
+        trained ids, or n_items + j for the j-th of `new_items` (user lists of items added after training, folded in as for `recommend`).
+        Equal lengths; ids are checked before anything runs."""
+        Rn = recommend.new_items_csr(new_items, self.n_users)
+        u, i = recommend.check_pairs(users, items, self.n_users, self.n_items + (0 if Rn is None else Rn.shape[0]))
+        return recommend.score_pairs(self._current_model(), u, i, new_items=Rn)
+
+    def rerank(self, candidates, users=None, K=None, exclude="none", histories=None, new_items=None):
+        """-> (ids int64 [m x K], scores fp32 [m x K]) on the device: each query's candidate list ordered by this model, the K best by
+        (score desc, id asc), padded with -1 / -inf.  candidates: a sequence of item-id lists, a (rowptr, col) pair, or a 2-D integer
+        tensor / ndarray [m x C] (the `candidate_indices` layout; -1 = padding); ids in [0, n_items + len(new_items)).  Queries as in
+        `recommend`: trained users (default every user, when there is one candidate row per user) or `histories` folded in, `users` then
+        naming each history's trained id (or -1).  Repeated ids are kept once.  exclude: "none" (default: a given shortlist is not thinned)
+        or "train" (drops what `recommend` masks).  K: 1..1024, None = the longest surviving row.  Scores are exact fp32 in every
+        --proj_mode, bit-identical to `recommend`'s for the same (user, item)."""
+        job = recommend.prepare_rerank(self.hot, self.graph.rowptr_u, self.graph.col_u, candidates, users=users, K=K, exclude=exclude,
+                                       histories=histories, new_items=new_items)
+        return recommend.run_rerank(self._current_model(), job)
+
+    def write_rerank(self, path, candidates, K):
+        """--rerank_out: every user's candidate row (`candidate_indices` layout [n_users x C]) re-ranked by this model, nothing excluded,
+        top K, pickled as a CPU int64 tensor [n_users x K] to `path` (atomically, as `write_candidates`)."""
+        ids, _ = self.rerank(candidates, K=K)
+        return recommend.write_candidates(path, ids)
+
     def write_candidates(self, path, K=10):
         """--candidates_out: the top-K of every user over the whole catalog, nothing excluded (torch.topk(U . I^T, k=K) of the reference's
         stage 1), pickled as a CPU int64 tensor [n_users x K] to `path` (atomically)."""
@@ -625,11 +652,31 @@ def main(argv=None):
     trainer = Trainer(data_config=config, data_generator=gen)         # --resume loads here, after set_seed and the model's own draws
     if args.candidates_out and trainer.masked_mode:
         raise ValueError("--candidates_out needs a fixed model: not with --mask / --mask_rate > 0 / --drop_rate > 0")
+    rerank_in, rerank_k = check_rerank_flags(args, trainer)
     ret = trainer.evaluate() if args.eval_only else trainer.train()
     if args.candidates_out:                                           # from the model in memory when the run ends
         trainer.write_candidates(args.candidates_out, args.candidates_k)
         trainer.logger.logging("candidates: top-%d of %d users written to %s" % (args.candidates_k, trainer.n_users, args.candidates_out))
+    if rerank_in is not None:
+        trainer.write_rerank(args.rerank_out, rerank_in, rerank_k)
+        trainer.logger.logging("rerank: %d users' candidates from %s, top-%d written to %s" % (trainer.n_users, args.rerank_in, rerank_k,
+                                                                                              args.rerank_out))
     return ret
+
+
+def check_rerank_flags(args, trainer):
+    """--rerank_in / --rerank_out / --rerank_k, checked before the first training step -> (the candidate array, K), or (None, None)."""
+    if not args.rerank_in and not args.rerank_out:
+        return None, None
+    if not (args.rerank_in and args.rerank_out):
+        raise ValueError("--rerank_in and --rerank_out go together: the candidate file to re-rank and the file to write")
+    if trainer.masked_mode:
+        raise ValueError("--rerank_in needs a fixed model: not with --mask / --mask_rate > 0 / --drop_rate > 0")
+    recommend.check_engine(trainer.hot)
+    cand = recommend.read_candidates(args.rerank_in, trainer.n_users, trainer.n_items)
+    K = int(cand.shape[1]) if args.rerank_k is None else args.rerank_k
+    recommend.check_rerank_k(K)
+    return cand, K
 
 
 if __name__ == "__main__":

@@ -572,6 +572,36 @@ def score_topk(U, I, users, mask_rowptr, mask_col, K, mode=0, want_vals=False):
     return (idx, val) if want_vals else idx
 
 
+RERANK_MAX_K = 1024        # LLMREC_RERANK_MAX_K: the selection width of llmrec_rerank_f32
+
+
+def score_pairs(U, I, qrow, item):
+    """fp32[n]: <U[qrow[p]], I[item[p]]> as one sequential fp32 FMA chain (the bits score_topk returns for the same pair)."""
+    _mat(U); _mat(I)
+    n = int(qrow.numel())
+    if int(item.numel()) != n:
+        raise ValueError(f"score_pairs: {n} query rows but {int(item.numel())} items")
+    out = torch.empty(n, dtype=torch.float32, device=U.device)
+    N.check(N.lib().llmrec_score_pairs_f32(_p(U), _ld(U), _p(I), _ld(I), _p(_i32(qrow)), _p(_i32(item)), n, int(I.shape[1]), _p(out),
+                                            _stream()), "score_pairs")
+    _count()
+    return out
+
+
+def rerank(U, I, qrow, cand_rowptr, cand_col, mask_rowptr, mask_col, K):
+    """(ids int32 [m x K], scores fp32 [m x K]): per query row r, the K best of its candidate row (CSR) scored against U[qrow[r]] by
+    (score desc, id asc); ids outside [0, I.shape[0]) and ids of mask row qrow[r] dropped, repeats kept once, padded with -1 / -inf."""
+    _mat(U); _mat(I)
+    m = int(qrow.numel())
+    idx = torch.empty((m, K), dtype=torch.int32, device=U.device)
+    val = torch.empty((m, K), dtype=torch.float32, device=U.device)
+    N.check(N.lib().llmrec_rerank_f32(_p(U), _ld(U), _p(I), _ld(I), _p(_i32(qrow)), m, _p(_i32(cand_rowptr)), _p(_i32(cand_col)),
+                                       _p(mask_rowptr), _p(mask_col), int(I.shape[0]), int(I.shape[1]), int(K), _p(idx), _p(val),
+                                       _stream()), "rerank")
+    _count()
+    return idx, val
+
+
 def topk_hits(idx, users, truth_rowptr, truth_col):
     hits = torch.empty(idx.shape, dtype=torch.uint8, device=idx.device)
     N.check(N.lib().llmrec_topk_hits(_p(_i32(idx)), idx.shape[0], idx.shape[1], _p(_i32(users)), _p(_i32(truth_rowptr)), _p(_i32(truth_col)),

@@ -7,6 +7,10 @@ the lowest item id, K <= 64; a row with fewer than K candidates is padded with i
 `engine.HotPath.fold_in`, new items (lists of the trained users who interacted with each) through `engine.HotPath.fold_in_items`; new
 item j gets catalog id n_items + j.  The host side only builds CSRs (the mask rows, the folded-in histories and item lists) and the
 output file.
+
+Scores of given (user, item) pairs are `ops.score_pairs` (llmrec_score_pairs_f32) and re-ranking of given candidate lists is
+`ops.rerank` (llmrec_rerank_f32, K <= 1024): the same sequential fp32 chain as score_topk's returned scores, so the bits agree, and the
+same mask rows (`exclusion_mask`) for exclude="train".
 """
 from __future__ import annotations
 
@@ -18,6 +22,7 @@ import scipy.sparse as sp
 import torch
 
 from . import ops
+from .engine import _known_ids
 from .graph import histories_csr, history_matrix
 
 MAX_K = 64                 # the selection of llmrec_score_topk_f32
@@ -102,6 +107,49 @@ def append_rows(a_rowptr, a_col, b_rowptr, b_col, offset):
     return rp.to(torch.int32), col
 
 
+def _queries(engine, train_rowptr, train_col, users, histories):
+    """The query rows of `top_k` / `rerank`, checked, before anything is folded in -> (R, rows int [m], own_rowptr, own_col, known):
+    trained users are rows `users` of U (default every user) with their training rows (R and known None); histories (R, their CSR) will
+    be rows 0..m-1 of their fold-in, with their own items, `users` naming each one's trained id or -1 (known)."""
+    dev = engine.E_u.device
+    if histories is None:
+        u = np.arange(engine.nu) if users is None else np.asarray(users, dtype=np.int64).reshape(-1)
+        if u.size and (u.min() < 0 or u.max() >= engine.nu):
+            raise ValueError(f"users: trained user ids are in [0, {engine.nu})")
+        return None, u, train_rowptr, train_col, None
+    R = histories_csr(histories, engine.ni)
+    m = R.shape[0]
+    kn = _known_ids(users, m, engine.nu, "fold_in: known must hold one trained user id in [0, {n}) or -1 per history ({m})")
+    return R, np.arange(m), _i32(R.indptr, dev), _i32(R.indices, dev), kn
+
+
+def _query_rows(engine, R, known):
+    """U for trained users (R None), else the fold-in of the histories R (HotPath.fold_in)"""
+    return engine.U if R is None else engine.fold_in(R.indptr, R.indices, known=known)
+
+
+def exclusion_mask(engine, rowptr, col, exclude, Rn=None, known=None):
+    """The mask rows (int32 device CSR, rows sorted) of exclude="train": each query's own row of (rowptr, col) -- a trained user's
+    training row, indexed by user id, or a history's own items -- followed by every new item n_items + j of Rn whose list names that user
+    (for a history: the list names its trained id `known`; -1 names none).  exclude="none": empty rows."""
+    dev = col.device
+    if exclude == "none":
+        return torch.zeros(rowptr.numel(), dtype=torch.int32, device=dev), col[:0]          # no row read
+    if Rn is not None and Rn.nnz:
+        Rt = sp.csr_matrix(Rn.T)                                              # row u: the new items whose list names trained user u
+        Rt.sort_indices()
+        nrp, ncol = _i32(Rt.indptr, dev), _i32(Rt.indices, dev)
+        if known is not None:                                                 # a history's row: that of its trained id, or none
+            nrp, ncol = select_rows(nrp, ncol, torch.from_numpy(known))
+        rowptr, col = append_rows(rowptr, col, nrp, ncol, engine.ni)
+    return rowptr, col
+
+
+def check_exclude(exclude):
+    if exclude not in EXCLUDE:
+        raise ValueError(f"exclude = {exclude!r}: one of {EXCLUDE}")
+
+
 def top_k(engine, train_rowptr, train_col, users=None, K=10, exclude="train", histories=None, mode=0, new_items=None):
     """Top-K of a model whose last full `forward()` is current (U, I and the item side).
     users: trained user ids (default every user), scored from U's rows; with `histories` they name the trained id of each history (or
@@ -115,31 +163,12 @@ def top_k(engine, train_rowptr, train_col, users=None, K=10, exclude="train", hi
     check_engine(engine)
     Rn = new_items_csr(new_items, engine.nu)
     K = check_k(K, engine.ni + (0 if Rn is None else Rn.shape[0]))
-    if exclude not in EXCLUDE:
-        raise ValueError(f"exclude = {exclude!r}: one of {EXCLUDE}")
-    dev = engine.E_u.device
-    if histories is None:
-        u = np.arange(engine.nu) if users is None else np.asarray(users, dtype=np.int64).reshape(-1)
-        if u.size and (u.min() < 0 or u.max() >= engine.nu):
-            raise ValueError(f"users: trained user ids are in [0, {engine.nu})")
-        U, rows, rp, col = engine.U, u, train_rowptr, train_col
-    else:
-        R = histories_csr(histories, engine.ni)
-        m = R.shape[0]
-        U = engine.fold_in(R.indptr, R.indices, known=users)                 # checks `users`
-        rows, rp, col = np.arange(m), _i32(R.indptr, dev), _i32(R.indices, dev)
+    check_exclude(exclude)
+    R, rows, rp, col, kn = _queries(engine, train_rowptr, train_col, users, histories)
+    U = _query_rows(engine, R, kn)
     I = _catalog(engine, Rn)
-    if exclude == "none":
-        rp, col = torch.zeros(rp.numel(), dtype=torch.int32, device=dev), col[:0]      # no row read
-    elif Rn is not None and Rn.nnz:
-        Rt = sp.csr_matrix(Rn.T)                                              # row u: the new items whose list names trained user u
-        Rt.sort_indices()
-        nrp, ncol = _i32(Rt.indptr, dev), _i32(Rt.indices, dev)
-        if histories is not None:                                             # a history's row: that of its trained id, or none
-            kn = np.full(m, -1) if users is None else (users.detach().cpu().numpy() if hasattr(users, "detach") else np.asarray(users))
-            nrp, ncol = select_rows(nrp, ncol, torch.from_numpy(kn.astype(np.int64).reshape(-1)))
-        rp, col = append_rows(rp, col, nrp, ncol, engine.ni)
-    return _score(U, I, _i32(rows, dev), rp, col, K, mode)
+    rp, col = exclusion_mask(engine, rp, col, exclude, Rn, kn)
+    return _score(U, I, _i32(rows, engine.E_u.device), rp, col, K, mode)
 
 
 def similar_items(engine, items, K=10, new_items=None, mode=0):
@@ -159,6 +188,175 @@ def similar_items(engine, items, K=10, new_items=None, mode=0):
     X = ops.row_normalize(_catalog(engine, Rn))
     eye_rp, eye_col = torch.arange(n + 1, dtype=torch.int32, device=dev), torch.arange(n, dtype=torch.int32, device=dev)
     return _score(X, X, _i32(q, dev), eye_rp, eye_col, K, mode)
+
+
+def _ids(a, what):
+    """An integer id array (list, ndarray or tensor on any device) -> int64 CPU tensor, flattened; anything else raises ValueError."""
+    t = a.detach().cpu() if torch.is_tensor(a) else torch.from_numpy(np.asarray(a))
+    if t.numel() == 0:
+        return t.reshape(-1).to(torch.int64)
+    if t.dtype == torch.bool or t.dtype.is_floating_point or t.dtype.is_complex:
+        raise ValueError(f"{what}: ids must be integers, got {t.dtype}")
+    return t.reshape(-1).to(torch.int64)
+
+
+def _check_range(ids, lo, n, what, unit):
+    if ids.numel() and (int(ids.min()) < lo or int(ids.max()) >= n):
+        bad = int(ids[(ids < lo) | (ids >= n)][0])
+        raise ValueError(f"{what}: {unit} {bad} is outside [{max(lo, 0)}, {n})" + (" (-1 = padding)" if lo < 0 else ""))
+
+
+def candidates_csr(candidates, n_catalog):
+    """A caller's candidate lists -> (rowptr int64 CPU tensor [m+1], col int64 CPU tensor [nnz]), ids checked against [0, n_catalog)
+    with -1 allowed as padding.  Three forms: a 2-D integer tensor / ndarray [m x C] (the `candidate_indices` layout, row r = query r's
+    candidates), a (rowptr, col) pair (a tuple of two arrays / tensors), or a sequence of id lists, one per query."""
+    if isinstance(candidates, tuple) and len(candidates) == 2 and all(hasattr(a, "shape") for a in candidates):
+        rp, col = _ids(candidates[0], "candidates rowptr"), _ids(candidates[1], "candidates")
+        if rp.numel() < 1 or int(rp[0]) != 0 or bool((rp[1:] < rp[:-1]).any()) or int(rp[-1]) != col.numel():
+            raise ValueError(f"candidates: rowptr must start at 0, never decrease and end at len(col) = {col.numel()}")
+    elif hasattr(candidates, "shape"):
+        if len(candidates.shape) != 2:
+            raise ValueError(f"candidates: a tensor / ndarray of candidates is 2-D [queries x C], got shape {tuple(candidates.shape)}")
+        m, c = (int(x) for x in candidates.shape)
+        col = _ids(candidates, "candidates")
+        rp = torch.arange(m + 1, dtype=torch.int64) * c
+    else:
+        rows = [_ids(list(r) if not hasattr(r, "shape") else r, "candidates") for r in candidates]
+        rp = torch.zeros(len(rows) + 1, dtype=torch.int64)
+        rp[1:] = torch.cumsum(torch.tensor([r.numel() for r in rows], dtype=torch.int64), 0)
+        col = torch.cat(rows) if rows else torch.zeros(0, dtype=torch.int64)
+    _check_range(col, -1, n_catalog, "candidates", "item id")
+    return rp, col
+
+
+def check_rerank_k(K):
+    if K is not None and (isinstance(K, bool) or not isinstance(K, (int, np.integer)) or not 1 <= int(K) <= ops.RERANK_MAX_K):
+        raise ValueError(f"K = {K!r}: re-ranking takes K in 1..{ops.RERANK_MAX_K} (the re-ranking kernel's selection width), or None")
+    return None if K is None else int(K)
+
+
+CAND_BLOCK = 1 << 30       # candidates per rerank launch at most (the kernel's CSR is int32)
+
+
+def _blocks(rp, limit):
+    """Query blocks [s, e) of a CSR's rows (int64 CPU rowptr) holding at most `limit` candidates each (at least one row)."""
+    m, s = rp.numel() - 1, 0
+    while s < m:
+        e = int(torch.searchsorted(rp, rp[s] + limit, right=True)) - 1
+        e = min(max(e, s + 1), m)
+        if int(rp[e] - rp[s]) >= 2 ** 31:
+            raise ValueError(f"candidates: row {s} holds {int(rp[e] - rp[s])} candidates (at most 2^31 - 1 per row)")
+        yield s, e
+        s = e
+
+
+def _survivors(rp, col, qrow, mrp, mcol, n):
+    """The longest row of distinct candidates left after padding and the mask (the K of K=None), on the device."""
+    dev = mcol.device
+    m = rp.numel() - 1
+    col = col.to(dev)
+    r = torch.repeat_interleave(torch.arange(m, device=dev), (rp[1:] - rp[:-1]).to(dev))
+    keep = col >= 0
+    keys = torch.unique(r[keep] * n + col[keep])
+    if mcol.numel():
+        q_rp, q_col = select_rows(mrp, mcol, qrow)
+        q_rp = q_rp.long()
+        mr = torch.repeat_interleave(torch.arange(m, device=dev), q_rp[1:] - q_rp[:-1])
+        keys = keys[~torch.isin(keys, mr * n + q_col.long())]
+    return int(torch.bincount(keys // n, minlength=1).max()) if keys.numel() else 0
+
+
+def prepare_rerank(engine, train_rowptr, train_col, candidates, users=None, K=None, exclude="none", histories=None, new_items=None):
+    """Every check of `rerank`, and its host-side inputs, before anything is launched: -> a dict for `run_rerank`."""
+    check_engine(engine)
+    Rn = new_items_csr(new_items, engine.nu)
+    n = engine.ni + (0 if Rn is None else Rn.shape[0])
+    K = check_rerank_k(K)
+    check_exclude(exclude)
+    rp, col = candidates_csr(candidates, n)
+    m = rp.numel() - 1
+    if histories is None and users is None and m != engine.nu:
+        raise ValueError(f"candidates: {m} rows; without `users` (or `histories`) there is one row per trained user ({engine.nu})")
+    R, rows, mrp, mcol, kn = _queries(engine, train_rowptr, train_col, users, histories)
+    if len(rows) != m:
+        raise ValueError(f"candidates: {m} rows for {len(rows)} " + ("users" if R is None else "histories"))
+    qrow = _i32(rows, engine.E_u.device)
+    mrp, mcol = exclusion_mask(engine, mrp, mcol, exclude, Rn, kn)
+    if K is None:
+        K = _survivors(rp, col, qrow, mrp, mcol, n)
+        if K > ops.RERANK_MAX_K:
+            raise ValueError(f"K = None: the longest candidate row keeps {K} ids, more than {ops.RERANK_MAX_K}; give K")
+        K = max(K, 1)
+    return dict(R=R, known=kn, Rn=Rn, rowptr=rp, col=col, qrow=qrow, mask_rowptr=mrp, mask_col=mcol, K=K)
+
+
+def run_rerank(engine, job):
+    """The launches of `rerank` for a `prepare_rerank` job: fold-ins, then one re-ranking launch per query block."""
+    U = _query_rows(engine, job["R"], job["known"])
+    I = _catalog(engine, job["Rn"])
+    rp, col, qrow, K = job["rowptr"], job["col"], job["qrow"], job["K"]
+    dev = qrow.device
+    m = qrow.numel()
+    ids = torch.empty((m, K), dtype=torch.int64, device=dev)
+    vals = torch.empty((m, K), dtype=torch.float32, device=dev)
+    for s, e in _blocks(rp, CAND_BLOCK):
+        brp = (rp[s:e + 1] - rp[s]).to(torch.int32).to(dev)
+        bcol = col[int(rp[s]):int(rp[e])].to(torch.int32).to(dev)
+        idx, v = ops.rerank(U, I, qrow[s:e], brp, bcol, job["mask_rowptr"], job["mask_col"], K)
+        ids[s:e].copy_(idx)
+        vals[s:e].copy_(v)
+    return ids, vals
+
+
+def rerank(engine, train_rowptr, train_col, candidates, users=None, K=None, exclude="none", histories=None, new_items=None):
+    """Re-rank given candidate lists with a model whose last full `forward()` is current: query r's candidates (`candidates_csr` forms)
+    scored against its user row by the exact fp32 chain of score_topk's returned scores, the K best by (score desc, id asc).
+    users / histories / new_items / exclude as in `top_k` (exclude="train" masks exactly what `top_k` masks); queries are trained users
+    (default: every user, when there are n_users candidate rows) or folded-in histories, one per candidate row.  Padding (-1), masked ids
+    and repeats are dropped; a NaN score ranks after every number, a real candidate before padding.  K: 1..1024, or None for the longest
+    surviving row.  -> (ids int64 [m x K], scores fp32 [m x K]) on the engine's device, padded with -1 / -inf."""
+    return run_rerank(engine, prepare_rerank(engine, train_rowptr, train_col, candidates, users, K, exclude, histories, new_items))
+
+
+def check_pairs(users, items, n_users, n_catalog):
+    """(users, items) of `score_pairs` -> int64 CPU tensors, checked: equal lengths, integers, trained users, catalog items."""
+    u, i = _ids(users, "users"), _ids(items, "items")
+    if u.numel() != i.numel():
+        raise ValueError(f"score: {u.numel()} users but {i.numel()} items (one pair per position)")
+    _check_range(u, 0, n_users, "users", "user id")
+    _check_range(i, 0, n_catalog, "items", "item id")
+    return u, i
+
+
+def score_pairs(engine, users, items, new_items=None):
+    """Scores of (user, item) pairs with a model whose last full `forward()` is current: <U[users[p]], I[items[p]]> by the exact fp32
+    chain of score_topk's returned scores.  users: trained ids; items: trained ids or n_items + j for the j-th of `new_items` (folded in as
+    in `top_k`).  -> fp32 [n] on the engine's device."""
+    check_engine(engine)
+    Rn = new_items_csr(new_items, engine.nu)
+    n_cat = engine.ni + (0 if Rn is None else Rn.shape[0])
+    u, i = check_pairs(users, items, engine.nu, n_cat)
+    dev = engine.E_u.device
+    I = _catalog(engine, Rn)
+    out = torch.empty(u.numel(), dtype=torch.float32, device=dev)
+    for s in range(0, u.numel(), CAND_BLOCK):
+        out[s:s + CAND_BLOCK] = ops.score_pairs(engine.U, I, _i32(u[s:s + CAND_BLOCK], dev), _i32(i[s:s + CAND_BLOCK], dev))
+    return out
+
+
+def read_candidates(path, n_users, n_catalog):
+    """A `candidate_indices` file (pickle of a 2-D integer tensor or ndarray [n_users x C], row u = user u's candidates, -1 = padding)
+    -> that array, checked: the file loads, is 2-D with n_users rows and holds item ids in [0, n_catalog) or -1."""
+    try:
+        with open(os.fspath(path), "rb") as f:
+            cand = pickle.load(f)
+    except Exception as e:                                                  # noqa: BLE001 -- any unreadable file is a flag error
+        raise ValueError(f"--rerank_in {path}: cannot read a pickled candidate array ({type(e).__name__}: {e})") from e
+    if not hasattr(cand, "shape") or len(cand.shape) != 2 or int(cand.shape[0]) != n_users:
+        raise ValueError(f"--rerank_in {path}: need a 2-D integer tensor / ndarray [n_users = {n_users} x C], got "
+                         f"{type(cand).__name__} {tuple(getattr(cand, 'shape', ()))}")
+    _check_range(_ids(cand, f"--rerank_in {path}"), -1, n_catalog, f"--rerank_in {path}", "item id")
+    return cand
 
 
 def write_candidates(path, ids):

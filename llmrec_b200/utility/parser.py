@@ -98,6 +98,13 @@ _EXTRA = [
                                                "items over the whole catalog, nothing excluded, as the pickled CPU int64 tensor [n_users x K] "
                                                "the augmentation stage reads (data/<dataset>/candidate_indices). Not with the mask / dropout branch")),
     ("candidates_k", dict(type=int, default=10, help="list length of --candidates_out (1..64, at most n_items)")),
+    ("rerank_in", dict(default=None, help="when the run ends, re-rank a candidate file with this model: a pickled 2-D integer tensor or "
+                                          "ndarray [n_users x C], row u = user u's candidates, -1 = padding (the --candidates_out / "
+                                          "candidate_indices format, so a file made by another model can be reordered by this one). "
+                                          "Needs --rerank_out. Not with the mask / dropout branch")),
+    ("rerank_out", dict(default=None, help="where --rerank_in's rows go, re-ranked by (score desc, id asc), nothing excluded, repeats kept "
+                                           "once: the pickled CPU int64 tensor [n_users x --rerank_k], padded with -1, written atomically")),
+    ("rerank_k", dict(type=int, default=None, help="list length of --rerank_out (1..1024; default: the width C of --rerank_in)")),
 ]
 
 DATASET_ALIASES = {"netflix": "netflix_valid_item", "movielens": "preprocessed_raw_MovieLens", "movieLens": "preprocessed_raw_MovieLens"}
