@@ -225,6 +225,7 @@ struct FwdUnit {
   using Cfg = ProjCfg<D, SPLIT, MB, BF16>;
   static_assert(!I8 || BF16, "int8 X runs the bf16 pipeline");
   static constexpr int kTransA = 0;   // bf16: A = the X tile as it arrived, K-major
+  struct BuildState {};               // no B to build: W arrives by TMA
   static constexpr int kBuilders = I8 ? 3 : 0;   // warps that write stage operands in the kernel: the int8 converters; W arrives by TMA
   // setmaxnreg: 128 * 40 + 256 * 232 = 384 * 168; the int8 converters hold a group's raw words in flight: 128 * 72 + 256 * 216
   static constexpr int kProducerRegs = I8 ? 72 : 40, kConsumerRegs = I8 ? 216 : 232;
@@ -302,8 +303,11 @@ struct WgUnit {
   // int8 X: warps 1..3 expand the raw X stage instead (I8Stage).
   static constexpr bool kBuildsB = SPLIT && !BF16;
   static constexpr int kBuilders = kBuildsB || I8 ? 3 : 0;
-  static constexpr int kProducerRegs = kBuilders ? 72 : 40;     // 128 * 72 + 256 * 216 = 384 * 168: the builders' loads in flight
-  static constexpr int kConsumerRegs = kBuilders ? 216 : 232;
+  // kAhead (d <= 64, below): the builders hold two stages' first batches, 128 * 120 + 256 * 192 = 384 * 168 (the consumers' d/2
+  // accumulators per m64 block fit); otherwise 128 * 72 + 256 * 216: the builders' loads in flight
+  static constexpr bool kAhead = kBuildsB && D <= 64;
+  static constexpr int kProducerRegs = kAhead ? 120 : kBuilders ? 72 : 40;
+  static constexpr int kConsumerRegs = kAhead ? 192 : kBuilders ? 216 : 232;
   static constexpr uint32_t kRawTx = I8 ? Cfg::TM * 64u : 0u;   // raw q bytes per stage, on the stage's own raw barrier
   static constexpr uint32_t kTx = kBuildsB ? Cfg::kX : I8 ? Cfg::kStage - Cfg::kX : Cfg::kStage;   // TMA bytes per stage on `full`
   __device__ void issue(uint8_t* st, uint64_t* bar, uint64_t* raw_bar, int kb, uint64_t pol) const {
@@ -335,35 +339,80 @@ struct WgUnit {
   // stage row l, so it reads its dY row through the row map once; a task is 8 columns (32 bytes of the row, two 16-byte loads),
   // the warps take every kBuilders-th task.  Each store of a warp writes one column c: chunk (l/4 ^ c) % 8, word l%4 -- 32
   // distinct banks, no conflict.  Rows at or past n are zeros, as TMA fills them.
+  // The builder is latency-bound on its row map -> dY -> store chain, so the chain is software-pipelined across the stages of a unit
+  // (BuildState), and no L2 load waits for the stage slot (`wait`).  kAhead (d <= 64, one batch is the whole stage): while stage kb
+  // is stored, stage kb + 1's dY loads and stage kb + 2's row-map entries are in flight.  Wider stages: stage kb + 1's row-map
+  // entries are loaded while stage kb is built, and stage kb's first batch of dY loads is issued before the wait.
   static constexpr int kTasks = D / 8;
   static constexpr int kBatch = 3;                   // tasks per thread whose loads are in flight together (24 floats)
-  __device__ void build(uint8_t* st, int kb, int bw, int lane) const {
-    const int n = P.prob[p].n, r = r0 + kb * kBk + lane;
+  static_assert(kTasks >= kBuilders, "every builder warp has tasks in its first batch");
+  static_assert(!kAhead || kTasks <= kBuilders * kBatch, "kAhead keeps a whole stage in one batch");
+  struct BuildState {
+    int row, next;                 // this lane's dY row of the current and of the next stage (-1 past n or past the unit)
+    float4 v[kBatch][2];           // the current stage's first batch (kAhead: loaded during the previous stage)
+  };
+  __device__ int dy_row(int kb, int lane) const {
+    if (kb >= kb_n) return -1;
+    const int r = r0 + kb * kBk + lane;
     const int* __restrict__ map = P.rows[p];
-    const float* src = r < n ? P.dY[p] + (long long)(map ? __ldg(map + r) : r) * P.lddy[p] : nullptr;
+    return r < P.prob[p].n ? (map ? __ldg(map + r) : r) : -1;
+  }
+  __device__ void load_batch(float4 (&v)[kBatch][2], int row, int t0) const {
+    const float* src = row >= 0 ? P.dY[p] + (long long)row * P.lddy[p] : nullptr;
+#pragma unroll
+    for (int j = 0; j < kBatch; ++j) {
+      const int t = t0 + kBuilders * j;
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+        v[j][h] = t < kTasks && src ? __ldg(reinterpret_cast<const float4*>(src + 8 * t + 4 * h)) : make_float4(0.f, 0.f, 0.f, 0.f);
+    }
+  }
+  __device__ void store_batch(uint8_t* st, const float4 (&v)[kBatch][2], int t0, int lane) const {
     uint8_t* b = st + Cfg::kX + (lane & 3) * 4;
     const int q = lane >> 2;
-    for (int t0 = bw; t0 < kTasks; t0 += kBuilders * kBatch) {
-      float4 v[kBatch][2];
 #pragma unroll
-      for (int j = 0; j < kBatch; ++j) {
-        const int t = t0 + kBuilders * j;
+    for (int j = 0; j < kBatch; ++j) {
+      const int t = t0 + kBuilders * j;
+      if (t >= kTasks) break;
 #pragma unroll
-        for (int h = 0; h < 2; ++h)
-          v[j][h] = t < kTasks && src ? __ldg(reinterpret_cast<const float4*>(src + 8 * t + 4 * h)) : make_float4(0.f, 0.f, 0.f, 0.f);
+      for (int e = 0; e < 8; ++e) {
+        const float4 w = v[j][e >> 2];
+        const float x = (e & 3) == 0 ? w.x : (e & 3) == 1 ? w.y : (e & 3) == 2 ? w.z : w.w, hi = tf32_hi(x);
+        uint8_t* o = b + (8 * t + e) * 128 + ((q ^ e) & 7) * 16;
+        *reinterpret_cast<float*>(o) = hi;
+        *reinterpret_cast<float*>(o + Cfg::kB) = x - hi;
       }
+    }
+  }
+  // the unit's first stage: its row and first batch, and the second stage's row
+  __device__ void build_begin(BuildState& bs, int bw, int lane) const {
+    bs.row = dy_row(0, lane);
+    if constexpr (kAhead) {
+      load_batch(bs.v, bs.row, bw);
+      bs.next = dy_row(1, lane);
+    }
+  }
+  template <class Wait>
+  __device__ void build(uint8_t* st, int kb, int bw, int lane, BuildState& bs, Wait wait) const {
+    if constexpr (kAhead) {   // one batch is the whole stage
+      float4 nv[kBatch][2];
+      load_batch(nv, bs.next, bw);                   // stage kb + 1's (zeros past the unit: never stored)
+      const int after = dy_row(kb + 2, lane);
+      wait();
+      store_batch(st, bs.v, bw, lane);
 #pragma unroll
-      for (int j = 0; j < kBatch; ++j) {
-        const int t = t0 + kBuilders * j;
-        if (t >= kTasks) break;
-#pragma unroll
-        for (int e = 0; e < 8; ++e) {
-          const float4 w = v[j][e >> 2];
-          const float x = (e & 3) == 0 ? w.x : (e & 3) == 1 ? w.y : (e & 3) == 2 ? w.z : w.w, hi = tf32_hi(x);
-          uint8_t* o = b + (8 * t + e) * 128 + ((q ^ e) & 7) * 16;
-          *reinterpret_cast<float*>(o) = hi;
-          *reinterpret_cast<float*>(o + Cfg::kB) = x - hi;
+      for (int j = 0; j < kBatch; ++j) { bs.v[j][0] = nv[j][0]; bs.v[j][1] = nv[j][1]; }
+      bs.next = after;
+    } else {
+      const int row = bs.row;
+      for (int t0 = bw; t0 < kTasks; t0 += kBuilders * kBatch) {
+        float4 v[kBatch][2];
+        load_batch(v, row, t0);
+        if (t0 == bw) {
+          bs.row = dy_row(kb + 1, lane);
+          wait();
         }
+        store_batch(st, v, t0, lane);
       }
     }
   }
@@ -427,6 +476,8 @@ __device__ __forceinline__ void proj_pipeline(const Params& P, int total) {
         for (int u = blockIdx.x; u < total; u += gridDim.x) {
           const Unit w(P, u);
           [[maybe_unused]] I8Stage<Unit> cv;
+          [[maybe_unused]] typename Unit::BuildState bs;
+          if constexpr (Unit::kRawTx == 0) w.build_begin(bs, warp - 1, lane);
           if constexpr (Unit::kRawTx > 0 && Unit::kScalesPerUnit) {
             converters_sync();            // every converter is done with the previous unit's scales
             w.tile_scales(tile_sc, tid - 32);
@@ -440,8 +491,7 @@ __device__ __forceinline__ void proj_pipeline(const Params& P, int total) {
               mbar_wait(&raw[s], ph);
               cv.expand(smem + s * Cfg::kStage, tid - 32);
             } else {
-              mbar_wait(&empty[s], ph ^ 1u);
-              w.build(smem + s * Cfg::kStage, kb, warp - 1, lane);
+              w.build(smem + s * Cfg::kStage, kb, warp - 1, lane, bs, [&] { mbar_wait(&empty[s], ph ^ 1u); });
             }
             fence_proxy_async_smem();   // the generic-proxy stores -> visible to wgmma
             __syncwarp();
