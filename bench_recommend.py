@@ -4,7 +4,7 @@ neighbours) on one H100.
     python bench_recommend.py [--reps 3] [--syn_users 131072] [--syn_histories 8192] [--syn_items 65536] [--syn_scale 1.0]
                               [--pairs 1048576] [--legs rerank,score_pairs]
 
-Seven legs per workload, each timed end to end on the host clock between device synchronises (median of --reps calls after one
+Eight legs per workload, each timed end to end on the host clock between device synchronises (median of --reps calls after one
 warm-up call):
   known         trained users scored from U with their training items excluded (exclude="train"), K = 10; users/s
   fold_in       held-out histories folded in (HotPath.fold_in) and scored, exclude="train", K = 10; users/s
@@ -15,6 +15,10 @@ warm-up call):
   rerank        every user (synthetic: --syn_users users) re-ranks --rerank_c random candidates (netflix 100, synthetic 200), K = 10,
                 nothing excluded (Trainer.rerank / recommend.rerank); queries/s and candidates/s
   score_pairs   --pairs random (trained user, trained item) pairs scored (Trainer.score / recommend.score_pairs); pairs/s
+  among         the known leg over a catalog of 1 %, 10 % and 100 % of the items (recommend.top_k(among=...)); users/s.  Each size also
+                times its kernel alone (llmrec_score_topk_among_f32, all users in one launch, between CUDA events), the plain call
+                (llmrec_score_topk_f32 over the whole catalog) and, where the [users x |among|] candidate CSR fits in int32, the same
+                question answered by llmrec_rerank_f32 with the set as every user's list
 Every call includes the full eval forward a recommendation starts with.  The rerank and score_pairs legs also time their kernel alone
 (llmrec_rerank_f32 / llmrec_score_pairs_f32 between CUDA events, median of 5 windows of 20 launches) and report it as GB/s of gathered
 rows: 4*d bytes per candidate row plus 4 per id (pairs: two rows and two ids), against the size of I (L2-resident at netflix,
@@ -59,12 +63,12 @@ def _timed(fn, reps):
 ONLY = set()               # --legs: the legs to run (empty: all)
 
 
-def _leg(name, n_users, fn, reps, unit="users"):
+def _leg(name, n_users, fn, reps, unit="users", label=None):
     if ONLY and name not in ONLY:
         return None
     med, lo, hi = _timed(fn, reps)
     out = {unit: n_users, "s_per_call": round(med, 5), "s_min": round(lo, 5), "s_max": round(hi, 5), unit + "_per_s": round(n_users / med, 1)}
-    sys.stderr.write(f"  {name:13s} {n_users:9d} {unit:7s}  {med * 1e3:9.2f} ms/call  {n_users / med:12.0f} {unit}/s\n")
+    sys.stderr.write(f"  {label or name:13s} {n_users:9d} {unit:7s}  {med * 1e3:9.2f} ms/call  {n_users / med:12.0f} {unit}/s\n")
     return out
 
 
@@ -125,6 +129,39 @@ def _pairs_legs(U, I, e2e_pairs, pu, pi, reps):
     return sp_
 
 
+def _among_legs(U, I, mask_rowptr, mask_col, e2e, n_q, mode, reps, seed=0):
+    """The among leg at 1 %, 10 % and 100 % of the catalog: end to end (`e2e(ids)`), and the kernels alone for the same users"""
+    import torch
+    from llmrec_b200 import ops
+    if ONLY and "among" not in ONLY:
+        return None
+    dev, ni = U.device, int(I.shape[0])
+    g = torch.Generator(device=dev).manual_seed(seed)
+    users = torch.arange(n_q, dtype=torch.int32, device=dev)
+    out = {}
+    for frac in (0.01, 0.1, 1.0):
+        n = max(10, int(round(frac * ni)))
+        S = torch.sort(torch.randperm(ni, device=dev, generator=g)[:n])[0].to(torch.int32)
+        leg = _leg("among", n_q, lambda: e2e(S), reps, label=f"among {frac:.0%}")
+        k = _kernel(lambda: ops.score_topk_among(U, I, users, S, mask_rowptr, mask_col, 10, mode=mode), reps=3, windows=3)
+        leg.update(n_among=n, kernel_s=round(k, 7), kernel_users_per_s=round(n_q / k, 1))
+        line = f"  {'kernel':13s} {n:9d} among    {k * 1e3:9.3f} ms"
+        if frac == 1.0:
+            kp = _kernel(lambda: ops.score_topk(U, I, users, mask_rowptr, mask_col, 10, mode=mode), reps=3, windows=3)
+            leg["plain_kernel_s"] = round(kp, 7)
+            line += f"   plain call {kp * 1e3:9.3f} ms"
+        if n_q * n < 2 ** 31:
+            rp = torch.arange(n_q + 1, dtype=torch.int64, device=dev).mul_(n).to(torch.int32)
+            col = S.repeat(n_q)
+            kr = _kernel(lambda: ops.rerank(U, I, users, rp, col, mask_rowptr, mask_col, 10), reps=3, windows=3)
+            leg["rerank_kernel_s"] = round(kr, 7)
+            line += f"   rerank {kr * 1e3:9.3f} ms"
+            del rp, col
+        sys.stderr.write(line + "\n")
+        out[f"{frac:.0%}"] = leg
+    return out
+
+
 def netflix(a, tmp):
     import numpy as np
     tr, gen, args = bench.make_trainer("netflix", types.SimpleNamespace(proj_mode=a.proj_mode, host_sampler="native", graph=1))
@@ -145,6 +182,8 @@ def netflix(a, tmp):
     res["similar"] = _leg("similar", ni, lambda: tr.similar_items(np.arange(ni), K=10), a.reps, unit="queries")
     hp = tr._current_model()
     res.update(_serving_legs(hp.U, hp.I, lambda cand: tr.rerank(cand, K=10), lambda u, i: tr.score(u, i), nu, 100, a.pairs, a.reps))
+    res["among"] = _among_legs(hp.U, hp.I, tr.graph.rowptr_u, tr.graph.col_u, lambda S: tr.recommend(K=10, exclude="train", among=S), nu,
+                               a.score_mode, a.reps)
     del tr, gen
     return res
 
@@ -217,6 +256,13 @@ def synthetic(a, tmp):
            "similar": _leg("similar", items.size, similar, a.reps, unit="queries")}
     hp.forward()
     res.update(_serving_legs(hp.U, hp.I, rr, pairs, n, 200, a.pairs, a.reps))
+
+    def among(S):
+        hp.forward()
+        recommend.top_k(hp, g.rowptr_u, g.col_u, users=users, K=10, exclude="train", mode=a.score_mode, among=S)
+
+    hp.forward()
+    res["among"] = _among_legs(hp.U, hp.I, g.rowptr_u, g.col_u, among, n, a.score_mode, a.reps)
     del hp, g, params
     torch.cuda.empty_cache()
     return res

@@ -368,6 +368,20 @@ int llmrec_score_topk_f32(const float* U, int64_t ldu, const float* I, int64_t l
                           float* scratch, int64_t scratch_elems, llmrec_stream_t stream);
 int64_t llmrec_score_topk_scratch(int32_t n_batch, int32_t n_items, int32_t d, int32_t K, int32_t mode);
 
+/* Top-K over a catalog given by ids: llmrec_score_topk_f32 with the catalog replaced by the rows
+ * among[0 .. n_among) of I.  among int32 STRICTLY ASCENDING, every id a row of I (not checked on the
+ * device).  Mask rows and out_idx hold GLOBAL item ids (rows of I); a masked id outside `among` is
+ * ignored.  Ties -> lowest global id; fewer than K survivors padded with -1 / -inf.  K is 1..64 and
+ * <= n_among.  Same modes and the same returned score bits as llmrec_score_topk_f32: mode 0 gathers
+ * the hi/lo copies of the n_among rows into the scratch, mode 2 scores a [b x n_among] block.  Called
+ * with among = 0..n_items-1 it returns what llmrec_score_topk_f32 returns. */
+int llmrec_score_topk_among_f32(const float* U, int64_t ldu, const float* I, int64_t ldi,
+                                const int32_t* users, int32_t n_batch, const int32_t* among, int32_t n_among, int32_t d,
+                                const int32_t* mask_rowptr, const int32_t* mask_col,
+                                int32_t K, int32_t* out_idx, float* out_val, int32_t mode,
+                                float* scratch, int64_t scratch_elems, llmrec_stream_t stream);
+int64_t llmrec_score_topk_among_scratch(int32_t n_batch, int32_t n_among, int32_t d, int32_t K, int32_t mode);
+
 /* hits[b,j] = 1 if out_idx[b,j] in truth row of users[b] (test_set membership, batch_test.py:30-34). */
 int llmrec_topk_hits(const int32_t* idx, int32_t n_batch, int32_t K, const int32_t* users,
                      const int32_t* truth_rowptr, const int32_t* truth_col, uint8_t* hits,

@@ -11,14 +11,14 @@ int proj_wgrad_simt(const float*, int64_t, const float*, int64_t, float*, float*
 int proj_wgrad_simt(const uint16_t*, int64_t, const float*, int64_t, float*, float*, int64_t, int, int, int, const int*, int64_t, cudaStream_t);
 int proj_fwd_simt(const int8_t*, int64_t, const float*, const float*, float*, int64_t, int64_t, int, int, const int*, cudaStream_t);
 int proj_wgrad_simt(const int8_t*, int64_t, const float*, int64_t, float*, float*, int64_t, int, int, int, const int*, int64_t, cudaStream_t);
-int score_topk_simt(const float*, int64_t, const float*, int64_t, const int*, int, int, int, const int*, const int*, int, int*, float*, float*, int64_t, cudaStream_t);
+int score_topk_simt(const float*, int64_t, const float*, int64_t, const int*, int, const int*, int, int, const int*, const int*, int, int*, float*, float*, int64_t, cudaStream_t);
 bool proj_tc_supported(int d, int64_t ldx, const void* X, int k, bool wgrad, XType xt);
 int proj_fwd_tc_group(const llmrec_proj_fwd_problem*, const int32_t* const*, int, int, int, XType, cudaStream_t);
 int proj_wgrad_tc_group(const llmrec_proj_wgrad_problem*, const int32_t* const*, const int64_t*, int, int, int, XType, float*, int64_t, cudaStream_t);
 int64_t proj_wgrad_tc_scratch(const llmrec_proj_wgrad_problem*, int, int, int, XType);
 bool score_tc_supported(int d, int K, long long ldu, long long ldi, const void* U, const void* I);
 long long score_tc_scratch(int n_batch, int n_items, int d, int K);
-int score_topk_tc(const float*, long long, const float*, long long, const int*, int, int, int, const int*, const int*, int, int*, float*, float*, long long, cudaStream_t);
+int score_topk_tc(const float*, long long, const float*, long long, const int*, int, const int*, int, int, const int*, const int*, int, int*, float*, float*, long long, cudaStream_t);
 }  // namespace llmrec
 using namespace llmrec;
 
@@ -229,14 +229,35 @@ extern "C" int64_t llmrec_score_topk_scratch(int32_t n_batch, int32_t n_items, i
   if (want < n_items) want = n_items;
   return want;
 }
+// among: NULL (the catalog is the n_items rows of I), or n_items ascending global ids of rows of I
+static int score_topk(const float* U, int64_t ldu, const float* I, int64_t ldi, const int32_t* users, int32_t n_batch, const int32_t* among,
+                      int32_t n_items, int32_t d, const int32_t* mask_rowptr, const int32_t* mask_col, int32_t K, int32_t* out_idx,
+                      float* out_val, int32_t mode, float* scratch, int64_t scratch_elems, llmrec_stream_t stream) {
+  LLMREC_REQUIRE_DEVICE();
+  LLMREC_CHECK_ARG(K >= 1 && K <= 64 && K <= n_items, among ? "score_topk_among: K=%d unsupported (1..64, <= n_among)"
+                                                            : "score_topk: K=%d unsupported (1..64, <= n_items)", K);
+  if (n_batch <= 0) return 0;
+  if (mode != 2 && score_tc_supported(d, K, ldu, ldi, U, I))
+    return score_topk_tc(U, ldu, I, ldi, users, n_batch, among, n_items, d, mask_rowptr, mask_col, K, out_idx, out_val, scratch, scratch_elems,
+                         as_stream(stream));
+  return score_topk_simt(U, ldu, I, ldi, users, n_batch, among, n_items, d, mask_rowptr, mask_col, K, out_idx, out_val, scratch, scratch_elems,
+                         as_stream(stream));
+}
 extern "C" int llmrec_score_topk_f32(const float* U, int64_t ldu, const float* I, int64_t ldi, const int32_t* users, int32_t n_batch,
                                      int32_t n_items, int32_t d, const int32_t* mask_rowptr, const int32_t* mask_col, int32_t K,
                                      int32_t* out_idx, float* out_val, int32_t mode, float* scratch, int64_t scratch_elems,
                                      llmrec_stream_t stream) {
-  LLMREC_REQUIRE_DEVICE();
-  LLMREC_CHECK_ARG(K >= 1 && K <= 64 && K <= n_items, "score_topk: K=%d unsupported (1..64, <= n_items)", K);
-  if (n_batch <= 0) return 0;
-  if (mode != 2 && score_tc_supported(d, K, ldu, ldi, U, I))
-    return score_topk_tc(U, ldu, I, ldi, users, n_batch, n_items, d, mask_rowptr, mask_col, K, out_idx, out_val, scratch, scratch_elems, as_stream(stream));
-  return score_topk_simt(U, ldu, I, ldi, users, n_batch, n_items, d, mask_rowptr, mask_col, K, out_idx, out_val, scratch, scratch_elems, as_stream(stream));
+  return score_topk(U, ldu, I, ldi, users, n_batch, nullptr, n_items, d, mask_rowptr, mask_col, K, out_idx, out_val, mode, scratch, scratch_elems,
+                    stream);
+}
+extern "C" int64_t llmrec_score_topk_among_scratch(int32_t n_batch, int32_t n_among, int32_t d, int32_t K, int32_t mode) {
+  return llmrec_score_topk_scratch(n_batch, n_among, d, K, mode);
+}
+extern "C" int llmrec_score_topk_among_f32(const float* U, int64_t ldu, const float* I, int64_t ldi, const int32_t* users, int32_t n_batch,
+                                           const int32_t* among, int32_t n_among, int32_t d, const int32_t* mask_rowptr, const int32_t* mask_col,
+                                           int32_t K, int32_t* out_idx, float* out_val, int32_t mode, float* scratch, int64_t scratch_elems,
+                                           llmrec_stream_t stream) {
+  LLMREC_CHECK_ARG(among || n_among <= 0, "score_topk_among: among is NULL");
+  return score_topk(U, ldu, I, ldi, users, n_batch, among, n_among, d, mask_rowptr, mask_col, K, out_idx, out_val, mode, scratch, scratch_elems,
+                    stream);
 }

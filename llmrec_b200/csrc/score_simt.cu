@@ -2,13 +2,24 @@
 // hit-vector lookup (:30-34).  mode 2 of llmrec_score_topk_f32: sequential-FMA fp32 scores, exact
 // selection with ties -> lowest item id.  It is the on-device checker of the wgmma kernel and the
 // path for K/d the tensor-core kernel does not cover.
+//
+// The catalog is I, or (among != NULL, llmrec_score_topk_among_f32) the rows among[0 .. n_items) of I with ids
+// ascending: column j of the score block is item among[j], mask rows and returned ids are global item ids.
 #include "common.cuh"
 
 namespace llmrec {
 
-// scores for a block of users into scratch[b][n_items]; train items -> -inf
+// position of global item id v in the ascending catalog ids among[0 .. n), or -1 when it is not there
+__device__ __forceinline__ int catalog_pos(const int* __restrict__ among, int n, int v) {
+  int lo = 0, hi = n;
+  while (lo < hi) { const int m = (lo + hi) >> 1; const int x = __ldg(among + m); if (x < v) lo = m + 1; else hi = m; }
+  return lo < n && __ldg(among + lo) == v ? lo : -1;
+}
+
+// scores for a block of users into scratch[b][n_items] (column j = catalog item j)
 __global__ void __launch_bounds__(256) score_rows_kernel(const float* __restrict__ U, int64_t ldu, const float* __restrict__ I, int64_t ldi,
-                                                         const int* __restrict__ users, int n_items, int d, float* __restrict__ S) {
+                                                         const int* __restrict__ users, const int* __restrict__ among, int n_items, int d,
+                                                         float* __restrict__ S) {
   extern __shared__ float us[];  // d
   const int b = blockIdx.y;
   const float* u = U + (int64_t)users[b] * ldu;
@@ -16,21 +27,25 @@ __global__ void __launch_bounds__(256) score_rows_kernel(const float* __restrict
   __syncthreads();
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n_items) return;
-  const float* it = I + (int64_t)i * ldi;
+  const float* it = I + (int64_t)(among ? __ldg(among + i) : i) * ldi;
   float a = 0.f;
   for (int j = 0; j < d; ++j) a = fmaf(us[j], it[j], a);
   S[(int64_t)b * n_items + i] = a;
 }
-__global__ void mask_rows_kernel(const int* __restrict__ users, const int* __restrict__ rowptr, const int* __restrict__ col, int n_items, float* __restrict__ S) {
+// masked items -> -inf; with `among`, a masked id outside the catalog is skipped
+__global__ void mask_rows_kernel(const int* __restrict__ users, const int* __restrict__ rowptr, const int* __restrict__ col,
+                                 const int* __restrict__ among, int n_items, float* __restrict__ S) {
   const int b = blockIdx.x;
   const int u = users[b];
   for (int e = rowptr[u] + threadIdx.x; e < rowptr[u + 1]; e += blockDim.x) {
     int c = col[e];
+    if (among) c = catalog_pos(among, n_items, c);
     if (c >= 0 && c < n_items) S[(int64_t)b * n_items + c] = -INFINITY;
   }
 }
-// K rounds of block arg-max with (score desc, id asc) order
-__global__ void __launch_bounds__(256) select_topk_kernel(float* __restrict__ S, int n_items, int K, int* __restrict__ out_idx, float* __restrict__ out_val) {
+// K rounds of block arg-max with (score desc, id asc) order; ascending catalog ids make the lowest column the lowest id
+__global__ void __launch_bounds__(256) select_topk_kernel(float* __restrict__ S, const int* __restrict__ among, int n_items, int K,
+                                                          int* __restrict__ out_idx, float* __restrict__ out_val) {
   __shared__ float bv[8]; __shared__ int bi[8];
   __shared__ int win;
   const int b = blockIdx.x;
@@ -51,7 +66,7 @@ __global__ void __launch_bounds__(256) select_topk_kernel(float* __restrict__ S,
     if (threadIdx.x == 0) {
       for (int w = 1; w < 8; ++w) if (bv[w] > best || (bv[w] == best && bi[w] < besti)) { best = bv[w]; besti = bi[w]; }
       bool ok = besti != 0x7fffffff && best != -INFINITY;
-      out_idx[(int64_t)b * K + r] = ok ? besti : -1;
+      out_idx[(int64_t)b * K + r] = ok ? (among ? among[besti] : besti) : -1;
       if (out_val) out_val[(int64_t)b * K + r] = ok ? best : -INFINITY;
       if (ok) s[besti] = -INFINITY;
       win = besti;
@@ -131,7 +146,8 @@ __global__ void __launch_bounds__(256) user_auc_kernel(const float* __restrict__
   }
 }
 
-int score_topk_simt(const float* U, int64_t ldu, const float* I, int64_t ldi, const int* users, int n_batch, int n_items, int d,
+// among: NULL (the catalog is I), or n_items ascending ids of rows of I (the catalog is those rows)
+int score_topk_simt(const float* U, int64_t ldu, const float* I, int64_t ldi, const int* users, int n_batch, const int* among, int n_items, int d,
                     const int* mask_rowptr, const int* mask_col, int K, int* out_idx, float* out_val,
                     float* scratch, int64_t scratch_elems, cudaStream_t st) {
   LLMREC_CHECK_ARG(scratch && scratch_elems >= (int64_t)n_items, "score_topk(simt): scratch too small");
@@ -140,10 +156,10 @@ int score_topk_simt(const float* U, int64_t ldu, const float* I, int64_t ldi, co
   for (int b0 = 0; b0 < n_batch; b0 += (int)per) {
     int nb = (int)((per < (int64_t)(n_batch - b0)) ? per : (int64_t)(n_batch - b0));
     dim3 grid((n_items + 255) / 256, nb);
-    score_rows_kernel<<<grid, 256, d * sizeof(float), st>>>(U, ldu, I, ldi, users + b0, n_items, d, scratch);
+    score_rows_kernel<<<grid, 256, d * sizeof(float), st>>>(U, ldu, I, ldi, users + b0, among, n_items, d, scratch);
     LLMREC_CHECK_LAUNCH("score_rows");
-    if (mask_rowptr) { mask_rows_kernel<<<nb, 128, 0, st>>>(users + b0, mask_rowptr, mask_col, n_items, scratch); LLMREC_CHECK_LAUNCH("mask_rows"); }
-    select_topk_kernel<<<nb, 256, 0, st>>>(scratch, n_items, K, out_idx + (int64_t)b0 * K, out_val ? out_val + (int64_t)b0 * K : nullptr);
+    if (mask_rowptr) { mask_rows_kernel<<<nb, 128, 0, st>>>(users + b0, mask_rowptr, mask_col, among, n_items, scratch); LLMREC_CHECK_LAUNCH("mask_rows"); }
+    select_topk_kernel<<<nb, 256, 0, st>>>(scratch, among, n_items, K, out_idx + (int64_t)b0 * K, out_val ? out_val + (int64_t)b0 * K : nullptr);
     LLMREC_CHECK_LAUNCH("select_topk");
   }
   return 0;

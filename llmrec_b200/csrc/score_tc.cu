@@ -17,6 +17,10 @@
 //     order -- the same arithmetic as the SIMT reference kernel -- and emits the final top-K by (score desc, id asc), so
 //     the 3xTF32 rounding of the selection pass (~1e-5 relative) cannot change the result unless it misranks by more
 //     than the slack.
+//   * the catalog may be a subset of I given by ascending ids (`among`, llmrec_score_topk_among_f32): the hi/lo copies
+//     are gathered compacted, column j of the catalog offers global id among[j] (each tile's 128 ids staged once in
+//     shared memory), and mask rows / returned ids stay global.  Ascending ids keep the merge pointer and the tie rule
+//     valid unchanged; among == NULL is the identity map (the whole of I).
 #include <stdlib.h>
 #include <string.h>
 #include "common.cuh"
@@ -35,7 +39,8 @@ constexpr uint32_t kTileI = SBN * SBK * 4;   // 16 KiB: one k-block of the hi or
 struct ScoreParams {
   CUtensorMap tmIhi, tmIlo;  // [n_items x d] hi / lo copies of I, box {32, 128}, SWIZZLE_128B
   const float* U; long long ldu;
-  const int* users; int n_batch, n_items, d;
+  const int* users; int n_batch, n_items, d;   // n_items: catalog size (rows of the hi / lo copies)
+  const int* among;                             // NULL, or catalog column j -> global item id among[j] (ascending)
   const int* mask_rowptr; const int* mask_col;  // train rows, columns sorted ascending
   int Kc, splits, tiles_per_split, stages;
   int* cand_idx; float* cand_val;  // [n_batch][splits][Kc]
@@ -55,6 +60,7 @@ __global__ void __launch_bounds__(128, 1) score_topk_tc_kernel(const __grid_cons
   float* lv = stg + SBM * kStageLd;                       // heap values [Kc][64]
   int* li = reinterpret_cast<int*>(lv + (size_t)Kc * SBM);   // heap ids [Kc][64]
   uint64_t* full = reinterpret_cast<uint64_t*>(li + (size_t)Kc * SBM);
+  int* tile_ids = reinterpret_cast<int*>(full + 8);       // [SBN] global ids of the current tile's columns (among only)
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int utile = blockIdx.x, split = blockIdx.y;
@@ -130,8 +136,8 @@ __global__ void __launch_bounds__(128, 1) score_topk_tc_kernel(const __grid_cons
     while (next_masked < item) { ++mp; next_masked = mp < mend ? __ldg(P.mask_col + mp) : 0x7fffffff; }
     return next_masked == item;
   };
-  auto offer = [&](float s, int item) {
-    if (item >= P.n_items || is_masked(item)) return;
+  auto offer = [&](float s, int col, int item) {   // catalog column col holds global item id `item`
+    if (col >= P.n_items || is_masked(item)) return;
     if (count < Kc) {
       HV(count) = s; HI(count) = item;
       if (++count == Kc) {
@@ -186,6 +192,10 @@ __global__ void __launch_bounds__(128, 1) score_topk_tc_kernel(const __grid_cons
             stg[(row + 8 * h) * kStageLd + col + 1] = acc[c][4 * j + 2 * h + 1];
           }
     }
+    if (P.among) {
+      const int col = t * SBN + tid;
+      tile_ids[tid] = col < P.n_items ? __ldg(P.among + col) : 0x7fffffff;
+    }
     __syncthreads();
     if (live) {
       const float* srow = stg + tid * kStageLd;
@@ -195,12 +205,12 @@ __global__ void __launch_bounds__(128, 1) score_topk_tc_kernel(const __grid_cons
         unsigned hit = 0;
 #pragma unroll
         for (int j = 0; j < 32; ++j) hit |= (srow[c0 + j] > thr ? 1u : 0u) << j;
-        const int item0 = t * SBN + c0;
+        const int col0 = t * SBN + c0;
         while (hit) {   // slow path: set bits in ascending item id
           const int j = __ffs(hit) - 1;
           hit &= hit - 1;
           const float s = srow[c0 + j];
-          if (count < Kc || s > thr) offer(s, item0 + j);
+          if (count < Kc || s > thr) offer(s, col0 + j, P.among ? tile_ids[c0 + j] : col0 + j);
         }
       }
     }
@@ -217,12 +227,14 @@ __global__ void __launch_bounds__(128, 1) score_topk_tc_kernel(const __grid_cons
   }
 }
 
-// I -> hi / lo copies (hi exactly TF32-representable)
-__global__ void split_hi_lo_kernel(const float* __restrict__ X, long long ldx, long long n, int d, float* __restrict__ hi, float* __restrict__ lo) {
+// I -> hi / lo copies (hi exactly TF32-representable); rows: NULL, or row r of the copies is row rows[r] of X
+__global__ void split_hi_lo_kernel(const float* __restrict__ X, long long ldx, const int* __restrict__ rows, long long n, int d,
+                                   float* __restrict__ hi, float* __restrict__ lo) {
   const long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;
   if (i >= n * d) return;
   const long long r = i / d; const int c = (int)(i - r * d);
-  const float v = X[r * ldx + c]; const float h = tf32_hi(v);
+  const long long src = rows ? (long long)__ldg(rows + r) : r;
+  const float v = X[src * ldx + c]; const float h = tf32_hi(v);
   hi[i] = h; lo[i] = v - h;
 }
 
@@ -302,7 +314,8 @@ long long score_tc_scratch(int n_batch, int n_items, int d, int K) {
   return 2LL * n_items * d + 2LL * n_batch * splits * score_kc(K) + 64;
 }
 
-int score_topk_tc(const float* U, long long ldu, const float* I, long long ldi, const int* users, int n_batch, int n_items, int d,
+// among: NULL (the catalog is I), or n_items ascending ids of rows of I (the catalog is those rows)
+int score_topk_tc(const float* U, long long ldu, const float* I, long long ldi, const int* users, int n_batch, const int* among, int n_items, int d,
                   const int* mask_rowptr, const int* mask_col, int K, int* out_idx, float* out_val, float* scratch, long long scratch_elems,
                   cudaStream_t st) {
   LLMREC_CHECK_ARG(scratch && scratch_elems >= score_tc_scratch(n_batch, n_items, d, K), "score_topk: scratch too small");
@@ -315,14 +328,15 @@ int score_topk_tc(const float* U, long long ldu, const float* I, long long ldi, 
   int* cidx = reinterpret_cast<int*>(cval + (long long)n_batch * P.splits * P.Kc);
   {
     const long long n = (long long)n_items * d;
-    split_hi_lo_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(I, ldi, n_items, d, Ihi, Ilo);
+    split_hi_lo_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(I, ldi, among, n_items, d, Ihi, Ilo);
     LLMREC_CHECK_LAUNCH("split_hi_lo");
   }
   if (!make_tmap_2d_f32(&P.tmIhi, Ihi, (uint64_t)d, (uint64_t)n_items, (uint64_t)d * 4, SBK, SBN)) return 4;
   if (!make_tmap_2d_f32(&P.tmIlo, Ilo, (uint64_t)d, (uint64_t)n_items, (uint64_t)d * 4, SBK, SBN)) return 4;
-  P.U = U; P.ldu = ldu; P.users = users; P.n_batch = n_batch; P.n_items = n_items; P.d = d;
+  P.U = U; P.ldu = ldu; P.users = users; P.n_batch = n_batch; P.n_items = n_items; P.d = d; P.among = among;
   P.mask_rowptr = mask_rowptr; P.mask_col = mask_col; P.cand_idx = cidx; P.cand_val = cval;
-  const size_t fixed = (size_t)2 * d * SBM * 4 /*A hi, lo*/ + (size_t)SBM * kStageLd * 4 + (size_t)P.Kc * SBM * 8 /*heaps*/ + 64 /*barriers*/ + 1024 /*align*/;
+  const size_t fixed = (size_t)2 * d * SBM * 4 /*A hi, lo*/ + (size_t)SBM * kStageLd * 4 + (size_t)P.Kc * SBM * 8 /*heaps*/ + 64 /*barriers*/ +
+                       (among ? SBN * 4 : 0) /*tile ids*/ + 1024 /*align*/;
   int stages = (int)((227 * 1024 - fixed) / (2 * kTileI));
   if (stages > 4) stages = 4;
   LLMREC_CHECK_ARG(stages >= 2, "score_topk: not enough shared memory for the pipeline");

@@ -491,7 +491,7 @@ class Trainer(object):
             self.hot.forward()
         return self.hot
 
-    def recommend(self, users=None, K=10, exclude="train", histories=None, new_items=None):
+    def recommend(self, users=None, K=10, exclude="train", histories=None, new_items=None, among=None, exclude_items=None):
         """-> (ids int64 [m x K], scores fp32 [m x K]) on the device: each row's K best items, ties to the lowest item id, padded with
         -1 / -inf when fewer than K items are left.
         users: trained user ids (default every user).  histories: item-id lists or a (rowptr, col) pair, folded in with the trained item
@@ -499,13 +499,18 @@ class Trainer(object):
         items added after training (user-id lists or a (rowptr, col) pair), folded in with the trained user side (HotPath.fold_in_items)
         and scored after the trained catalog as ids n_items + j.  exclude: "train" masks a trained user's training items and a history's
         own items, and every new item whose list names the user (a history: its trained id); "none" masks nothing (the reference's
-        candidate lists).  K: 1..64 and at most the catalog size.  --proj_mode picks the scoring mode."""
-        Rn = recommend.new_items_csr(new_items, self.n_users)
-        recommend.check_k(K, self.n_items + (0 if Rn is None else Rn.shape[0]))
+        candidate lists).
+        among: rank only these item ids (an int list, ndarray or tensor; ids in [0, n_items + m), so new item j is n_items + j; order
+        and repeats do not matter); None ranks the whole catalog.  exclude_items: per query, item ids to leave out on top of `exclude`
+        (one row per query: id lists, a (rowptr, col) pair, or a 2-D array [m x C] with -1 as padding; ids in [0, n_items + m)); it
+        only hides items, the scores are unchanged.  Returned ids are catalog ids either way.
+        K: 1..64, at most the catalog size and at most the number of distinct ids in `among`.  Every argument is checked before
+        anything runs.  --proj_mode picks the scoring mode."""
+        job = recommend.prepare_top_k(self.hot, self.graph.rowptr_u, self.graph.col_u, users=users, K=K, exclude=exclude,
+                                      histories=histories, new_items=new_items, among=among, exclude_items=exclude_items)
         hot = self._current_model()
         mode = ops.SCORE_MODE.get(getattr(self.args, "proj_mode", "3xtf32"), 0)
-        return recommend.top_k(hot, self.graph.rowptr_u, self.graph.col_u, users=users, K=K, exclude=exclude, histories=histories, mode=mode,
-                               new_items=Rn)
+        return recommend.run_top_k(hot, job, mode)
 
     def fold_in(self, histories, known=None):
         """-> U_new [m x d]: the fused user representations of item-id histories (lists or a (rowptr, col) pair) under the current
@@ -522,15 +527,21 @@ class Trainer(object):
             raise ValueError("fold_in_items: give one user-id list per item")
         return self._current_model().fold_in_items(R.indptr, R.indices, known=known)
 
-    def similar_items(self, items, K=10, new_items=None):
+    def similar_items(self, items, K=10, new_items=None, among=None):
         """-> (ids int64 [q x K], cosines fp32 [q x K]) on the device: each query item's K nearest items by cosine of the fused item rows,
         never the query itself, ties to the lowest id, padded with -1 / -inf.  items: trained ids, or n_items + j for the j-th of
-        `new_items` (user lists of items added after training, as for `recommend`).  K: 1..64 and below the catalog size."""
+        `new_items` (user lists of items added after training, as for `recommend`).  among: the neighbours come only from these item
+        ids (as for `recommend`; a query need not be one of them); None = the whole catalog.  K: 1..64 and below the catalog size, or
+        with `among` at most its number of distinct ids."""
         Rn = recommend.new_items_csr(new_items, self.n_users)
-        recommend.check_k(K, self.n_items + (0 if Rn is None else Rn.shape[0]) - 1, "the catalog size - 1")
+        n = self.n_items + (0 if Rn is None else Rn.shape[0])
+        if among is None:
+            recommend.check_k(K, n - 1, "the catalog size - 1")
+        else:
+            recommend.check_k(K, recommend.catalog_ids(among, n, self.hot.E_u.device).numel(), "|among|")
         hot = self._current_model()
         mode = ops.SCORE_MODE.get(getattr(self.args, "proj_mode", "3xtf32"), 0)
-        return recommend.similar_items(hot, items, K=K, new_items=Rn, mode=mode)
+        return recommend.similar_items(hot, items, K=K, new_items=Rn, mode=mode, among=among)
 
     def score(self, users, items, new_items=None):
         """-> fp32 [n] on the device: the model's score <U[users[p]], I[items[p]]> of each (user, item) pair, by the exact fp32 chain of the
@@ -559,10 +570,11 @@ class Trainer(object):
         ids, _ = self.rerank(candidates, K=K)
         return recommend.write_candidates(path, ids)
 
-    def write_candidates(self, path, K=10):
-        """--candidates_out: the top-K of every user over the whole catalog, nothing excluded (torch.topk(U . I^T, k=K) of the reference's
-        stage 1), pickled as a CPU int64 tensor [n_users x K] to `path` (atomically)."""
-        ids, _ = self.recommend(K=K, exclude="none")
+    def write_candidates(self, path, K=10, among=None):
+        """--candidates_out: the top-K of every user over the whole catalog, or over the item ids `among` (--candidates_among), nothing
+        excluded (torch.topk(U . I^T, k=K) of the reference's stage 1), pickled as a CPU int64 tensor [n_users x K] to `path`
+        (atomically)."""
+        ids, _ = self.recommend(K=K, exclude="none", among=among)
         return recommend.write_candidates(path, ids)
 
     # ---- training loop (main.py:189-326) -----------------------------------------------------------------
@@ -647,21 +659,36 @@ def main(argv=None):
     gen = Data(path=ddir, batch_size=args.batch_size, sampler=args.host_sampler)
     batch_test.init(gen, args)
     config = dict(n_users=gen.n_users, n_items=gen.n_items)
-    if args.candidates_out:                                           # before any training: a bad K or flag mix fails at once
-        recommend.check_k(args.candidates_k, gen.n_items)
+    cand_among = check_candidates_flags(args, gen.n_items)           # before any training: a bad K, file or flag mix fails at once
     trainer = Trainer(data_config=config, data_generator=gen)         # --resume loads here, after set_seed and the model's own draws
     if args.candidates_out and trainer.masked_mode:
         raise ValueError("--candidates_out needs a fixed model: not with --mask / --mask_rate > 0 / --drop_rate > 0")
     rerank_in, rerank_k = check_rerank_flags(args, trainer)
     ret = trainer.evaluate() if args.eval_only else trainer.train()
     if args.candidates_out:                                           # from the model in memory when the run ends
-        trainer.write_candidates(args.candidates_out, args.candidates_k)
+        trainer.write_candidates(args.candidates_out, args.candidates_k, among=cand_among)
         trainer.logger.logging("candidates: top-%d of %d users written to %s" % (args.candidates_k, trainer.n_users, args.candidates_out))
     if rerank_in is not None:
         trainer.write_rerank(args.rerank_out, rerank_in, rerank_k)
         trainer.logger.logging("rerank: %d users' candidates from %s, top-%d written to %s" % (trainer.n_users, args.rerank_in, rerank_k,
                                                                                               args.rerank_out))
     return ret
+
+
+def check_candidates_flags(args, n_items):
+    """--candidates_out / --candidates_k / --candidates_among, checked before the first training step -> the ids of --candidates_among
+    (int64 CPU, sorted, distinct), or None."""
+    among_path = getattr(args, "candidates_among", None)
+    if among_path and not args.candidates_out:
+        raise ValueError("--candidates_among restricts the --candidates_out file: give --candidates_out too")
+    if not args.candidates_out:
+        return None
+    if not among_path:
+        recommend.check_k(args.candidates_k, n_items)
+        return None
+    among = recommend.read_among(among_path, n_items)
+    recommend.check_k(args.candidates_k, among.numel(), "|--candidates_among|")
+    return among
 
 
 def check_rerank_flags(args, trainer):

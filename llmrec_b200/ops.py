@@ -552,22 +552,42 @@ SCORE_MODE = {"3xtf32": 0, "fp32": 2}
 _score_scratch = {}
 
 
+def _score_topk_scratch(need, device):
+    """The per-device scratch of score_topk / score_topk_among, grown to `need` fp32 elements (None while nothing was needed)."""
+    key = device.index
+    scratch = _score_scratch.get(key)
+    if need and (scratch is None or scratch.numel() < need):
+        if scratch is not None:
+            _retired.append(scratch)
+        scratch = _score_scratch[key] = torch.empty(need, dtype=torch.float32, device=device)
+    return scratch
+
+
 def score_topk(U, I, users, mask_rowptr, mask_col, K, mode=0, want_vals=False):
     """Top-K item ids per user among items not in the user's mask row; ties -> lowest id."""
     _mat(U); _mat(I)
     nb, ni, d = int(users.numel()), int(I.shape[0]), int(I.shape[1])
     idx = torch.empty((nb, K), dtype=torch.int32, device=U.device)
     val = torch.empty((nb, K), dtype=torch.float32, device=U.device) if want_vals else None
-    need = int(N.lib().llmrec_score_topk_scratch(nb, ni, d, K, mode))
-    key = U.device.index
-    scratch = _score_scratch.get(key)
-    if need and (scratch is None or scratch.numel() < need):
-        if scratch is not None:
-            _retired.append(scratch)
-        scratch = _score_scratch[key] = torch.empty(need, dtype=torch.float32, device=U.device)
+    scratch = _score_topk_scratch(int(N.lib().llmrec_score_topk_scratch(nb, ni, d, K, mode)), U.device)
     N.check(N.lib().llmrec_score_topk_f32(_p(U), _ld(U), _p(I), _ld(I), _p(_i32(users)), nb, ni, d, _p(mask_rowptr), _p(mask_col), K,
                                            _p(idx), _p(val), mode, _p(scratch), scratch.numel() if scratch is not None else 0,
                                            _stream()), "score_topk")
+    _count(3)
+    return (idx, val) if want_vals else idx
+
+
+def score_topk_among(U, I, users, among, mask_rowptr, mask_col, K, mode=0, want_vals=False):
+    """score_topk over the catalog rows `among` of I (int32 device ids, strictly ascending): mask rows and returned ids are global
+    item ids, a masked id outside `among` is ignored, ties -> lowest id, K <= among.numel()."""
+    _mat(U); _mat(I)
+    nb, na, d = int(users.numel()), int(among.numel()), int(I.shape[1])
+    idx = torch.empty((nb, K), dtype=torch.int32, device=U.device)
+    val = torch.empty((nb, K), dtype=torch.float32, device=U.device) if want_vals else None
+    scratch = _score_topk_scratch(int(N.lib().llmrec_score_topk_among_scratch(nb, na, d, K, mode)), U.device)
+    N.check(N.lib().llmrec_score_topk_among_f32(_p(U), _ld(U), _p(I), _ld(I), _p(_i32(users)), nb, _p(_i32(among, "among")), na, d,
+                                                 _p(mask_rowptr), _p(mask_col), K, _p(idx), _p(val), mode, _p(scratch),
+                                                 scratch.numel() if scratch is not None else 0, _stream()), "score_topk_among")
     _count(3)
     return (idx, val) if want_vals else idx
 

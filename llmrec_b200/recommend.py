@@ -8,6 +8,10 @@ the lowest item id, K <= 64; a row with fewer than K candidates is padded with i
 item j gets catalog id n_items + j.  The host side only builds CSRs (the mask rows, the folded-in histories and item lists) and the
 output file.
 
+`among` restricts the catalog to given item ids and `exclude_items` adds per-query ids to the mask rows: the catalog rows are the
+argument of `ops.score_topk_among` (llmrec_score_topk_among_f32, the same kernels with the catalog given by ids), and the caller's rows
+are merged with the rows of `exclude` on the device (`merge_rows`).
+
 Scores of given (user, item) pairs are `ops.score_pairs` (llmrec_score_pairs_f32) and re-ranking of given candidate lists is
 `ops.rerank` (llmrec_rerank_f32, K <= 1024): the same sequential fp32 chain as score_topk's returned scores, so the bits agree, and the
 same mask rows (`exclusion_mask`) for exclude="train".
@@ -49,13 +53,17 @@ def _i32(a, dev):
     return torch.from_numpy(np.ascontiguousarray(np.asarray(a).astype(np.int32))).to(dev)
 
 
-def _score(U, I, users, mask_rowptr, mask_col, K, mode):
-    """score_topk over `users` (int32 device rows of U) in blocks -> (ids int64 [n x K], scores fp32 [n x K]) on the device"""
+def _score(U, I, users, mask_rowptr, mask_col, K, mode, among=None):
+    """score_topk over `users` (int32 device rows of U) in blocks -> (ids int64 [n x K], scores fp32 [n x K]) on the device; among:
+    None (the whole catalog I) or the catalog's ids (int32 device, strictly ascending; score_topk_among)"""
     n, dev = int(users.numel()), U.device
     ids = torch.empty((n, K), dtype=torch.int64, device=dev)
     vals = torch.empty((n, K), dtype=torch.float32, device=dev)
     for s in range(0, n, USER_BLOCK):
-        idx, v = ops.score_topk(U, I, users[s:s + USER_BLOCK], mask_rowptr, mask_col, K, mode=mode, want_vals=True)
+        if among is None:
+            idx, v = ops.score_topk(U, I, users[s:s + USER_BLOCK], mask_rowptr, mask_col, K, mode=mode, want_vals=True)
+        else:
+            idx, v = ops.score_topk_among(U, I, users[s:s + USER_BLOCK], among, mask_rowptr, mask_col, K, mode=mode, want_vals=True)
         ids[s:s + USER_BLOCK].copy_(idx)
         vals[s:s + USER_BLOCK].copy_(v)
     return ids, vals
@@ -150,7 +158,66 @@ def check_exclude(exclude):
         raise ValueError(f"exclude = {exclude!r}: one of {EXCLUDE}")
 
 
-def top_k(engine, train_rowptr, train_col, users=None, K=10, exclude="train", histories=None, mode=0, new_items=None):
+def catalog_ids(among, n_catalog, device, what="among"):
+    """The item ids of a restricted catalog (int list, ndarray or tensor) -> int32 device tensor, sorted with repeats removed on the
+    device; raises ValueError on non-integers, ids outside [0, n_catalog) or an empty set."""
+    a = _ids(among, what)
+    if a.numel() == 0:
+        raise ValueError(f"{what}: the catalog to rank is empty; give at least one item id")
+    _check_range(a, 0, n_catalog, what, "item id")
+    return torch.unique(a.to(device)).to(torch.int32)
+
+
+def merge_rows(a_rowptr, a_col, b_rowptr, b_col, n_catalog):
+    """Row r of the result = the sorted union of row r of a and row r of b without repeats (CSRs with the same number of rows, ids in
+    [0, n_catalog); ids < 0 in b are padding and dropped) -> (rowptr, col) int32 on a's device."""
+    dev = a_col.device
+    a, b = a_rowptr.to(dev).long(), b_rowptr.to(dev).long()
+    m = a.numel() - 1
+    ra = torch.repeat_interleave(torch.arange(m, device=dev), a[1:] - a[:-1])
+    rb = torch.repeat_interleave(torch.arange(m, device=dev), b[1:] - b[:-1])
+    bc = b_col.to(dev).long()
+    keep = bc >= 0
+    keys = torch.unique(torch.cat([ra * n_catalog + a_col.long(), rb[keep] * n_catalog + bc[keep]]))      # sorted: by row, then id
+    rp = torch.zeros(m + 1, dtype=torch.long, device=dev)
+    rp[1:] = torch.cumsum(torch.bincount(keys // n_catalog, minlength=m), 0)
+    return rp.to(torch.int32), (keys % n_catalog).to(torch.int32)
+
+
+def prepare_top_k(engine, train_rowptr, train_col, users=None, K=10, exclude="train", histories=None, new_items=None, among=None,
+                  exclude_items=None):
+    """Every check of `top_k`, and its host-side inputs, before anything is launched: -> a dict for `run_top_k`."""
+    check_engine(engine)
+    Rn = new_items_csr(new_items, engine.nu)
+    n = engine.ni + (0 if Rn is None else Rn.shape[0])
+    dev = engine.E_u.device
+    S = None if among is None else catalog_ids(among, n, dev)
+    K = check_k(K, n) if S is None else check_k(K, S.numel(), "|among|")
+    check_exclude(exclude)
+    extra = None if exclude_items is None else candidates_csr(exclude_items, n)
+    R, rows, rp, col, kn = _queries(engine, train_rowptr, train_col, users, histories)
+    if extra is not None and extra[0].numel() - 1 != len(rows):
+        raise ValueError(f"exclude_items: {extra[0].numel() - 1} rows for {len(rows)} " + ("users" if R is None else "histories"))
+    rp, col = exclusion_mask(engine, rp, col, exclude, Rn, kn)
+    qrow = _i32(rows, dev)
+    if extra is not None:                                    # per-query mask rows: query b reads mask row b, and U row b of its own copy
+        rp, col = merge_rows(*select_rows(rp, col, qrow), extra[0], extra[1], n)
+    return dict(R=R, known=kn, Rn=Rn, qrow=qrow, per_query=extra is not None, mask_rowptr=rp, mask_col=col, K=K, among=S)
+
+
+def run_top_k(engine, job, mode=0):
+    """The launches of `top_k` for a `prepare_top_k` job: fold-ins, then the scoring launches."""
+    U = _query_rows(engine, job["R"], job["known"])
+    I = _catalog(engine, job["Rn"])
+    qrow = job["qrow"]
+    if job["per_query"]:
+        U = U[qrow.long()].contiguous()                      # the same fp32 rows, so the same score bits
+        qrow = torch.arange(qrow.numel(), dtype=torch.int32, device=qrow.device)
+    return _score(U, I, qrow, job["mask_rowptr"], job["mask_col"], job["K"], mode, job["among"])
+
+
+def top_k(engine, train_rowptr, train_col, users=None, K=10, exclude="train", histories=None, mode=0, new_items=None, among=None,
+          exclude_items=None):
     """Top-K of a model whose last full `forward()` is current (U, I and the item side).
     users: trained user ids (default every user), scored from U's rows; with `histories` they name the trained id of each history (or
     -1), and may be omitted.  histories: a sequence of item-id lists or a (rowptr, col) pair; they are folded in (HotPath.fold_in).
@@ -158,36 +225,34 @@ def top_k(engine, train_rowptr, train_col, users=None, K=10, exclude="train", hi
     after the trained catalog as ids n_items + j.
     exclude: "train" masks the training row of a trained user, and the history itself for a folded-in one, plus every new item whose
     list names that user (for a history: its trained id); "none" masks nothing.
+    among: None (the whole catalog), or the item ids to rank (int list, ndarray or tensor; ids in [0, n_items + m), repeats collapsed);
+    K is then at most the number of distinct ids.
+    exclude_items: None, or one row of item ids per query (`candidates_csr` forms; -1 = padding) masked on top of what `exclude` masks.
     train_rowptr / train_col: the training rows (int32 device CSR, rows sorted), the mask of exclude="train".
-    mode: ops.SCORE_MODE.  -> (ids int64 [m x K], scores fp32 [m x K]) on the engine's device."""
-    check_engine(engine)
-    Rn = new_items_csr(new_items, engine.nu)
-    K = check_k(K, engine.ni + (0 if Rn is None else Rn.shape[0]))
-    check_exclude(exclude)
-    R, rows, rp, col, kn = _queries(engine, train_rowptr, train_col, users, histories)
-    U = _query_rows(engine, R, kn)
-    I = _catalog(engine, Rn)
-    rp, col = exclusion_mask(engine, rp, col, exclude, Rn, kn)
-    return _score(U, I, _i32(rows, engine.E_u.device), rp, col, K, mode)
+    mode: ops.SCORE_MODE.  -> (ids int64 [m x K], scores fp32 [m x K]) on the engine's device; ids are catalog ids."""
+    job = prepare_top_k(engine, train_rowptr, train_col, users, K, exclude, histories, new_items, among, exclude_items)
+    return run_top_k(engine, job, mode)
 
 
-def similar_items(engine, items, K=10, new_items=None, mode=0):
+def similar_items(engine, items, K=10, new_items=None, mode=0, among=None):
     """Item-to-item neighbours of a model whose last full `forward()` is current: each query's K nearest items by cosine of the fused
     item rows, over the trained catalog and the m new items of `new_items` (ids n_items + j, as in `top_k`); the query itself is never
-    returned.  items: query ids in [0, n_items + m).  -> (ids int64 [q x K], cosines fp32 [q x K]) on the engine's device, ties to the
-    lowest id, padded with -1 / -inf.  The rows are normalised by llmrec_row_normalize_f32 and scored against each other by
-    score_topk; the mask row of catalog item i holds i alone."""
+    returned.  items: query ids in [0, n_items + m).  among: None (the whole catalog), or the ids the neighbours come from (as in
+    `top_k`; a query need not be one of them); K is then at most the number of distinct ids.  -> (ids int64 [q x K], cosines fp32
+    [q x K]) on the engine's device, ties to the lowest id, padded with -1 / -inf.  The rows are normalised by
+    llmrec_row_normalize_f32 and scored against each other by score_topk; the mask row of catalog item i holds i alone."""
     check_engine(engine)
     Rn = new_items_csr(new_items, engine.nu)
     n = engine.ni + (0 if Rn is None else Rn.shape[0])
-    K = check_k(K, n - 1, "the catalog size - 1")
+    dev = engine.E_u.device
+    S = None if among is None else catalog_ids(among, n, dev)
+    K = check_k(K, n - 1, "the catalog size - 1") if S is None else check_k(K, S.numel(), "|among|")
     q = (items.detach().cpu().numpy() if hasattr(items, "detach") else np.asarray(items)).reshape(-1)
     if q.size and (q.dtype.kind not in "iu" or q.min() < 0 or q.max() >= n):
         raise ValueError(f"items: query ids are integers in [0, {n}) (trained items, then the new ones)")
-    dev = engine.E_u.device
     X = ops.row_normalize(_catalog(engine, Rn))
     eye_rp, eye_col = torch.arange(n + 1, dtype=torch.int32, device=dev), torch.arange(n, dtype=torch.int32, device=dev)
-    return _score(X, X, _i32(q, dev), eye_rp, eye_col, K, mode)
+    return _score(X, X, _i32(q, dev), eye_rp, eye_col, K, mode, S)
 
 
 def _ids(a, what):
@@ -357,6 +422,26 @@ def read_candidates(path, n_users, n_catalog):
                          f"{type(cand).__name__} {tuple(getattr(cand, 'shape', ()))}")
     _check_range(_ids(cand, f"--rerank_in {path}"), -1, n_catalog, f"--rerank_in {path}", "item id")
     return cand
+
+
+def read_among(path, n_catalog):
+    """The --candidates_among file (a pickled 1-D integer tensor, ndarray or list of item ids) -> int64 CPU tensor of the distinct ids,
+    sorted, checked: the file loads, is 1-D, holds integers in [0, n_catalog) and at least one id."""
+    flag = f"--candidates_among {path}"
+    try:
+        with open(os.fspath(path), "rb") as f:
+            ids = pickle.load(f)
+    except Exception as e:                                                  # noqa: BLE001 -- any unreadable file is a flag error
+        raise ValueError(f"{flag}: cannot read a pickled id list ({type(e).__name__}: {e})") from e
+    if isinstance(ids, list):
+        try:
+            ids = np.asarray(ids)
+        except ValueError:                                                  # a ragged list of lists
+            ids = None
+    if not hasattr(ids, "shape") or len(ids.shape) != 1:
+        raise ValueError(f"{flag}: need a 1-D integer tensor / ndarray or a list of item ids, got {type(ids).__name__} "
+                         f"{tuple(getattr(ids, 'shape', ()))}")
+    return catalog_ids(ids, n_catalog, "cpu", flag).long()
 
 
 def write_candidates(path, ids):

@@ -98,6 +98,9 @@ _EXTRA = [
                                                "items over the whole catalog, nothing excluded, as the pickled CPU int64 tensor [n_users x K] "
                                                "the augmentation stage reads (data/<dataset>/candidate_indices). Not with the mask / dropout branch")),
     ("candidates_k", dict(type=int, default=10, help="list length of --candidates_out (1..64, at most n_items)")),
+    ("candidates_among", dict(default=None, help="restrict --candidates_out to these items: a pickled 1-D integer tensor, ndarray or list "
+                                                 "of item ids (order and repeats do not matter); each user's list is then the top "
+                                                 "--candidates_k of these ids (at most their number). Needs --candidates_out")),
     ("rerank_in", dict(default=None, help="when the run ends, re-rank a candidate file with this model: a pickled 2-D integer tensor or "
                                           "ndarray [n_users x C], row u = user u's candidates, -1 = padding (the --candidates_out / "
                                           "candidate_indices format, so a file made by another model can be reordered by this one). "
