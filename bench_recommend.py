@@ -2,9 +2,9 @@
 neighbours) on one H100.
 
     python bench_recommend.py [--reps 3] [--syn_users 131072] [--syn_histories 8192] [--syn_items 65536] [--syn_scale 1.0]
-                              [--pairs 1048576] [--legs rerank,score_pairs]
+                              [--pairs 1048576] [--legs rerank,score_pairs,explain]
 
-Eight legs per workload, each timed end to end on the host clock between device synchronises (median of --reps calls after one
+Nine legs per workload, each timed end to end on the host clock between device synchronises (median of --reps calls after one
 warm-up call):
   known         trained users scored from U with their training items excluded (exclude="train"), K = 10; users/s
   fold_in       held-out histories folded in (HotPath.fold_in) and scored, exclude="train", K = 10; users/s
@@ -19,6 +19,11 @@ warm-up call):
                 times its kernel alone (llmrec_score_topk_among_f32, all users in one launch, between CUDA events), the plain call
                 (llmrec_score_topk_f32 over the whole catalog) and, where the [users x |among|] candidate CSR fits in int32, the same
                 question answered by llmrec_rerank_f32 with the set as every user's list
+  explain       the known leg's top-10 of every user (synthetic: --syn_users users) explained (Trainer.explain / recommend.explain:
+                every (target, history item, channel) contribution, own and last); queries/s.  Also times the kernel alone
+                (llmrec_explain_f32, all queries in one launch, between CUDA events, median of 5 windows of 20 launches) and reports
+                it as GB/s of gathered rows: per query its 10 target rows, its two user rows and, per history item, the n_id + n_side
+                source rows (4*d bytes each)
 Every call includes the full eval forward a recommendation starts with.  The rerank and score_pairs legs also time their kernel alone
 (llmrec_rerank_f32 / llmrec_score_pairs_f32 between CUDA events, median of 5 windows of 20 launches) and report it as GB/s of gathered
 rows: 4*d bytes per candidate row plus 4 per id (pairs: two rows and two ids), against the size of I (L2-resident at netflix,
@@ -162,6 +167,29 @@ def _among_legs(U, I, mask_rowptr, mask_col, e2e, n_q, mode, reps, seed=0):
     return out
 
 
+def _explain_leg(hp, rowptr, col, ids, e2e, users, reps):
+    """The explain leg: end to end (`e2e(ids)`, with its eval forward), and the kernel alone on the same queries"""
+    import numpy as np
+    from llmrec_b200 import ops, recommend
+    if ONLY and "explain" not in ONLY:
+        return None
+    n_q = int(ids.shape[0])
+    leg = _leg("explain", n_q, lambda: e2e(ids), reps, unit="queries")
+    job = recommend.prepare_explain(hp, rowptr, col, ids, users=users)
+    args = recommend.explain_args(hp, job)
+    k = _kernel(lambda: ops.explain(*args))
+    nnz, d, P = int(job["hist_col"].numel()), hp.d, int(ids.shape[1])
+    rows_per_item = len(args[2]) + len(args[5])                  # side terms + id sources
+    gb = ((nnz * rows_per_item + n_q * (P + 2)) * 4 * d) / 1e9
+    leg.update(targets_per_query=P, history_items=nnz, channels=1 + len(args[2]), kernel_s=round(k, 7),
+               kernel_queries_per_s=round(n_q / k, 1), kernel_GB_per_s=round(gb / k, 1),
+               outputs_per_s=round(P * nnz * (1 + len(args[2])) / k, 1))
+    sys.stderr.write(f"  {'explain kern':13s} {n_q:9d} queries  {k * 1e3:9.3f} ms       {n_q / k:12.0f} queries/s "
+                     f"{gb / k:7.1f} GB/s ({nnz} history items, {rows_per_item} rows each)\n")
+    del args, job
+    return leg
+
+
 def netflix(a, tmp):
     import numpy as np
     tr, gen, args = bench.make_trainer("netflix", types.SimpleNamespace(proj_mode=a.proj_mode, host_sampler="native", graph=1))
@@ -184,6 +212,9 @@ def netflix(a, tmp):
     res.update(_serving_legs(hp.U, hp.I, lambda cand: tr.rerank(cand, K=10), lambda u, i: tr.score(u, i), nu, 100, a.pairs, a.reps))
     res["among"] = _among_legs(hp.U, hp.I, tr.graph.rowptr_u, tr.graph.col_u, lambda S: tr.recommend(K=10, exclude="train", among=S), nu,
                                a.score_mode, a.reps)
+    if not ONLY or "explain" in ONLY:
+        ids, _ = tr.recommend(K=10, exclude="train")
+        res["explain"] = _explain_leg(tr._current_model(), tr.graph.rowptr_u, tr.graph.col_u, ids, lambda t: tr.explain(t), None, a.reps)
     del tr, gen
     return res
 
@@ -263,6 +294,15 @@ def synthetic(a, tmp):
 
     hp.forward()
     res["among"] = _among_legs(hp.U, hp.I, g.rowptr_u, g.col_u, among, n, a.score_mode, a.reps)
+
+    def explain(ids):
+        hp.forward()
+        recommend.explain(hp, g.rowptr_u, g.col_u, ids, users=users)
+
+    if not ONLY or "explain" in ONLY:
+        hp.forward()
+        ids, _ = recommend.top_k(hp, g.rowptr_u, g.col_u, users=users, K=10, exclude="train", mode=a.score_mode)
+        res["explain"] = _explain_leg(hp, g.rowptr_u, g.col_u, ids, explain, users, a.reps)
     del hp, g, params
     torch.cuda.empty_cache()
     return res

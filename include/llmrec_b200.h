@@ -417,6 +417,39 @@ int llmrec_rerank_f32(const float* U, int64_t ldu, const float* I, int64_t ldi, 
                       const int32_t* cand_rowptr, const int32_t* cand_col, const int32_t* mask_rowptr, const int32_t* mask_col,
                       int32_t n_catalog, int32_t d, int32_t K, int32_t* out_idx, float* out_val, llmrec_stream_t stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * Explanations: the exact split of scores <U[u], I[i]> over the query's history items and the model's
+ * channels (id, then the n_side side terms of the fusion in order).  With ui = diag(su) R, every user-side
+ * term but two is linear in the user's history: for history item j and target i,
+ *   contrib[.., 0]     = ((sum_{l < n_id} dot(id_src[l][j], I[i])) * su) * inv            (0 when n_id = 0)
+ *   contrib[.., 1 + t] = dot(side_src[t][j], I[i]) * ((coef[t] / max(sqrt(ss_t), 1e-12)) * su)
+ *   own = dot(own_src[u], I[i]) * inv,   last = dot(last_src[u], I[i]) * inv,   inv = 1.0f / n_layers
+ * where u = qrow[b], su = su[b], ss_t = the chain of x*x over side_usr[t][u] (the side row the fusion
+ * normalised), id_src = Il[0 .. L-2] (n_id = L - 1, n_layers = L + 1), own_src = Ul[0], last_src = Ul[L],
+ * and dot = the sequential chain a = 0; a = fmaf(x[k], y[k], a), k = 0..d-1, of llmrec_score_pairs_f32.
+ * Every product and sum is one IEEE fp32 operation in the order written, so each output has exactly one
+ * value, independent of the launch's grouping; own + last + sum contrib = <U[u], I[i]> up to the rounding of
+ * the propagation sums and of the fusion.
+ *
+ * Query b (< m) has history hist_col[hist_rowptr[b] .. hist_rowptr[b+1]) (H_b item ids; the caller
+ * collapses repeats) and targets targets[b * P .. b * P + P) (ids outside [0, n_catalog), e.g. -1, are
+ * padding).  contrib fp32 [P * nnz_h x (1 + n_side)]: query b's block starts at row P * hist_rowptr[b] and
+ * is [P x H_b x (1 + n_side)].  own / last fp32 [m x P].  A padding target gets zeros everywhere.
+ * top_n = 0: no selection; 1..LLMREC_EXPLAIN_MAX_TOP: top_ids int32 / top_vals fp32 [m x P x top_n] hold
+ * the top_n history items of each (query, target) with the largest total = sum of the channels in order
+ * (fp32, from 0), by (total desc, id asc) with the keys of llmrec_rerank_f32, padded with -1 / -inf (a
+ * padding target: -1 / 0).  Pointer tables (side_*, id_src, ld_*, coef) are host arrays.  No scratch, no
+ * host sync; one launch, and a second one with top_n > 0.
+ * --------------------------------------------------------------------------------------------- */
+#define LLMREC_EXPLAIN_MAX_TOP 64
+int llmrec_explain_f32(const float* own_src, int64_t ld_own, const float* last_src, int64_t ld_last,
+                       const float* const* side_usr, const int64_t* ld_side_usr, const float* const* side_src,
+                       const int64_t* ld_side_src, const float* coef, int32_t n_side, const float* const* id_src,
+                       const int64_t* ld_id, int32_t n_id, const float* I, int64_t ldi, int32_t n_catalog, int32_t d,
+                       int32_t n_layers, const int32_t* qrow, const float* su, int32_t m, const int32_t* hist_rowptr,
+                       const int32_t* hist_col, const int32_t* targets, int32_t P, float* contrib, float* own, float* last,
+                       int32_t top_n, int32_t* top_ids, float* top_vals, llmrec_stream_t stream);
+
 /* Host-side (CPU, no GPU needed) BPR item sampler, bit-identical to Data.sample()'s numpy draws
  * (utility/load_data.py:166-187): hand over numpy's legacy MT19937 state (np.random.get_state()), get the
  * positives / rejection-sampled negatives for `users` and the advanced state back.  All pointers HOST. */

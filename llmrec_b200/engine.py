@@ -389,34 +389,53 @@ class HotPath:
         kn = _known_ids(known, R.shape[0], self.ni, "fold_in_items: known must hold one trained item id in [0, {n}) or -1 per item ({m})")
         return self._fold_in(False, R, kn)
 
+    def fold_in_operands(self, rowptr, col, known=None):
+        """The per-row operands of `fold_in` before the fusion -> (layers, F, prof, su): the L + 1 layers [m x d] (layer 0 = E_u[known]
+        or zeros), the side-feature blocks F [m x S*d] and profile rows prof [m x d] (None without side features) and the row scales su
+        fp32 [m] of ui = diag(su) R.  `fold_in` fuses exactly these; explanations split a score over them (recommend.explain)."""
+        from .graph import history_matrix
+        R = history_matrix(rowptr, col, self.ni)
+        kn = _known_ids(known, R.shape[0], self.nu, "fold_in: known must hold one trained user id in [0, {n}) or -1 per history ({m})")
+        return self._fold_in_operands(True, R, kn)
+
     def _fold_in(self, users, R, kn):
         """The fold-in of m new rows of one side (users: R's rows are users over item ids, else items over user ids) with layer-0 ids
-        kn: the segments of the one launch are the other side's S blocks, its profile and its ID layers (softmax on l = L)."""
-        from .graph import inv_sqrt_degree
-        m, d, L, dev = R.shape[0], self.d, self.L, self.E_u.device
+        kn: the operands of `_fold_in_operands`, fused."""
+        m, d, dev = R.shape[0], self.d, self.E_u.device
         if m == 0:
             return torch.empty(0, d, dtype=torch.float32, device=dev)
+        layers, F, prof, _ = self._fold_in_operands(users, R, kn)
+        sides = self.sides.fused(F, prof) if self.has_feats else []
+        out = torch.empty(m, d, dtype=torch.float32, device=dev)
+        ops.fuse_fwd(layers, sides, self._side_coefs(), out)                                                                # :185-197
+        return out
+
+    def _fold_in_operands(self, users, R, kn):
+        """The one launch of a fold-in: the segments are the other side's S blocks, its profile and its ID layers (softmax on l = L).
+        -> (layers [L + 1] of [m x d], F [m x S*d] or None, prof [m x d] or None, the rows' scales fp32 [m])."""
+        from .graph import inv_sqrt_degree
+        m, d, L, dev = R.shape[0], self.d, self.L, self.E_u.device
         train_op, E = (self.ui, self.E_u) if users else (self.iu, self.E_i)
         t = lambda a, dt: torch.from_numpy(np.ascontiguousarray(a.astype(dt))).to(dev)
-        op = ops.CsrOperator(t(R.indptr, np.int32), t(R.indices, np.int32), m, R.shape[1], rs=t(inv_sqrt_degree(R), np.float32),
-                             tile_nnz=getattr(train_op.plan, "tile_nnz", 0))       # pieces cut as the training operator cuts them
         new = lambda *s: torch.empty(*s, dtype=torch.float32, device=dev)
+        rs = t(inv_sqrt_degree(R), np.float32)
+        if m == 0:
+            return [new(0, d) for _ in range(L + 1)], *((new(0, self.S * d), new(0, d)) if self.has_feats else (None, None)), rs
+        op = ops.CsrOperator(t(R.indptr, np.int32), t(R.indices, np.int32), m, R.shape[1], rs=rs,
+                             tile_nnz=getattr(train_op.plan, "tile_nnz", 0))       # pieces cut as the training operator cuts them
         layers = [new(m, d) for _ in range(L + 1)]
         self._fold_in_sources(users, R)
-        segs, sides = [], []
+        segs, F, prof = [], None, None
         if self.has_feats:
             F, prof = new(m, self.S * d), new(m, d)
             src_F, src_prof = (self.Pi, self.prof_i) if users else (self.Fu, self.P_usr)                   # :153-157,162-163,166-167
             segs += [(self.blk(src_F, s), self.blk(F, s), None, False) for s in range(self.S)]
             segs.append((src_prof, prof, None, False))
-            sides = self.sides.fused(F, prof)
         src_layers = self.Il[:L] if users else self.Ul[1:]                                                    # :174-180
         segs += [(src_layers[l - 1], layers[l], None, l == L) for l in range(1, L + 1)]
         op.apply(segs)
         ops.gather_rows(E, t(kn, np.int32), layers[0])                          # known -> E row, -1 -> zeros
-        out = new(m, d)
-        ops.fuse_fwd(layers, sides, self._side_coefs(), out)                                                                # :185-197
-        return out
+        return layers, F, prof, rs
 
     def _fold_in_sources(self, users, R):
         """Bring what a fold-in reads up to date: Pi on the items of R (users), or P_usr (items).  This engine's forward projects

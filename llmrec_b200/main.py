@@ -564,6 +564,20 @@ class Trainer(object):
                                        histories=histories, new_items=new_items)
         return recommend.run_rerank(self._current_model(), job)
 
+    def explain(self, items, users=None, histories=None, new_items=None, top=None):
+        """-> recommend.Explanation on the device: why this model scores each query's targets as it does.  Each score <U[u], I[i]> splits
+        exactly into one term per (history item, channel) -- channels "id", "image", "text", "profile" and one per attribute key (only
+        "id" without side features) -- plus `own` (the user's ID embedding) and `last` (the softmax layer l = L), which are not linear in
+        the history.  items: each query's targets, in the forms `rerank` takes for candidates (`ids` from `recommend` goes straight in;
+        -1 = padding, whose outputs are zeros).  Queries as in `recommend`: trained users (default every user, with one target row per
+        user), whose history is their training row, or `histories` folded in, `users` then naming each history's trained id (or -1: no
+        ID embedding, own = 0).  new_items: user lists of items added after training; target n_items + j is the j-th.  top: None, or N
+        in 1..64 for each target's N history items with the largest summed contribution.  Every argument is checked before anything
+        runs; the outputs are exact fp32, the same bits whatever else is in the call."""
+        job = recommend.prepare_explain(self.hot, self.graph.rowptr_u, self.graph.col_u, items, users=users, histories=histories,
+                                        new_items=new_items, top=top)
+        return recommend.run_explain(self._current_model(), job)
+
     def write_rerank(self, path, candidates, K):
         """--rerank_out: every user's candidate row (`candidate_indices` layout [n_users x C]) re-ranked by this model, nothing excluded,
         top K, pickled as a CPU int64 tensor [n_users x K] to `path` (atomically, as `write_candidates`)."""

@@ -622,6 +622,40 @@ def rerank(U, I, qrow, cand_rowptr, cand_col, mask_rowptr, mask_col, K):
     return idx, val
 
 
+EXPLAIN_MAX_TOP = 64       # LLMREC_EXPLAIN_MAX_TOP: the selection width of llmrec_explain_f32
+
+
+def explain(own_src, last_src, side_usr, side_src, coefs, id_src, I, qrow, su, hist_rowptr, hist_col, targets, n_layers, top=0):
+    """Exact split of <U[qrow[b]], I[targets[b, p]]> over query b's history (llmrec_explain_f32): own_src / last_src = Ul[0] / Ul[L] and
+    side_usr = the fused side rows of the user side, indexed by qrow; side_src = their item-side sources and id_src = Il[0 .. L-2], indexed
+    by history id; su fp32 [m] the queries' row scales; hist_rowptr / hist_col an int32 CSR of ascending history ids; targets int32
+    [m x P] (-1 = padding).  -> (contrib fp32 [P * nnz x (1 + n_side)], own fp32 [m x P], last fp32 [m x P], top_ids int32 [m x P x top]
+    or None, top_vals fp32 or None)."""
+    for t in [own_src, last_src, I] + list(side_usr) + list(side_src) + list(id_src):
+        _mat(t)
+    m, P = int(targets.shape[0]), int(targets.shape[1])
+    if len(side_usr) != len(side_src) or len(coefs) != len(side_usr) or int(su.numel()) != m or int(qrow.numel()) != m:
+        raise ValueError("explain: one user-side row, one source and one coefficient per side term; one qrow and su per query")
+    nnz, dev = int(hist_col.numel()), I.device
+    C_ = 1 + len(side_usr)
+    contrib = torch.empty((P * nnz, C_), dtype=torch.float32, device=dev)
+    own = torch.empty((m, P), dtype=torch.float32, device=dev)
+    last = torch.empty((m, P), dtype=torch.float32, device=dev)
+    top = int(top or 0)
+    tids = torch.empty((m, P, top), dtype=torch.int32, device=dev) if top else None
+    tvals = torch.empty((m, P, top), dtype=torch.float32, device=dev) if top else None
+    if su.dtype != torch.float32 or not su.is_cuda or not su.is_contiguous():
+        raise ValueError("explain: su needs a contiguous CUDA fp32 vector")
+    cf = (C.c_float * max(1, len(coefs)))(*[float(c) for c in coefs])
+    N.check(N.lib().llmrec_explain_f32(_p(own_src), _ld(own_src), _p(last_src), _ld(last_src), _ptr_table(side_usr), _ld_table(side_usr),
+                                        _ptr_table(side_src), _ld_table(side_src), cf, len(side_usr), _ptr_table(id_src), _ld_table(id_src),
+                                        len(id_src), _p(I), _ld(I), int(I.shape[0]), int(I.shape[1]), int(n_layers), _p(_i32(qrow)), _p(su), m,
+                                        _p(_i32(hist_rowptr)), _p(_i32(hist_col)), _p(_i32(targets.reshape(-1), "targets")), P, _p(contrib),
+                                        _p(own), _p(last), top, _p(tids), _p(tvals), _stream()), "explain")
+    _count(2 if top else 1)
+    return contrib, own, last, tids, tvals
+
+
 def topk_hits(idx, users, truth_rowptr, truth_col):
     hits = torch.empty(idx.shape, dtype=torch.uint8, device=idx.device)
     N.check(N.lib().llmrec_topk_hits(_p(_i32(idx)), idx.shape[0], idx.shape[1], _p(_i32(users)), _p(_i32(truth_rowptr)), _p(_i32(truth_col)),

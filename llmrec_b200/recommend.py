@@ -12,6 +12,10 @@ output file.
 argument of `ops.score_topk_among` (llmrec_score_topk_among_f32, the same kernels with the catalog given by ids), and the caller's rows
 are merged with the rows of `exclude` on the device (`merge_rows`).
 
+Explanations (`explain`) split scores exactly over the query's history items and the model's channels with `ops.explain`
+(llmrec_explain_f32), reading the per-row operands of the user side: the forward's rows for trained users, `HotPath.fold_in_operands`
+for histories.
+
 Scores of given (user, item) pairs are `ops.score_pairs` (llmrec_score_pairs_f32) and re-ranking of given candidate lists is
 `ops.rerank` (llmrec_rerank_f32, K <= 1024): the same sequential fp32 chain as score_topk's returned scores, so the bits agree, and the
 same mask rows (`exclusion_mask`) for exclude="train".
@@ -464,3 +468,115 @@ def write_candidates(path, ids):
             os.unlink(tmp)
         raise
     return path
+
+
+# ---- explanations ---------------------------------------------------------------------------------------------------------------
+def channels(engine):
+    """The channels an explanation splits a score over: "id" (the ID layers l = 1..L-1), then the side terms of the fusion in its
+    order -- "image", "text", "profile" and one per attribute key (SideLayout.fused)."""
+    return ["id"] + (["image", "text", "profile"] + list(engine.keys) if engine.has_feats else [])
+
+
+def check_top(top):
+    if top is not None and (isinstance(top, bool) or not isinstance(top, (int, np.integer)) or not 1 <= int(top) <= ops.EXPLAIN_MAX_TOP):
+        raise ValueError(f"top = {top!r}: explanations select the top 1..{ops.EXPLAIN_MAX_TOP} history items per target, or None")
+    return None if top is None else int(top)
+
+
+class Explanation:
+    """The result of `explain` (tensors on the engine's device; m queries, P targets each, C channels):
+    channels: the C channel names.  hist_rowptr int64 [m+1], hist int64 [nnz]: each query's history ids (ascending, repeats collapsed).
+    contrib fp32 [P * nnz x C]: query q's block, rows P * hist_rowptr[q] .. P * hist_rowptr[q+1], is [P x H_q x C] (target, history item,
+    channel).  own, last fp32 [m x P]: the user's own ID layer and the softmax layer l = L.  top_ids int64 / top_vals fp32 [m x P x N]:
+    with top=N, each target's N history items with the largest summed contribution (ties to the lowest id; -1 / -inf past the history;
+    a padding target -1 / 0); else None.  targets int64 [m x P]: the targets, -1 = padding (whose outputs are zeros)."""
+
+    def __init__(self, channels, hist_rowptr, hist, contrib, own, last, top_ids, top_vals, targets):
+        self.channels, self.hist_rowptr, self.hist, self.contrib = list(channels), hist_rowptr, hist, contrib
+        self.own, self.last, self.top_ids, self.top_vals, self.targets = own, last, top_ids, top_vals, targets
+        self._rp = hist_rowptr.cpu().tolist()
+
+    def __len__(self):
+        return len(self._rp) - 1
+
+    def of(self, q):
+        """Query q's views: dict(targets [P], hist [H], contrib [P x H x C], own [P], last [P], top_ids / top_vals [P x N] or None)."""
+        if not 0 <= q < len(self):
+            raise IndexError(f"query {q} of {len(self)}")
+        a, b = self._rp[q], self._rp[q + 1]
+        P = int(self.own.shape[1])
+        return dict(targets=self.targets[q], hist=self.hist[a:b], contrib=self.contrib[P * a:P * b].view(P, b - a, len(self.channels)),
+                    own=self.own[q], last=self.last[q], top_ids=None if self.top_ids is None else self.top_ids[q],
+                    top_vals=None if self.top_vals is None else self.top_vals[q])
+
+
+def prepare_explain(engine, train_rowptr, train_col, items, users=None, histories=None, new_items=None, top=None):
+    """Every check of `explain`, and its host-side inputs, before anything is launched: -> a dict for `run_explain`."""
+    check_engine(engine)
+    Rn = new_items_csr(new_items, engine.nu)
+    n = engine.ni + (0 if Rn is None else Rn.shape[0])
+    top = check_top(top)
+    rp, col = candidates_csr(items, n)
+    m = rp.numel() - 1
+    if histories is None and users is None and m != engine.nu:
+        raise ValueError(f"items: {m} rows; without `users` (or `histories`) there is one row per trained user ({engine.nu})")
+    R, rows, hrp, hcol, kn = _queries(engine, train_rowptr, train_col, users, histories)
+    if len(rows) != m:
+        raise ValueError(f"items: {m} rows for {len(rows)} " + ("users" if R is None else "histories"))
+    dev = engine.E_u.device
+    lens = rp[1:] - rp[:-1]
+    P = int(lens.max()) if m else 0
+    targets = torch.full((m, P), -1, dtype=torch.int64)                        # ragged rows padded to the longest
+    if col.numel():
+        owner = torch.repeat_interleave(torch.arange(m), lens)
+        targets[owner, torch.arange(col.numel()) - rp[owner]] = col
+    qrow = _i32(rows, dev)
+    if R is None:                                                              # a trained user's history: its training row
+        hrp, hcol = select_rows(train_rowptr, train_col, qrow)
+    return dict(R=R, known=kn, Rn=Rn, qrow=qrow, hist_rowptr=hrp, hist_col=hcol, targets=targets.to(dev), top=top)
+
+
+def explain_args(engine, job):
+    """The positional arguments of `ops.explain` for a `prepare_explain` job, after the launches that produce them: the new items'
+    fold-in (the catalog), and the histories' fold-in operands (or, for trained users, the forward's own rows)."""
+    dev, L = engine.E_u.device, engine.L
+    I = _catalog(engine, job["Rn"])
+    R, qrow = job["R"], job["qrow"]
+    if R is None:                                                              # trained users: the forward's own rows
+        engine._fold_in_sources(True, sp.csr_matrix((qrow.numel(), engine.ni), dtype=np.float32))    # (the hoisted engine's Pi)
+        layers, F, prof = engine.Ul, engine.Fu if engine.has_feats else None, engine.prof_u if engine.has_feats else None
+        su = engine.ui.rs[qrow.long()].contiguous()
+    else:                                                                      # histories: the operands of their fold-in
+        layers, F, prof, su = engine._fold_in_operands(True, R, job["known"])
+        qrow = torch.arange(qrow.numel(), dtype=torch.int32, device=dev)
+    side_usr, side_src, coefs = [], [], []
+    if engine.has_feats:
+        side_usr, side_src, coefs = engine.sides.fused(F, prof), engine.sides.fused(engine.Pi, engine.prof_i), engine._side_coefs()
+    return (layers[0], layers[L], side_usr, side_src, coefs, engine.Il[:L - 1], I, qrow, su, job["hist_rowptr"], job["hist_col"],
+            job["targets"].to(torch.int32), L + 1, job["top"] or 0)
+
+
+def run_explain(engine, job):
+    """The launches of `explain` for a `prepare_explain` job: the new items' and histories' fold-ins, then the explanation kernel."""
+    dev = engine.E_u.device
+    m, P = job["targets"].shape
+    top, N = job["top"] is not None, job["top"] or 0
+    if m and P:
+        contrib, own, last, tids, tvals = ops.explain(*explain_args(engine, job))
+    else:                                                                      # nothing to launch
+        contrib = torch.zeros((0, len(channels(engine))), dtype=torch.float32, device=dev)
+        own, last = (torch.zeros((m, P), dtype=torch.float32, device=dev) for _ in range(2))
+        tids, tvals = torch.full((m, P, N), -1, dtype=torch.int32, device=dev), torch.zeros((m, P, N), dtype=torch.float32, device=dev)
+    return Explanation(channels(engine), job["hist_rowptr"].long(), job["hist_col"].long(), contrib, own, last,
+                       tids.long() if top else None, tvals if top else None, job["targets"])
+
+
+def explain(engine, train_rowptr, train_col, items, users=None, histories=None, new_items=None, top=None):
+    """Explain scores of a model whose last full `forward()` is current: <U[u], I[i]> of every query u and each of its targets i, split
+    exactly over u's history items and the model's channels (`channels`), plus the user's own ID layer and the softmax layer (see
+    `Explanation` and llmrec_explain_f32).  items: each query's targets in the forms `rerank` takes for candidates (a 2-D [m x P] array
+    with -1 padding, id lists padded to the longest, or a (rowptr, col) pair); ids in [0, n_items + m_new).  users / histories /
+    new_items as in `top_k`: trained users (default every user, with one row per user) have their training rows as history, histories
+    are folded in (repeats collapse; an unknown user has no ID layer, so own = 0) and new item j is target n_items + j.  top: None, or
+    N in 1..64 to also select each target's N most helpful history items on the device.  -> Explanation."""
+    return run_explain(engine, prepare_explain(engine, train_rowptr, train_col, items, users, histories, new_items, top))
