@@ -84,8 +84,9 @@ class RowSet:                                            # llmrec_mark_neighbors
                 self._set.update(c[rp[r]:rp[r + 1]].tolist())
         self._sync()
 
-    def add_ids(self, ids):
-        self._set.update(i for i in ids.long().tolist() if i >= 0)
+    def add_ids(self, ids, n=None):                   # llmrec_mark_ids / llmrec_mark_ids_rows: ids[0 .. min(n[0], len(ids)))
+        live = ids.long() if n is None else ids.long()[:int(n[0])]
+        self._set.update(i for i in live.tolist() if i >= 0)
         self._sync()
 
     def compact(self):
@@ -132,7 +133,16 @@ def _unit(x):
     return x / x.norm(dim=1, keepdim=True).clamp_min(1e-12)           # F.normalize(x, p=2, dim=1)
 
 
-def fuse_fwd(layers, sides, coefs, out, rows=None, compact=False):      # llmrec_fuse_fwd_f32
+def _live_rows(rows, count, max_rows):
+    """rows[0 .. min(count[0], max_rows)), entries < 0 skipped (the device-count row-list forms)"""
+    mx = rows.numel() if max_rows is None else min(int(max_rows), rows.numel())
+    r = rows[:min(int(count[0]), mx)].long()
+    return r[r >= 0]
+
+
+def fuse_fwd(layers, sides, coefs, out, rows=None, compact=False, count=None, max_rows=None):   # llmrec_fuse_fwd_f32 / _rows_f32
+    if count is not None:
+        rows = _live_rows(rows, count, max_rows)
     if compact:                                          # layers at rows[b]; sides and out are compact [len(rows) x d] blocks
         r = rows.long()
         m = sum(l[r.clamp(min=0)] for l in layers) / len(layers)
@@ -167,14 +177,15 @@ def feat_reg_gram(W, b, G, h, n2, c, dW, db, loss):      # llmrec_feat_reg_gram_
     db += c * (Wh + n2 * b)
 
 
-def fuse_bwd(g, n_layers, d_layer, sides, coefs, d_sides, accumulate, rows=None):   # llmrec_fuse_bwd_f32
-    assert rows is None
+def fuse_bwd(g, n_layers, d_layer, sides, coefs, d_sides, accumulate, rows=None, count=None, max_rows=None):   # llmrec_fuse_bwd_f32 / _rows_f32
+    assert rows is None or count is not None
+    r = slice(None) if count is None else _live_rows(rows, count, max_rows)     # the row-list form writes the listed rows only
     if d_layer is not None:
-        d_layer.copy_(g / n_layers)
+        d_layer[r] = g[r] / n_layers
     for x, c, dx in zip(sides, coefs, d_sides):
-        y = _unit(x)
-        t = c * (g - y * (y * g).sum(1, keepdim=True)) / x.norm(dim=1, keepdim=True).clamp_min(1e-12)
-        dx.copy_(dx + t if accumulate else t)
+        y = _unit(x[r])
+        t = c * (g[r] - y * (y * g[r]).sum(1, keepdim=True)) / x[r].norm(dim=1, keepdim=True).clamp_min(1e-12)
+        dx[r] = dx[r] + t if accumulate else t
 
 
 def proj_fwd_group(problems, d, mode=0):                 # llmrec_proj_fwd_group_f32
@@ -285,24 +296,23 @@ class AdamW:                                             # llmrec_adamw_advance 
         self._update(self.params[i], grad, self.m[i], self.v[i])
 
     def _update(self, p, g, m, v):
-        b1, b2 = self.betas
-        p.mul_(1 - self.lr * self.wd)
-        m.mul_(b1).add_(g, alpha=1 - b1)
-        v.mul_(b2).addcmul_(g, g, value=1 - b2)
-        denom = (v.sqrt() / (1 - b2 ** self.t) ** 0.5).add_(self.eps)
-        p.addcdiv_(m, denom, value=-self.lr / (1 - b1 ** self.t))
+        """adam1 of csrc/adamw.cu: fp32 hyper-parameters (1 - beta formed from fp32 beta), the step size and bias correction the
+        advance kernel forms in double, rounded to fp32"""
+        f = lambda x: torch.tensor(x, dtype=torch.float32)
+        b1, b2, eps = f(self.betas[0]), f(self.betas[1]), f(self.eps)
+        step = f(self.lr / (1 - self.betas[0] ** self.t))
+        bc2s = f((1 - self.betas[1] ** self.t) ** 0.5)
+        p.mul_(f(1) - f(self.lr) * f(self.wd))
+        m.add_((1 - b1) * (g - m))
+        v.copy_(v * b2 + (1 - b2) * g * g)
+        p.sub_(step * (m / (v.sqrt() / bc2s + eps)))
 
     def step(self, grads, row_masks=None):
         self.t += 1
-        b1, b2 = self.betas
         if row_masks is not None:                        # llmrec_adamw_step_rows_f32: g is read on the flagged rows only
             grads = [g if mk is None else torch.where(_bits(mk, g.shape[0])[:, None], g, torch.zeros_like(g)) for g, mk in zip(grads, row_masks)]
         for p, g, m, v in zip(self.params, grads, self.m, self.v):
-            p.mul_(1 - self.lr * self.wd)
-            m.mul_(b1).add_(g, alpha=1 - b1)
-            v.mul_(b2).addcmul_(g, g, value=1 - b2)
-            denom = (v.sqrt() / (1 - b2 ** self.t) ** 0.5).add_(self.eps)
-            p.addcdiv_(m, denom, value=-self.lr / (1 - b1 ** self.t))
+            self._update(p, g, m, v)
 
 
 def install():

@@ -35,6 +35,8 @@ wrong emulation (a term dropped or doubled, a wrong tie rule, an off-by-one chun
 family is printed at the end of the module (run with -s)."""
 import ctypes as C
 import math
+import os
+import sys
 import zlib
 from fractions import Fraction
 
@@ -43,12 +45,13 @@ import pytest
 import scipy.sparse as sp
 import torch
 
+sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+from fp64_bounds import RATIOS, U, adamw_ref, check, passes, ratio_of, state_ok  # noqa: E402,F401
+
 gpu = pytest.mark.gpu
 cuda = "cuda"
 
-U = 2.0 ** -24
 EPS = 1e-12
-RATIOS = {}
 
 
 @pytest.fixture(scope="module", autouse=True)
@@ -56,28 +59,6 @@ def _report_ratios():
     yield
     if RATIOS:
         print("\nlargest error / bound per family: " + ", ".join(f"{k} {v:.3g}" for k, v in sorted(RATIOS.items())))
-
-
-def ratio_of(got, y, bound):
-    err = np.abs(np.asarray(got, np.float64) - y)
-    return np.divide(err, bound, out=np.where(err == 0, 0.0, np.inf), where=bound > 0)
-
-
-def passes(got, y, bound):
-    """every element within its bound (a NaN fails)"""
-    return bool(np.all(ratio_of(got, y, bound) <= 1.0))
-
-
-def check(got, y, bound, family, what=""):
-    got = got.detach().double().cpu().numpy() if isinstance(got, torch.Tensor) else np.asarray(got, np.float64)
-    y, bound = np.broadcast_to(y, got.shape), np.broadcast_to(bound, got.shape)
-    assert np.isfinite(got).all(), f"{what}: {int((~np.isfinite(got)).sum())} non-finite outputs (unwritten, or a NaN row was read)"
-    ratio = ratio_of(got, y, bound)
-    RATIOS[family] = max(RATIOS.get(family, 0.0), float(ratio.max(initial=0.0)))
-    if ratio.size and ratio.max() > 1.0:
-        k = np.unravel_index(np.argmax(ratio), ratio.shape)
-        raise AssertionError(f"{what}: {int((ratio > 1).sum())} elements beyond the fp64 bound; worst at {k}: got {got[k]!r}, "
-                             f"want {y[k]!r}, error {abs(got[k] - y[k]):.3g} > bound {bound[k]:.3g}")
 
 
 def same_bits(a, b):
@@ -651,25 +632,6 @@ def test_sqnorm_grad_matches_fp64(with_g, acc):
 # =================================================================================================================================
 # 3. AdamW
 # =================================================================================================================================
-def adamw_ref(p, g, m, v, t, lr, b1, b2, eps, wd):
-    """one AdamW step in fp64 from fp32 state -> [(p', bound), (m', bound), (v', bound)]"""
-    f = lambda z: float(np.float32(z))
-    b1f, b2f, epsf = f(b1), f(b2), f(eps)
-    decay = 1.0 - f(lr) * f(wd)
-    step, bc2s = lr / (1.0 - b1 ** t), math.sqrt(1.0 - b2 ** t)
-    p, g, m, v = (a.astype(np.float64) for a in (p, g, m, v))
-    p1 = p * decay
-    m1 = m + (1 - b1f) * (g - m)
-    v1 = v * b2f + (1 - b2f) * g * g
-    den = np.sqrt(v1) / bc2s + epsf
-    upd = step * m1 / den
-    p2 = p1 - upd
-    bm = 8 * U * (np.abs(m) + (1 - b1f) * (np.abs(g) + np.abs(m)))
-    bv = 8 * U * (v * b2f + (1 - b2f) * g * g)
-    bp = 2 * U * (2 * np.abs(p1) + np.abs(p2)) + step / den * bm + 24 * U * np.abs(upd)
-    return [(p2, bp), (m1, bm), (v1, bv)]
-
-
 def adamw_emul(p, g, m, v, t, lr, b1, b2, eps, wd, wrong=None):
     """fp32 adam1 of the kernel; wrong: 'no_bc2' | 'step_t_minus_1' | 'skip' (the element is not updated)"""
     f = np.float32
@@ -702,15 +664,6 @@ def test_adamw_bound_accepts_fp32_and_rejects_wrong_steps(t):
             continue                                           # both bias corrections are 1 to within rounding by then
         got = adamw_emul(p, g, m, v, t, *hp, wrong=wrong)
         assert (ratio_of(got[0], *refs[0]) > 1).mean() > 0.5, wrong
-
-
-def state_ok(st, t, lr, b1, b2):
-    """the device's step size lr / (1 - b1^t) and sqrt(1 - b2^t) against Python's, to a few double ulp of pow, amplified by the
-    cancellation in 1 - b^t"""
-    e = 2.0 ** -52
-    ok1 = abs(st[1] - lr / (1 - b1 ** t)) <= st[1] * 4 * e * (b1 ** t / (1 - b1 ** t) + 2)
-    ok2 = abs(st[2] - math.sqrt(1 - b2 ** t)) <= st[2] * 4 * e * (b2 ** t / (1 - b2 ** t) + 2)
-    return ok1 and ok2
 
 
 ADAM_NUMELS = [1, 2, 3, 4, 5, 6, 7, 9, 1023, 1025, 1026, 1027, 4096, 4097, 33, 64, 65, 130, 131, 100003]   # 20 tensors: two launches
