@@ -2,9 +2,9 @@
 neighbours) on one H100.
 
     python bench_recommend.py [--reps 3] [--syn_users 131072] [--syn_histories 8192] [--syn_items 65536] [--syn_scale 1.0]
-                              [--pairs 1048576] [--legs rerank,score_pairs,explain]
+                              [--pairs 1048576] [--legs rerank,score_pairs,explain,diversify]
 
-Nine legs per workload, each timed end to end on the host clock between device synchronises (median of --reps calls after one
+Ten legs per workload, each timed end to end on the host clock between device synchronises (median of --reps calls after one
 warm-up call):
   known         trained users scored from U with their training items excluded (exclude="train"), K = 10; users/s
   fold_in       held-out histories folded in (HotPath.fold_in) and scored, exclude="train", K = 10; users/s
@@ -24,6 +24,12 @@ warm-up call):
                 (llmrec_explain_f32, all queries in one launch, between CUDA events, median of 5 windows of 20 launches) and reports
                 it as GB/s of gathered rows: per query its 10 target rows, its two user rows and, per history item, the n_id + n_side
                 source rows (4*d bytes each)
+  diversify     diversified lists, lambda = 0.5, K = 10 (Trainer.recommend / recommend.top_k / recommend.rerank with diversity=):
+                every user's (synthetic: --syn_users users') pick from the top-64 pool of `recommend`, and at the synthetic shape also
+                from the re-ranked pool of 200 random candidates; queries/s.  Also times the kernel alone on the same pools
+                (llmrec_diversify_f32, all queries in one launch, between CUDA events, median of 5 windows of 20 launches) and reports,
+                for lambda = 1, 0.7 and 0.5, the lists' mean pairwise cosine of the normalised item rows and their mean score (lambda = 1
+                is the plain top-10 of the pool)
 Every call includes the full eval forward a recommendation starts with.  The rerank and score_pairs legs also time their kernel alone
 (llmrec_rerank_f32 / llmrec_score_pairs_f32 between CUDA events, median of 5 windows of 20 launches) and report it as GB/s of gathered
 rows: 4*d bytes per candidate row plus 4 per id (pairs: two rows and two ids), against the size of I (L2-resident at netflix,
@@ -190,6 +196,39 @@ def _explain_leg(hp, rowptr, col, ids, e2e, users, reps):
     return leg
 
 
+def _list_quality(X, ids, vals, block=8192):
+    """mean cosine over the ordered pairs of distinct positions inside each list (rows of the normalised X, fp32 products summed in
+    fp64) and mean score of the listed items"""
+    import torch
+    K = ids.shape[1]
+    off = ~torch.eye(K, dtype=torch.bool, device=ids.device)
+    cos, pairs = 0.0, 0
+    for s in range(0, ids.shape[0], block):
+        i = ids[s:s + block]
+        ok = i >= 0
+        R = X[i.clamp(min=0)].double()
+        pair = ok[:, :, None] & ok[:, None, :] & off
+        cos += float(torch.bmm(R, R.transpose(1, 2))[pair].sum())
+        pairs += int(pair.sum())
+    return {"mean_pairwise_cos": round(cos / max(pairs, 1), 4), "mean_score": round(float(vals[ids >= 0].double().mean()), 4)}
+
+
+def _diversify_leg(X, pool_ids, pool_vals, e2e, reps, label):
+    """One diversify measurement: end to end (`e2e()`, with its eval forward), the kernel alone on the same pools (K = 10,
+    lambda = 0.5), and the lists' quality at lambda = 1, 0.7 and 0.5"""
+    from llmrec_b200 import ops
+    n_q, P = (int(x) for x in pool_ids.shape)
+    leg = _leg("diversify", n_q, e2e, reps, unit="queries", label=label)
+    k = _kernel(lambda: ops.diversify(X, pool_ids, pool_vals, 10, 0.5))
+    quality = {str(lam): _list_quality(X, *ops.diversify(X, pool_ids, pool_vals, 10, lam)[:2]) for lam in (1.0, 0.7, 0.5)}
+    leg.update(pool=P, K=10, lam=0.5, kernel_s=round(k, 7), kernel_queries_per_s=round(n_q / k, 1),
+               kernel_GFMA_per_s=round(n_q * 9 * P * int(X.shape[1]) / k / 1e9, 1), quality=quality)
+    sys.stderr.write(f"  {label + ' kern':13s} {n_q:9d} queries  {k * 1e3:9.3f} ms       {n_q / k:12.0f} queries/s  pool {P}\n")
+    for lam, q in quality.items():
+        sys.stderr.write(f"    lambda {lam}: mean pairwise cos {q['mean_pairwise_cos']:.4f}, mean score {q['mean_score']:.4f}\n")
+    return leg
+
+
 def netflix(a, tmp):
     import numpy as np
     tr, gen, args = bench.make_trainer("netflix", types.SimpleNamespace(proj_mode=a.proj_mode, host_sampler="native", graph=1))
@@ -215,6 +254,12 @@ def netflix(a, tmp):
     if not ONLY or "explain" in ONLY:
         ids, _ = tr.recommend(K=10, exclude="train")
         res["explain"] = _explain_leg(tr._current_model(), tr.graph.rowptr_u, tr.graph.col_u, ids, lambda t: tr.explain(t), None, a.reps)
+    if not ONLY or "diversify" in ONLY:
+        from llmrec_b200 import ops
+        p_ids, p_vals = tr.recommend(K=64, exclude="train")
+        X = ops.row_normalize(tr._current_model().I)
+        res["diversify"] = _diversify_leg(X, p_ids, p_vals, lambda: tr.recommend(K=10, exclude="train", diversity=0.5, pool=64), a.reps,
+                                          "diversify")
     del tr, gen
     return res
 
@@ -303,6 +348,26 @@ def synthetic(a, tmp):
         hp.forward()
         ids, _ = recommend.top_k(hp, g.rowptr_u, g.col_u, users=users, K=10, exclude="train", mode=a.score_mode)
         res["explain"] = _explain_leg(hp, g.rowptr_u, g.col_u, ids, explain, users, a.reps)
+    if not ONLY or "diversify" in ONLY:
+        from llmrec_b200 import ops
+
+        def div_known():
+            hp.forward()
+            recommend.top_k(hp, g.rowptr_u, g.col_u, users=users, K=10, exclude="train", mode=a.score_mode, diversity=0.5, pool=64)
+
+        cand200 = torch.randint(0, ni, (n, 200), device=dev, generator=torch.Generator(device=dev).manual_seed(1))
+
+        def div_rerank():
+            hp.forward()
+            recommend.rerank(hp, g.rowptr_u, g.col_u, cand200, users=users, K=10, diversity=0.5, pool=200)
+
+        hp.forward()
+        X = ops.row_normalize(hp.I)
+        p_ids, p_vals = recommend.top_k(hp, g.rowptr_u, g.col_u, users=users, K=64, exclude="train", mode=a.score_mode)
+        res["diversify"] = _diversify_leg(X, p_ids, p_vals, div_known, a.reps, "diversify")
+        r_ids, r_vals = recommend.rerank(hp, g.rowptr_u, g.col_u, cand200, users=users, K=200)
+        res["diversify_rerank"] = _diversify_leg(X, r_ids, r_vals, div_rerank, a.reps, "div rerank")
+        del X, p_ids, p_vals, r_ids, r_vals, cand200
     del hp, g, params
     torch.cuda.empty_cache()
     return res

@@ -450,6 +450,27 @@ int llmrec_explain_f32(const float* own_src, int64_t ld_own, const float* last_s
                        const int32_t* hist_col, const int32_t* targets, int32_t P, float* contrib, float* own, float* last,
                        int32_t top_n, int32_t* top_ids, float* top_vals, llmrec_stream_t stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * Diversified selection: greedy maximal marginal relevance over each query's pool of scored items.
+ * Query b (< m) has the pool entries p < P: (pool_ids[b * ldp + p], pool_scores[b * ldp + p]); an id outside
+ * [0, n_catalog) (e.g. -1) is padding, at any position.  X fp32 [n_catalog x d] holds the normalised catalog
+ * rows (llmrec_row_normalize_f32), and cos(a, b) is the sequential chain c = 0; c = fmaf(X[a][j], X[b][j], c),
+ * j = 0..d-1.  mu = 1.0f - lambda (one fp32 subtract).
+ *   Round 1 picks the valid entry with the smallest key (s_p, id_p) in the order of llmrec_rerank_f32 (score
+ *   desc, id asc, NaN last).  After each pick k, every unpicked entry with id_k retires (a repeated id is
+ *   picked once) and every other one takes m_p = c when c = cos(id_p, id_k) > m_p (m_p starts at -inf; a NaN
+ *   never replaces it).  Round t >= 2 picks the smallest key (obj_p, id_p), obj_p = lambda * s_p - mu * m_p
+ *   (two fp32 multiplies and one subtract, each rounded once).  Equal keys go to the lower pool position.
+ * Writes K entries per query in pick order: out_idx int32 / out_val fp32 (the pick's s) / out_sim fp32 (the
+ * pick's m when picked; -inf for the first) [m x K], padded with -1 / -inf / -inf when fewer than K valid
+ * distinct ids remain.  Every output is one exact fp32 value, independent of the launch's grouping.
+ * 1 <= K <= P <= LLMREC_RERANK_MAX_K, 0 <= lambda <= 1.  One block per query; the pool's rows are kept in
+ * shared memory when P * (d | 1) * 4 <= 110 KiB, else read from L2 each round.  No scratch, no host sync.
+ * --------------------------------------------------------------------------------------------- */
+int llmrec_diversify_f32(const float* X, int64_t ldx, const int32_t* pool_ids, const float* pool_scores, int64_t ldp,
+                         int32_t m, int32_t P, int32_t n_catalog, int32_t d, int32_t K, float lambda,
+                         int32_t* out_idx, float* out_val, float* out_sim, llmrec_stream_t stream);
+
 /* Host-side (CPU, no GPU needed) BPR item sampler, bit-identical to Data.sample()'s numpy draws
  * (utility/load_data.py:166-187): hand over numpy's legacy MT19937 state (np.random.get_state()), get the
  * positives / rejection-sampled negatives for `users` and the advanced state back.  All pointers HOST. */

@@ -155,6 +155,8 @@ SIGNATURES = {
                                      C.POINTER(C.c_int64), C.POINTER(C.c_float), C.c_int32, C.POINTER(C.c_void_p), C.POINTER(C.c_int64), C.c_int32,
                                      c_f32p, C.c_int64, C.c_int32, C.c_int32, C.c_int32, c_i32p, c_f32p, C.c_int32, c_i32p, c_i32p, c_i32p,
                                      C.c_int32, c_f32p, c_f32p, c_f32p, C.c_int32, c_i32p, c_f32p, c_stream]),
+    "llmrec_diversify_f32": (C.c_int, [c_f32p, C.c_int64, c_i32p, c_f32p, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
+                                       C.c_float, c_i32p, c_f32p, c_f32p, c_stream]),
     "llmrec_host_sample_items":(C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]),
     "llmrec_host_sample_batch": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32,
                                            C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32,

@@ -491,7 +491,8 @@ class Trainer(object):
             self.hot.forward()
         return self.hot
 
-    def recommend(self, users=None, K=10, exclude="train", histories=None, new_items=None, among=None, exclude_items=None):
+    def recommend(self, users=None, K=10, exclude="train", histories=None, new_items=None, among=None, exclude_items=None, diversity=None,
+                  pool=None):
         """-> (ids int64 [m x K], scores fp32 [m x K]) on the device: each row's K best items, ties to the lowest item id, padded with
         -1 / -inf when fewer than K items are left.
         users: trained user ids (default every user).  histories: item-id lists or a (rowptr, col) pair, folded in with the trained item
@@ -504,10 +505,15 @@ class Trainer(object):
         and repeats do not matter); None ranks the whole catalog.  exclude_items: per query, item ids to leave out on top of `exclude`
         (one row per query: id lists, a (rowptr, col) pair, or a 2-D array [m x C] with -1 as padding; ids in [0, n_items + m)); it
         only hides items, the scores are unchanged.  Returned ids are catalog ids either way.
-        K: 1..64, at most the catalog size and at most the number of distinct ids in `among`.  Every argument is checked before
-        anything runs.  --proj_mode picks the scoring mode."""
+        K: 1..64, at most the catalog size and at most the number of distinct ids in `among`.
+        diversity: None, or lambda in [0, 1] for a diversified list: the K items are picked greedily from the row's own top-`pool` list,
+        first the best-scored, then each time the item with the largest lambda * score - (1 - lambda) * (its largest cosine to an item
+        already picked), cosines those of `similar_items` (recommend.diversify); rows come back in pick order with their scores.
+        lambda = 1 gives the first K of the pool.  pool: K..64, default the smallest of 64 and the number of rankable ids.
+        Every argument is checked before anything runs.  --proj_mode picks the scoring mode."""
         job = recommend.prepare_top_k(self.hot, self.graph.rowptr_u, self.graph.col_u, users=users, K=K, exclude=exclude,
-                                      histories=histories, new_items=new_items, among=among, exclude_items=exclude_items)
+                                      histories=histories, new_items=new_items, among=among, exclude_items=exclude_items,
+                                      diversity=diversity, pool=pool)
         hot = self._current_model()
         mode = ops.SCORE_MODE.get(getattr(self.args, "proj_mode", "3xtf32"), 0)
         return recommend.run_top_k(hot, job, mode)
@@ -552,16 +558,18 @@ class Trainer(object):
         u, i = recommend.check_pairs(users, items, self.n_users, self.n_items + (0 if Rn is None else Rn.shape[0]))
         return recommend.score_pairs(self._current_model(), u, i, new_items=Rn)
 
-    def rerank(self, candidates, users=None, K=None, exclude="none", histories=None, new_items=None):
+    def rerank(self, candidates, users=None, K=None, exclude="none", histories=None, new_items=None, diversity=None, pool=None):
         """-> (ids int64 [m x K], scores fp32 [m x K]) on the device: each query's candidate list ordered by this model, the K best by
         (score desc, id asc), padded with -1 / -inf.  candidates: a sequence of item-id lists, a (rowptr, col) pair, or a 2-D integer
         tensor / ndarray [m x C] (the `candidate_indices` layout; -1 = padding); ids in [0, n_items + len(new_items)).  Queries as in
         `recommend`: trained users (default every user, when there is one candidate row per user) or `histories` folded in, `users` then
         naming each history's trained id (or -1).  Repeated ids are kept once.  exclude: "none" (default: a given shortlist is not thinned)
         or "train" (drops what `recommend` masks).  K: 1..1024, None = the longest surviving row.  Scores are exact fp32 in every
-        --proj_mode, bit-identical to `recommend`'s for the same (user, item)."""
+        --proj_mode, bit-identical to `recommend`'s for the same (user, item).
+        diversity / pool: a diversified list as for `recommend`, picked from each row's own re-ranked top-`pool` list; pool: K..1024,
+        default the smallest of 1024 and the longest surviving row (at least K); K=None then means K = pool."""
         job = recommend.prepare_rerank(self.hot, self.graph.rowptr_u, self.graph.col_u, candidates, users=users, K=K, exclude=exclude,
-                                       histories=histories, new_items=new_items)
+                                       histories=histories, new_items=new_items, diversity=diversity, pool=pool)
         return recommend.run_rerank(self._current_model(), job)
 
     def explain(self, items, users=None, histories=None, new_items=None, top=None):
@@ -584,11 +592,11 @@ class Trainer(object):
         ids, _ = self.rerank(candidates, K=K)
         return recommend.write_candidates(path, ids)
 
-    def write_candidates(self, path, K=10, among=None):
+    def write_candidates(self, path, K=10, among=None, diversity=None, pool=None):
         """--candidates_out: the top-K of every user over the whole catalog, or over the item ids `among` (--candidates_among), nothing
-        excluded (torch.topk(U . I^T, k=K) of the reference's stage 1), pickled as a CPU int64 tensor [n_users x K] to `path`
-        (atomically)."""
-        ids, _ = self.recommend(K=K, exclude="none", among=among)
+        excluded (torch.topk(U . I^T, k=K) of the reference's stage 1), or with `diversity` (--candidates_diversity, --candidates_pool) the
+        diversified K of `recommend`, pickled as a CPU int64 tensor [n_users x K] to `path` (atomically)."""
+        ids, _ = self.recommend(K=K, exclude="none", among=among, diversity=diversity, pool=pool)
         return recommend.write_candidates(path, ids)
 
     # ---- training loop (main.py:189-326) -----------------------------------------------------------------
@@ -680,7 +688,8 @@ def main(argv=None):
     rerank_in, rerank_k = check_rerank_flags(args, trainer)
     ret = trainer.evaluate() if args.eval_only else trainer.train()
     if args.candidates_out:                                           # from the model in memory when the run ends
-        trainer.write_candidates(args.candidates_out, args.candidates_k, among=cand_among)
+        trainer.write_candidates(args.candidates_out, args.candidates_k, among=cand_among, diversity=args.candidates_diversity,
+                                 pool=args.candidates_pool)
         trainer.logger.logging("candidates: top-%d of %d users written to %s" % (args.candidates_k, trainer.n_users, args.candidates_out))
     if rerank_in is not None:
         trainer.write_rerank(args.rerank_out, rerank_in, rerank_k)
@@ -690,18 +699,26 @@ def main(argv=None):
 
 
 def check_candidates_flags(args, n_items):
-    """--candidates_out / --candidates_k / --candidates_among, checked before the first training step -> the ids of --candidates_among
-    (int64 CPU, sorted, distinct), or None."""
+    """--candidates_out / --candidates_k / --candidates_among / --candidates_diversity / --candidates_pool, checked before the first
+    training step -> the ids of --candidates_among (int64 CPU, sorted, distinct), or None."""
     among_path = getattr(args, "candidates_among", None)
+    lam, pool = getattr(args, "candidates_diversity", None), getattr(args, "candidates_pool", None)
     if among_path and not args.candidates_out:
         raise ValueError("--candidates_among restricts the --candidates_out file: give --candidates_out too")
+    for flag, v in (("--candidates_diversity", lam), ("--candidates_pool", pool)):
+        if v is not None and not args.candidates_out:
+            raise ValueError(f"{flag} diversifies the --candidates_out file: give --candidates_out too")
+    if pool is not None and lam is None:
+        raise ValueError("--candidates_pool is the pool of a diversified --candidates_out file: give --candidates_diversity too")
     if not args.candidates_out:
         return None
-    if not among_path:
-        recommend.check_k(args.candidates_k, n_items)
-        return None
-    among = recommend.read_among(among_path, n_items)
-    recommend.check_k(args.candidates_k, among.numel(), "|--candidates_among|")
+    among = None if not among_path else recommend.read_among(among_path, n_items)
+    rankable = n_items if among is None else among.numel()
+    K = recommend.check_k(args.candidates_k, n_items) if among is None else \
+        recommend.check_k(args.candidates_k, rankable, "|--candidates_among|")
+    if recommend.check_diversity(lam) is not None and pool is not None:
+        recommend.check_pool(pool, K, min(recommend.MAX_K, rankable), f"--candidates_pool: at most {recommend.MAX_K} and at most the "
+                                                                      f"{rankable} rankable ids")
     return among
 
 

@@ -656,6 +656,29 @@ def explain(own_src, last_src, side_usr, side_src, coefs, id_src, I, qrow, su, h
     return contrib, own, last, tids, tvals
 
 
+def diversify(X, pool_ids, pool_scores, K, lam):
+    """Greedy maximal-marginal-relevance selection (llmrec_diversify_f32): per query row b, K entries of the pool (pool_ids [m x P], any
+    integer dtype, ids outside [0, X.shape[0]) are padding; pool_scores fp32 [m x P]) in pick order, by lam * score - (1 - lam) * the
+    largest cosine to an earlier pick, cosines the fmaf chain over the normalised rows X.  -> (ids int64 [m x K], scores fp32 [m x K],
+    sims fp32 [m x K]: each pick's largest cosine when picked, -inf for the first), padded with -1 / -inf / -inf."""
+    _mat(X)
+    m, P = int(pool_ids.shape[0]), int(pool_ids.shape[1])
+    if tuple(pool_scores.shape) != (m, P) or pool_scores.dtype != torch.float32 or not pool_scores.is_cuda:
+        raise ValueError(f"diversify: pool_scores needs a CUDA fp32 [{m} x {P}] tensor like pool_ids, got {tuple(pool_scores.shape)} "
+                         f"{pool_scores.dtype}")
+    n = int(X.shape[0])
+    ids = pool_ids.to(X.device)
+    ids = torch.where((ids < 0) | (ids >= n), torch.full_like(ids, -1), ids).to(torch.int32).contiguous()
+    sc = pool_scores.contiguous()
+    out_i = torch.empty((m, K), dtype=torch.int32, device=X.device)
+    out_v = torch.empty((m, K), dtype=torch.float32, device=X.device)
+    out_s = torch.empty((m, K), dtype=torch.float32, device=X.device)
+    N.check(N.lib().llmrec_diversify_f32(_p(X), _ld(X), _p(ids), _p(sc), P, m, P, n, int(X.shape[1]), int(K), C.c_float(float(lam)),
+                                          _p(out_i), _p(out_v), _p(out_s), _stream()), "diversify")
+    _count()
+    return out_i.long(), out_v, out_s
+
+
 def topk_hits(idx, users, truth_rowptr, truth_col):
     hits = torch.empty(idx.shape, dtype=torch.uint8, device=idx.device)
     N.check(N.lib().llmrec_topk_hits(_p(_i32(idx)), idx.shape[0], idx.shape[1], _p(_i32(users)), _p(_i32(truth_rowptr)), _p(_i32(truth_col)),

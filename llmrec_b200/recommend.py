@@ -16,6 +16,9 @@ Explanations (`explain`) split scores exactly over the query's history items and
 (llmrec_explain_f32), reading the per-row operands of the user side: the forward's rows for trained users, `HotPath.fold_in_operands`
 for histories.
 
+Diversified lists (`diversity=`, `pool=` of `top_k` and `rerank`) take the call's own top-P list as each query's pool and select K
+of it by maximal marginal relevance with `ops.diversify` (llmrec_diversify_f32), whose cosines are those of `similar_items`.
+
 Scores of given (user, item) pairs are `ops.score_pairs` (llmrec_score_pairs_f32) and re-ranking of given candidate lists is
 `ops.rerank` (llmrec_rerank_f32, K <= 1024): the same sequential fp32 chain as score_topk's returned scores, so the bits agree, and the
 same mask rows (`exclusion_mask`) for exclude="train".
@@ -189,7 +192,7 @@ def merge_rows(a_rowptr, a_col, b_rowptr, b_col, n_catalog):
 
 
 def prepare_top_k(engine, train_rowptr, train_col, users=None, K=10, exclude="train", histories=None, new_items=None, among=None,
-                  exclude_items=None):
+                  exclude_items=None, diversity=None, pool=None):
     """Every check of `top_k`, and its host-side inputs, before anything is launched: -> a dict for `run_top_k`."""
     check_engine(engine)
     Rn = new_items_csr(new_items, engine.nu)
@@ -197,6 +200,14 @@ def prepare_top_k(engine, train_rowptr, train_col, users=None, K=10, exclude="tr
     dev = engine.E_u.device
     S = None if among is None else catalog_ids(among, n, dev)
     K = check_k(K, n) if S is None else check_k(K, S.numel(), "|among|")
+    lam = _check_pool_use(diversity, pool)
+    div = None
+    if lam is not None:                                       # the pool is the top-P list of the same call
+        rankable = n if S is None else S.numel()
+        cap = min(MAX_K, rankable)
+        P = cap if pool is None else check_pool(pool, K, cap, f"at most {MAX_K}, the scoring kernel's selection width, and at most the "
+                                                               f"{rankable} rankable ids")
+        div, K = (K, lam), P
     check_exclude(exclude)
     extra = None if exclude_items is None else candidates_csr(exclude_items, n)
     R, rows, rp, col, kn = _queries(engine, train_rowptr, train_col, users, histories)
@@ -206,7 +217,7 @@ def prepare_top_k(engine, train_rowptr, train_col, users=None, K=10, exclude="tr
     qrow = _i32(rows, dev)
     if extra is not None:                                    # per-query mask rows: query b reads mask row b, and U row b of its own copy
         rp, col = merge_rows(*select_rows(rp, col, qrow), extra[0], extra[1], n)
-    return dict(R=R, known=kn, Rn=Rn, qrow=qrow, per_query=extra is not None, mask_rowptr=rp, mask_col=col, K=K, among=S)
+    return dict(R=R, known=kn, Rn=Rn, qrow=qrow, per_query=extra is not None, mask_rowptr=rp, mask_col=col, K=K, among=S, diversify=div)
 
 
 def run_top_k(engine, job, mode=0):
@@ -217,11 +228,14 @@ def run_top_k(engine, job, mode=0):
     if job["per_query"]:
         U = U[qrow.long()].contiguous()                      # the same fp32 rows, so the same score bits
         qrow = torch.arange(qrow.numel(), dtype=torch.int32, device=qrow.device)
-    return _score(U, I, qrow, job["mask_rowptr"], job["mask_col"], job["K"], mode, job["among"])
+    ids, vals = _score(U, I, qrow, job["mask_rowptr"], job["mask_col"], job["K"], mode, job["among"])
+    if job["diversify"] is None:
+        return ids, vals
+    return diversify(engine, job["Rn"], ids, vals, *job["diversify"], I=I)[:2]
 
 
 def top_k(engine, train_rowptr, train_col, users=None, K=10, exclude="train", histories=None, mode=0, new_items=None, among=None,
-          exclude_items=None):
+          exclude_items=None, diversity=None, pool=None):
     """Top-K of a model whose last full `forward()` is current (U, I and the item side).
     users: trained user ids (default every user), scored from U's rows; with `histories` they name the trained id of each history (or
     -1), and may be omitted.  histories: a sequence of item-id lists or a (rowptr, col) pair; they are folded in (HotPath.fold_in).
@@ -232,9 +246,11 @@ def top_k(engine, train_rowptr, train_col, users=None, K=10, exclude="train", hi
     among: None (the whole catalog), or the item ids to rank (int list, ndarray or tensor; ids in [0, n_items + m), repeats collapsed);
     K is then at most the number of distinct ids.
     exclude_items: None, or one row of item ids per query (`candidates_csr` forms; -1 = padding) masked on top of what `exclude` masks.
+    diversity: None, or lambda in [0, 1]: the K items are then picked by `diversify` from the call's own top-`pool` list (K <= pool <= 64,
+    default the smallest of 64 and the number of rankable ids), in pick order.
     train_rowptr / train_col: the training rows (int32 device CSR, rows sorted), the mask of exclude="train".
     mode: ops.SCORE_MODE.  -> (ids int64 [m x K], scores fp32 [m x K]) on the engine's device; ids are catalog ids."""
-    job = prepare_top_k(engine, train_rowptr, train_col, users, K, exclude, histories, new_items, among, exclude_items)
+    job = prepare_top_k(engine, train_rowptr, train_col, users, K, exclude, histories, new_items, among, exclude_items, diversity, pool)
     return run_top_k(engine, job, mode)
 
 
@@ -335,12 +351,16 @@ def _survivors(rp, col, qrow, mrp, mcol, n):
     return int(torch.bincount(keys // n, minlength=1).max()) if keys.numel() else 0
 
 
-def prepare_rerank(engine, train_rowptr, train_col, candidates, users=None, K=None, exclude="none", histories=None, new_items=None):
+def prepare_rerank(engine, train_rowptr, train_col, candidates, users=None, K=None, exclude="none", histories=None, new_items=None,
+                   diversity=None, pool=None):
     """Every check of `rerank`, and its host-side inputs, before anything is launched: -> a dict for `run_rerank`."""
     check_engine(engine)
     Rn = new_items_csr(new_items, engine.nu)
     n = engine.ni + (0 if Rn is None else Rn.shape[0])
     K = check_rerank_k(K)
+    lam = _check_pool_use(diversity, pool)
+    if lam is not None and pool is not None:
+        pool = check_pool(pool, K or 1, ops.RERANK_MAX_K, f"at most {ops.RERANK_MAX_K}, the re-ranking kernel's selection width")
     check_exclude(exclude)
     rp, col = candidates_csr(candidates, n)
     m = rp.numel() - 1
@@ -351,12 +371,17 @@ def prepare_rerank(engine, train_rowptr, train_col, candidates, users=None, K=No
         raise ValueError(f"candidates: {m} rows for {len(rows)} " + ("users" if R is None else "histories"))
     qrow = _i32(rows, engine.E_u.device)
     mrp, mcol = exclusion_mask(engine, mrp, mcol, exclude, Rn, kn)
-    if K is None:
+    div = None
+    if lam is not None:                                       # the pool is the call's own re-ranked top-P list
+        if pool is None:
+            pool = max(min(ops.RERANK_MAX_K, _survivors(rp, col, qrow, mrp, mcol, n)), K or 1)
+        div, K = (pool if K is None else K, lam), pool
+    elif K is None:
         K = _survivors(rp, col, qrow, mrp, mcol, n)
         if K > ops.RERANK_MAX_K:
             raise ValueError(f"K = None: the longest candidate row keeps {K} ids, more than {ops.RERANK_MAX_K}; give K")
         K = max(K, 1)
-    return dict(R=R, known=kn, Rn=Rn, rowptr=rp, col=col, qrow=qrow, mask_rowptr=mrp, mask_col=mcol, K=K)
+    return dict(R=R, known=kn, Rn=Rn, rowptr=rp, col=col, qrow=qrow, mask_rowptr=mrp, mask_col=mcol, K=K, diversify=div)
 
 
 def run_rerank(engine, job):
@@ -374,17 +399,60 @@ def run_rerank(engine, job):
         idx, v = ops.rerank(U, I, qrow[s:e], brp, bcol, job["mask_rowptr"], job["mask_col"], K)
         ids[s:e].copy_(idx)
         vals[s:e].copy_(v)
-    return ids, vals
+    if job["diversify"] is None:
+        return ids, vals
+    return diversify(engine, job["Rn"], ids, vals, *job["diversify"], I=I)[:2]
 
 
-def rerank(engine, train_rowptr, train_col, candidates, users=None, K=None, exclude="none", histories=None, new_items=None):
+def rerank(engine, train_rowptr, train_col, candidates, users=None, K=None, exclude="none", histories=None, new_items=None, diversity=None,
+           pool=None):
     """Re-rank given candidate lists with a model whose last full `forward()` is current: query r's candidates (`candidates_csr` forms)
     scored against its user row by the exact fp32 chain of score_topk's returned scores, the K best by (score desc, id asc).
     users / histories / new_items / exclude as in `top_k` (exclude="train" masks exactly what `top_k` masks); queries are trained users
     (default: every user, when there are n_users candidate rows) or folded-in histories, one per candidate row.  Padding (-1), masked ids
     and repeats are dropped; a NaN score ranks after every number, a real candidate before padding.  K: 1..1024, or None for the longest
-    surviving row.  -> (ids int64 [m x K], scores fp32 [m x K]) on the engine's device, padded with -1 / -inf."""
-    return run_rerank(engine, prepare_rerank(engine, train_rowptr, train_col, candidates, users, K, exclude, histories, new_items))
+    surviving row.  diversity: None, or lambda in [0, 1]: the K items are then picked by `diversify` from the call's own re-ranked
+    top-`pool` list (K <= pool <= 1024, default the smallest of 1024 and the longest surviving row, and at least K; K=None means K = pool),
+    in pick order.  -> (ids int64 [m x K], scores fp32 [m x K]) on the engine's device, padded with -1 / -inf."""
+    job = prepare_rerank(engine, train_rowptr, train_col, candidates, users, K, exclude, histories, new_items, diversity, pool)
+    return run_rerank(engine, job)
+
+
+# ---- diversified lists -------------------------------------------------------------------------------------------------------
+def check_diversity(diversity):
+    """None, or the trade-off lambda of `diversify`: a real number in [0, 1] -> float."""
+    if diversity is None:
+        return None
+    if isinstance(diversity, (bool, np.bool_)) or not isinstance(diversity, (int, float, np.integer, np.floating)) or \
+            not 0 <= float(diversity) <= 1:
+        raise ValueError(f"diversity = {diversity!r}: lambda is a number in [0, 1] (1 ranks by score alone, 0 by dissimilarity to the "
+                         "items picked before), or None")
+    return float(diversity)
+
+
+def check_pool(pool, K, cap, why):
+    """The pool size P of a diversified call: an integer with K <= P <= cap."""
+    if isinstance(pool, (bool, np.bool_)) or not isinstance(pool, (int, np.integer)) or not K <= int(pool) <= cap:
+        raise ValueError(f"pool = {pool!r}: a diversified call picks K = {K} items from a pool of P, P in {K}..{cap} ({why})")
+    return int(pool)
+
+
+def _check_pool_use(diversity, pool):
+    lam = check_diversity(diversity)
+    if lam is None and pool is not None:
+        raise ValueError(f"pool = {pool!r}: the pool of a diversified list; give diversity too")
+    return lam
+
+
+def diversify(engine, Rn, pool_ids, pool_scores, K, lam, I=None):
+    """K items of each query's pool (ids int64 [m x P], -1 = padding; scores fp32 [m x P], the exact scores of `top_k` / `rerank`) picked
+    greedily by maximal marginal relevance (llmrec_diversify_f32): first the best-scored, then each round the item with the largest
+    lam * score - (1 - lam) * (its largest cosine to an item picked before), ties to the lowest id; a repeated id is picked once.
+    Cosines are the fmaf chain over ops.row_normalize of the catalog (the trained items, then the new items of Rn; I: that catalog when
+    the caller has it already), the cosines `similar_items` returns.  -> (ids int64 [m x K], scores fp32 [m x K], sims fp32 [m x K]:
+    each pick's largest cosine to an earlier pick, -inf for the first), padded with -1 / -inf / -inf."""
+    X = ops.row_normalize(_catalog(engine, Rn) if I is None else I)
+    return ops.diversify(X, pool_ids, pool_scores, K, lam)
 
 
 def check_pairs(users, items, n_users, n_catalog):

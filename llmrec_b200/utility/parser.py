@@ -101,6 +101,12 @@ _EXTRA = [
     ("candidates_among", dict(default=None, help="restrict --candidates_out to these items: a pickled 1-D integer tensor, ndarray or list "
                                                  "of item ids (order and repeats do not matter); each user's list is then the top "
                                                  "--candidates_k of these ids (at most their number). Needs --candidates_out")),
+    ("candidates_diversity", dict(type=float, default=None, help="diversify --candidates_out: lambda in [0, 1]; each user's list is picked "
+                                                                 "greedily from the user's top --candidates_pool items, each time the item "
+                                                                 "with the largest lambda * score - (1 - lambda) * (its largest cosine to an "
+                                                                 "item already picked); 1 = the plain top list. Needs --candidates_out")),
+    ("candidates_pool", dict(type=int, default=None, help="pool size of --candidates_diversity (--candidates_k..64, at most the number of "
+                                                          "rankable items; default the smaller of 64 and that number)")),
     ("rerank_in", dict(default=None, help="when the run ends, re-rank a candidate file with this model: a pickled 2-D integer tensor or "
                                           "ndarray [n_users x C], row u = user u's candidates, -1 = padding (the --candidates_out / "
                                           "candidate_indices format, so a file made by another model can be reordered by this one). "
