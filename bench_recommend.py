@@ -4,7 +4,7 @@ neighbours) on one H100.
     python bench_recommend.py [--reps 3] [--syn_users 131072] [--syn_histories 8192] [--syn_items 65536] [--syn_scale 1.0]
                               [--pairs 1048576] [--legs rerank,score_pairs,explain,diversify]
 
-Ten legs per workload, each timed end to end on the host clock between device synchronises (median of --reps calls after one
+Eleven legs per workload, each timed end to end on the host clock between device synchronises (median of --reps calls after one
 warm-up call):
   known         trained users scored from U with their training items excluded (exclude="train"), K = 10; users/s
   fold_in       held-out histories folded in (HotPath.fold_in) and scored, exclude="train", K = 10; users/s
@@ -30,6 +30,10 @@ warm-up call):
                 (llmrec_diversify_f32, all queries in one launch, between CUDA events, median of 5 windows of 20 launches) and reports,
                 for lambda = 1, 0.7 and 0.5, the lists' mean pairwise cosine of the normalised item rows and their mean score (lambda = 1
                 is the plain top-10 of the pool)
+  groups        group lists, K = 10, exclude="train" (Trainer.recommend_groups / recommend.top_k_groups): every user (synthetic: the
+                first 131,072 = 4 x 32,768) in random groups of 4, agg mean and min; groups/s.  Also times the kernel alone
+                (llmrec_score_topk_group_f32, all groups in one launch, between CUDA events) next to llmrec_score_topk_f32 for the same
+                members one by one, the known leg's kernel
 Every call includes the full eval forward a recommendation starts with.  The rerank and score_pairs legs also time their kernel alone
 (llmrec_rerank_f32 / llmrec_score_pairs_f32 between CUDA events, median of 5 windows of 20 launches) and report it as GB/s of gathered
 rows: 4*d bytes per candidate row plus 4 per id (pairs: two rows and two ids), against the size of I (L2-resident at netflix,
@@ -173,6 +177,34 @@ def _among_legs(U, I, mask_rowptr, mask_col, e2e, n_q, mode, reps, seed=0):
     return out
 
 
+def _groups_leg(U, I, rowptr, col, e2e, n_users, mode, reps, seed=0):
+    """The groups leg: n_users users in random groups of 4, end to end (`e2e(groups, agg)`) for agg mean and min, and the kernels alone:
+    the group kernel and the per-member score_topk launch of the same users"""
+    import numpy as np
+    import torch
+    from llmrec_b200 import ops, recommend
+    if ONLY and "groups" not in ONLY:
+        return None
+    dev, ni = U.device, int(I.shape[0])
+    perm = np.random.default_rng(seed).permutation(n_users)
+    groups = [perm[i:i + 4].tolist() for i in range(0, n_users, 4)]
+    grp_rp, grp_col = recommend.groups_csr(groups, int(U.shape[0]))
+    members = grp_col.to(dev, torch.int32)
+    mrp, mcol = recommend.group_rows(rowptr, col, members, grp_rp, ni)
+    users = members.clone()
+    out = {}
+    k_known = _kernel(lambda: ops.score_topk(U, I, users, rowptr, col, 10, mode=mode), reps=3, windows=3)
+    for agg in ("mean", "min"):
+        leg = _leg("groups", len(groups), lambda: e2e(groups, agg), reps, unit="groups", label=f"groups {agg}")
+        k = _kernel(lambda: ops.score_topk_group(U, I, grp_rp, members, None, mrp, mcol, 10, agg=agg, mode=mode), reps=3, windows=3)
+        leg.update(members=int(members.numel()), kernel_s=round(k, 7), kernel_groups_per_s=round(len(groups) / k, 1),
+                   known_kernel_s=round(k_known, 7))
+        sys.stderr.write(f"  {'kernel':13s} {len(groups):9d} groups   {k * 1e3:9.3f} ms   known kernel, same {members.numel()} users "
+                         f"{k_known * 1e3:9.3f} ms\n")
+        out[agg] = leg
+    return out
+
+
 def _explain_leg(hp, rowptr, col, ids, e2e, users, reps):
     """The explain leg: end to end (`e2e(ids)`, with its eval forward), and the kernel alone on the same queries"""
     import numpy as np
@@ -251,6 +283,8 @@ def netflix(a, tmp):
     res.update(_serving_legs(hp.U, hp.I, lambda cand: tr.rerank(cand, K=10), lambda u, i: tr.score(u, i), nu, 100, a.pairs, a.reps))
     res["among"] = _among_legs(hp.U, hp.I, tr.graph.rowptr_u, tr.graph.col_u, lambda S: tr.recommend(K=10, exclude="train", among=S), nu,
                                a.score_mode, a.reps)
+    res["groups"] = _groups_leg(hp.U, hp.I, tr.graph.rowptr_u, tr.graph.col_u, lambda gr, agg: tr.recommend_groups(gr, K=10, agg=agg), nu,
+                                a.score_mode, a.reps)
     if not ONLY or "explain" in ONLY:
         ids, _ = tr.recommend(K=10, exclude="train")
         res["explain"] = _explain_leg(tr._current_model(), tr.graph.rowptr_u, tr.graph.col_u, ids, lambda t: tr.explain(t), None, a.reps)
@@ -339,6 +373,13 @@ def synthetic(a, tmp):
 
     hp.forward()
     res["among"] = _among_legs(hp.U, hp.I, g.rowptr_u, g.col_u, among, n, a.score_mode, a.reps)
+
+    def groups(gr, agg):
+        hp.forward()
+        recommend.top_k_groups(hp, g.rowptr_u, g.col_u, gr, K=10, agg=agg, mode=a.score_mode)
+
+    hp.forward()
+    res["groups"] = _groups_leg(hp.U, hp.I, g.rowptr_u, g.col_u, groups, n, a.score_mode, a.reps)
 
     def explain(ids):
         hp.forward()

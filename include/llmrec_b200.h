@@ -382,6 +382,40 @@ int llmrec_score_topk_among_f32(const float* U, int64_t ldu, const float* I, int
                                 float* scratch, int64_t scratch_elems, llmrec_stream_t stream);
 int64_t llmrec_score_topk_among_scratch(int32_t n_batch, int32_t n_among, int32_t d, int32_t K, int32_t mode);
 
+/* Top-K for groups of users who choose together.  Group g's members are the rows
+ * members[member_rowptr_host[g] .. member_rowptr_host[g+1]) of U: 1..64 per group (64 = one wgmma M tile; a group
+ * never straddles a tile), ascending and distinct by the caller's convention (not checked; the order is
+ * the summation order of mean).  member_rowptr_host is a HOST int32 [n_groups+1] array: the tile plan is built
+ * from it and copied into the scratch from pageable memory, so unlike the other entry points this call waits
+ * for the stream's earlier work before it returns.  members is device int32.  Let s(u, i) be the sequential fp32 FMA
+ * chain of llmrec_score_pairs_f32.  The group score of item i is, by agg:
+ *   LLMREC_AGG_MEAN: the fp32 sum 0 + s(u_0, i) + s(u_1, i) + ... in member order, then one IEEE fp32
+ *                    division by the member count;
+ *   LLMREC_AGG_MIN / LLMREC_AGG_MAX: the exact minimum / maximum; a NaN member score makes it NaN.
+ * The catalog is I (among NULL, n_items rows) or the rows among[0 .. n_items) of I (STRICTLY ASCENDING,
+ * as for llmrec_score_topk_among_f32).  Mask rows are indexed by GROUP (mask_rowptr int32[n_groups+1],
+ * rows sorted ascending, NULL = no mask) and hold global ids.  out_idx int32 / out_val fp32 [n_groups x K]
+ * by (group score desc, id asc); NaN and -inf group scores are never returned; short rows padded with -1 /
+ * -inf.  K is 1..64 and <= n_items.  mode 0: the member rows are packed into 64-row tiles, every member is
+ * scored on the tensor cores (3xTF32), each group's approximate scores are aggregated by the same rule in
+ * shared memory and selected with K+16.. slack, then the candidates are rescored exactly (d in
+ * {32,64,96,128}, aligned operands; other shapes take mode 2); mode 2: exact fp32 SIMT.  Both return the
+ * same ids and bits unless two group scores closer than the TF32x3 rounding straddle rank K+16.  In mode 2
+ * a group's row does not depend on the other groups of the call; in mode 0 it does not either, unless such
+ * near ties straddle the slack (the number of catalog slices, and so of candidates per group, follows the
+ * number of tiles in the call, as for llmrec_score_topk_f32).  scratch: llmrec_score_topk_group_scratch
+ * with the same member_rowptr_host. */
+#define LLMREC_AGG_MEAN 0
+#define LLMREC_AGG_MIN 1
+#define LLMREC_AGG_MAX 2
+int llmrec_score_topk_group_f32(const float* U, int64_t ldu, const float* I, int64_t ldi,
+                                const int32_t* member_rowptr_host, const int32_t* members, int32_t n_groups,
+                                const int32_t* among, int32_t n_items, int32_t d,
+                                const int32_t* mask_rowptr, const int32_t* mask_col, int32_t K, int32_t agg,
+                                int32_t* out_idx, float* out_val, int32_t mode,
+                                float* scratch, int64_t scratch_elems, llmrec_stream_t stream);
+int64_t llmrec_score_topk_group_scratch(const int32_t* member_rowptr_host, int32_t n_groups, int32_t n_items, int32_t d, int32_t K, int32_t mode);
+
 /* hits[b,j] = 1 if out_idx[b,j] in truth row of users[b] (test_set membership, batch_test.py:30-34). */
 int llmrec_topk_hits(const int32_t* idx, int32_t n_batch, int32_t K, const int32_t* users,
                      const int32_t* truth_rowptr, const int32_t* truth_col, uint8_t* hits,

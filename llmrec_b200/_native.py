@@ -146,6 +146,9 @@ SIGNATURES = {
     "llmrec_score_topk_among_f32": (C.c_int, [c_f32p, C.c_int64, c_f32p, C.c_int64, c_i32p, C.c_int32, c_i32p, C.c_int32, C.c_int32, c_i32p,
                                               c_i32p, C.c_int32, c_i32p, c_f32p, C.c_int32, c_f32p, C.c_int64, c_stream]),
     "llmrec_score_topk_among_scratch": (C.c_int64, [C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32]),
+    "llmrec_score_topk_group_f32": (C.c_int, [c_f32p, C.c_int64, c_f32p, C.c_int64, c_i32p, c_i32p, C.c_int32, c_i32p, C.c_int32, C.c_int32,
+                                              c_i32p, c_i32p, C.c_int32, C.c_int32, c_i32p, c_f32p, C.c_int32, c_f32p, C.c_int64, c_stream]),
+    "llmrec_score_topk_group_scratch": (C.c_int64, [c_i32p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32]),
     "llmrec_topk_hits": (C.c_int, [c_i32p, C.c_int32, C.c_int32, c_i32p, c_i32p, c_i32p, C.c_void_p, c_stream]),
     "llmrec_user_auc_f32": (C.c_int, [c_f32p, C.c_int64, c_f32p, C.c_int64, c_i32p, C.c_int32, C.c_int32, C.c_int32, c_i32p, c_i32p, c_i32p, c_i32p, c_f32p, c_stream]),
     "llmrec_score_pairs_f32": (C.c_int, [c_f32p, C.c_int64, c_f32p, C.c_int64, c_i32p, c_i32p, C.c_int32, C.c_int32, c_f32p, c_stream]),

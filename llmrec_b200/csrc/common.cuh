@@ -82,6 +82,17 @@ __device__ __forceinline__ void fma4(float4& a, float w, const float4& x) {
   a.x = fmaf(w, x.x, a.x); a.y = fmaf(w, x.y, a.y); a.z = fmaf(w, x.z, a.z); a.w = fmaf(w, x.w, a.w);
 }
 
+// Group scores (llmrec_score_topk_group_f32): v = agg_start; v = agg_fold(v, s_m) for the members in ascending id; agg_end(v, n).
+// mean: the fp32 sum 0 + s_0 + s_1 + ..., then one IEEE division by n; min / max: the exact extreme, a NaN member makes it NaN
+// (fminf / fmaxf would drop the NaN).  __fadd_rn / __fdiv_rn keep nvcc from contracting or approximating them.
+__device__ __forceinline__ float agg_start(int agg) { return agg == LLMREC_AGG_MEAN ? 0.f : agg == LLMREC_AGG_MIN ? INFINITY : -INFINITY; }
+__device__ __forceinline__ float agg_fold(int agg, float v, float s) {
+  if (agg == LLMREC_AGG_MEAN) return __fadd_rn(v, s);
+  if (s != s) return s;
+  return (agg == LLMREC_AGG_MIN ? s < v : s > v) ? s : v;   // once v is NaN no comparison is true: it stays NaN
+}
+__device__ __forceinline__ float agg_end(int agg, float v, int n) { return agg == LLMREC_AGG_MEAN ? __fdiv_rn(v, (float)n) : v; }
+
 inline cudaStream_t as_stream(llmrec_stream_t s) { return reinterpret_cast<cudaStream_t>(s); }
 inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
 

@@ -19,6 +19,11 @@ int64_t proj_wgrad_tc_scratch(const llmrec_proj_wgrad_problem*, int, int, int, X
 bool score_tc_supported(int d, int K, long long ldu, long long ldi, const void* U, const void* I);
 long long score_tc_scratch(int n_batch, int n_items, int d, int K);
 int score_topk_tc(const float*, long long, const float*, long long, const int*, int, const int*, int, int, const int*, const int*, int, int*, float*, float*, long long, cudaStream_t);
+long long score_tc_group_scratch(const int* rp, int n_groups, int n_items, int d, int K);
+int score_topk_group_tc(const float*, long long, const float*, long long, const int*, const int*, int, const int*, int, int, const int*, const int*, int,
+                        int, int*, float*, float*, long long, cudaStream_t);
+int score_topk_group_simt(const float*, int64_t, const float*, int64_t, const int*, const int*, const int*, int, const int*, int, int, const int*,
+                          const int*, int, int, int*, float*, float*, int64_t, cudaStream_t);
 }  // namespace llmrec
 using namespace llmrec;
 
@@ -260,4 +265,54 @@ extern "C" int llmrec_score_topk_among_f32(const float* U, int64_t ldu, const fl
   LLMREC_CHECK_ARG(among || n_among <= 0, "score_topk_among: among is NULL");
   return score_topk(U, ldu, I, ldi, users, n_batch, among, n_among, d, mask_rowptr, mask_col, K, out_idx, out_val, mode, scratch, scratch_elems,
                     stream);
+}
+
+// ---- groups ----------------------------------------------------------------------------------------------------------------
+// mode 2: the device copy of the member CSR (rounded to 4 elements), then rows of group and member scores
+static int64_t group_rowptr_elems(int32_t n_groups) { return ((int64_t)n_groups + 1 + 3) / 4 * 4; }
+static int64_t group_simt_scratch(const int32_t* rp, int32_t n_groups, int32_t n_items) {
+  int64_t want = ((int64_t)n_groups + (rp[n_groups] - rp[0])) * n_items;
+  const int64_t cap = (int64_t)1 << 28;   // 1 GiB of fp32 scores at most; the SIMT path loops over blocks of groups
+  if (want > cap) want = (cap / n_items) * n_items;
+  if (want < 65LL * n_items) want = 65LL * n_items;   // one group of 64 members and its group row
+  return group_rowptr_elems(n_groups) + want;
+}
+static bool group_tc_shape(int32_t d, int32_t K, int32_t mode) { return mode != 2 && (d == 32 || d == 64 || d == 96 || d == 128) && K <= 64; }
+extern "C" int64_t llmrec_score_topk_group_scratch(const int32_t* member_rowptr_host, int32_t n_groups, int32_t n_items, int32_t d, int32_t K, int32_t mode) {
+  if (!member_rowptr_host || n_groups <= 0 || n_items <= 0) return 0;
+  for (int g = 0; g < n_groups; ++g)   // a malformed CSR sizes nothing; the call itself reports it
+    if (member_rowptr_host[g + 1] - member_rowptr_host[g] < 1 || member_rowptr_host[g + 1] - member_rowptr_host[g] > 64) return 0;
+  if (!group_tc_shape(d, K, mode)) return group_simt_scratch(member_rowptr_host, n_groups, n_items);
+  // the call may still take the SIMT path (leading dimensions, alignment): leave room for its smallest block (one group of 64
+  // members and its group row), not for its full 1 GiB of blocks
+  const int64_t tc = score_tc_group_scratch(member_rowptr_host, n_groups, n_items, d, K);
+  const int64_t simt_min = group_rowptr_elems(n_groups) + 65LL * n_items;
+  return tc > simt_min ? tc : simt_min;
+}
+extern "C" int llmrec_score_topk_group_f32(const float* U, int64_t ldu, const float* I, int64_t ldi, const int32_t* member_rowptr_host,
+                                           const int32_t* members, int32_t n_groups, const int32_t* among, int32_t n_items, int32_t d,
+                                           const int32_t* mask_rowptr, const int32_t* mask_col, int32_t K, int32_t agg, int32_t* out_idx,
+                                           float* out_val, int32_t mode, float* scratch, int64_t scratch_elems, llmrec_stream_t stream) {
+  LLMREC_REQUIRE_DEVICE();
+  LLMREC_CHECK_ARG(K >= 1 && K <= 64 && K <= n_items, "score_topk_group: K=%d unsupported (1..64, <= n_items = %d)", K, n_items);
+  LLMREC_CHECK_ARG(agg == LLMREC_AGG_MEAN || agg == LLMREC_AGG_MIN || agg == LLMREC_AGG_MAX, "score_topk_group: agg=%d is not "
+                   "LLMREC_AGG_MEAN / _MIN / _MAX", agg);
+  LLMREC_CHECK_ARG(n_groups >= 0 && d >= 1, "score_topk_group: bad sizes");
+  if (n_groups == 0) return 0;
+  LLMREC_CHECK_ARG(member_rowptr_host && members && member_rowptr_host[0] == 0, "score_topk_group: member CSR missing or not starting at 0");
+  for (int g = 0; g < n_groups; ++g) {
+    const int n = member_rowptr_host[g + 1] - member_rowptr_host[g];
+    LLMREC_CHECK_ARG(n >= 1 && n <= 64, "score_topk_group: group %d has %d members (1..64)", g, n);
+  }
+  cudaStream_t st = as_stream(stream);
+  if (group_tc_shape(d, K, mode) && score_tc_supported(d, K, ldu, ldi, U, I))
+    return score_topk_group_tc(U, ldu, I, ldi, member_rowptr_host, members, n_groups, among, n_items, d, mask_rowptr, mask_col, K, agg, out_idx,
+                               out_val, scratch, scratch_elems, st);
+  const int64_t head = group_rowptr_elems(n_groups);
+  LLMREC_CHECK_ARG(scratch && scratch_elems >= head + 65LL * n_items, "score_topk_group(simt): scratch too small");
+  int32_t* drp = reinterpret_cast<int32_t*>(scratch);
+  // pageable source: the copy is staged before this returns
+  LLMREC_CHECK_CUDA(cudaMemcpyAsync(drp, member_rowptr_host, ((size_t)n_groups + 1) * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+  return score_topk_group_simt(U, ldu, I, ldi, member_rowptr_host, drp, members, n_groups, among, n_items, d, mask_rowptr, mask_col, K, agg, out_idx,
+                               out_val, scratch + head, scratch_elems - head, st);
 }

@@ -32,16 +32,28 @@ __global__ void __launch_bounds__(256) score_rows_kernel(const float* __restrict
   for (int j = 0; j < d; ++j) a = fmaf(us[j], it[j], a);
   S[(int64_t)b * n_items + i] = a;
 }
-// masked items -> -inf; with `among`, a masked id outside the catalog is skipped
+// masked items -> -inf; with `among`, a masked id outside the catalog is skipped; users NULL: row b reads mask row b
 __global__ void mask_rows_kernel(const int* __restrict__ users, const int* __restrict__ rowptr, const int* __restrict__ col,
                                  const int* __restrict__ among, int n_items, float* __restrict__ S) {
   const int b = blockIdx.x;
-  const int u = users[b];
+  const int u = users ? users[b] : b;
   for (int e = rowptr[u] + threadIdx.x; e < rowptr[u + 1]; e += blockDim.x) {
     int c = col[e];
     if (among) c = catalog_pos(among, n_items, c);
     if (c >= 0 && c < n_items) S[(int64_t)b * n_items + c] = -INFINITY;
   }
+}
+// group rows of a block of groups g0 .. g0 + gridDim.y from the scores of their members (rows of Sm from member m_base on):
+// Sg[g - g0][i] = the exact group score of catalog column i (common.cuh agg_*)
+__global__ void __launch_bounds__(256) aggregate_group_rows_kernel(const float* __restrict__ Sm, const int* __restrict__ grp_rowptr, int g0,
+                                                                   int m_base, int n_items, int agg, float* __restrict__ Sg) {
+  const int g = g0 + blockIdx.y;
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n_items) return;
+  const int m0 = __ldg(grp_rowptr + g), m1 = __ldg(grp_rowptr + g + 1);
+  float v = agg_start(agg);
+  for (int m = m0; m < m1; ++m) v = agg_fold(agg, v, Sm[(int64_t)(m - m_base) * n_items + i]);
+  Sg[(int64_t)blockIdx.y * n_items + i] = agg_end(agg, v, m1 - m0);
 }
 // K rounds of block arg-max with (score desc, id asc) order; ascending catalog ids make the lowest column the lowest id
 __global__ void __launch_bounds__(256) select_topk_kernel(float* __restrict__ S, const int* __restrict__ among, int n_items, int K,
@@ -161,6 +173,32 @@ int score_topk_simt(const float* U, int64_t ldu, const float* I, int64_t ldi, co
     if (mask_rowptr) { mask_rows_kernel<<<nb, 128, 0, st>>>(users + b0, mask_rowptr, mask_col, among, n_items, scratch); LLMREC_CHECK_LAUNCH("mask_rows"); }
     select_topk_kernel<<<nb, 256, 0, st>>>(scratch, among, n_items, K, out_idx + (int64_t)b0 * K, out_val ? out_val + (int64_t)b0 * K : nullptr);
     LLMREC_CHECK_LAUNCH("select_topk");
+  }
+  return 0;
+}
+
+// groups: rp is the HOST member CSR, grp_rowptr its device copy; members are rows of U; mask rows are indexed by group.  Blocks of
+// groups whose group rows and member rows fit the scratch: member scores (score_rows_kernel), group rows, mask, selection.
+int score_topk_group_simt(const float* U, int64_t ldu, const float* I, int64_t ldi, const int* rp, const int* grp_rowptr, const int* members,
+                          int n_groups, const int* among, int n_items, int d, const int* mask_rowptr, const int* mask_col, int K, int agg,
+                          int* out_idx, float* out_val, float* scratch, int64_t scratch_elems, cudaStream_t st) {
+  const int64_t rows = scratch ? scratch_elems / n_items : 0;
+  LLMREC_CHECK_ARG(rows >= 65, "score_topk_group(simt): scratch too small (one group of 64 members needs 65 rows of %d)", n_items);
+  for (int g0 = 0; g0 < n_groups;) {
+    int g1 = g0 + 1;
+    while (g1 < n_groups && g1 + 1 - g0 <= 65535 && rp[g1 + 1] - rp[g0] <= 65535 && (g1 + 1 - g0) + (int64_t)(rp[g1 + 1] - rp[g0]) <= rows) ++g1;
+    const int ng = g1 - g0, nm = rp[g1] - rp[g0];
+    float* Sg = scratch;
+    float* Sm = scratch + (int64_t)ng * n_items;
+    dim3 grid_m((n_items + 255) / 256, nm), grid_g((n_items + 255) / 256, ng);
+    score_rows_kernel<<<grid_m, 256, d * sizeof(float), st>>>(U, ldu, I, ldi, members + rp[g0], among, n_items, d, Sm);
+    LLMREC_CHECK_LAUNCH("score_rows");
+    aggregate_group_rows_kernel<<<grid_g, 256, 0, st>>>(Sm, grp_rowptr, g0, rp[g0], n_items, agg, Sg);
+    LLMREC_CHECK_LAUNCH("aggregate_group_rows");
+    if (mask_rowptr) { mask_rows_kernel<<<ng, 128, 0, st>>>(nullptr, mask_rowptr + g0, mask_col, among, n_items, Sg); LLMREC_CHECK_LAUNCH("mask_rows"); }
+    select_topk_kernel<<<ng, 256, 0, st>>>(Sg, among, n_items, K, out_idx + (int64_t)g0 * K, out_val ? out_val + (int64_t)g0 * K : nullptr);
+    LLMREC_CHECK_LAUNCH("select_topk");
+    g0 = g1;
   }
   return 0;
 }

@@ -21,8 +21,18 @@
 //     are gathered compacted, column j of the catalog offers global id among[j] (each tile's 128 ids staged once in
 //     shared memory), and mask rows / returned ids stay global.  Ascending ids keep the merge pointer and the tie rule
 //     valid unchanged; among == NULL is the identity map (the whole of I).
+//   * groups (llmrec_score_topk_group_f32, the GROUP instantiation): the A tile holds the member rows of whole groups,
+//     packed in the order given (a tile slot plan built on the host; padding slots are zero rows).  Selection thread t
+//     owns group t of the tile: after staging, the whole CTA folds each group's member rows of the score tile into the first
+//     of them by the group rule (mean / min / max, common.cuh agg_*), and thread t runs the threshold test, mask merge
+//     pointer and heap on its group's row unchanged; mask rows and candidate rows are indexed by group.  rescore_topk_group_kernel recomputes every
+//     member's exact chain per candidate and aggregates exactly.  The slack argument carries over: a member's 3xTF32 score
+//     is within e of its exact chain, so the mean of n such scores is within e of the exact mean (up to the rounding of
+//     an fp32 sum of n terms), and min / max move by at most the largest member error -- the aggregated error is bounded
+//     by the largest member error.  Every member is scored: the tensor work equals recommending for each member.
 #include <stdlib.h>
 #include <string.h>
+#include <vector>
 #include "common.cuh"
 #include "tc_common.cuh"
 
@@ -43,10 +53,14 @@ struct ScoreParams {
   const int* among;                             // NULL, or catalog column j -> global item id among[j] (ascending)
   const int* mask_rowptr; const int* mask_col;  // train rows, columns sorted ascending
   int Kc, splits, tiles_per_split, stages;
-  int* cand_idx; float* cand_val;  // [n_batch][splits][Kc]
+  int* cand_idx; float* cand_val;  // [n_batch][splits][Kc]  (GROUP: [n_groups][splits][Kc])
+  // GROUP only (users = the members): slot r of tile t holds members[slot_pos[t * 64 + r]] (-1 = a zero row); tile t holds
+  // groups tile_g0[t] .. tile_g0[t+1]; group g's members are rows gofs[g] .. gofs[g] + n of its tile, n from grp_rowptr
+  const int* slot_pos; const int* tile_g0; const int* gofs; const int* grp_rowptr;
+  int agg;
 };
 
-template <int D>
+template <int D, bool GROUP>
 __global__ void __launch_bounds__(128, 1) score_topk_tc_kernel(const __grid_constant__ ScoreParams P) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -84,8 +98,14 @@ __global__ void __launch_bounds__(128, 1) score_topk_tc_kernel(const __grid_cons
   // A operand: gather the 64 user rows, split hi/lo
   for (int i = tid; i < SBM * (D / 4); i += 128) {
     const int r = i / (D / 4), c4 = i - r * (D / 4);
-    const int b = utile * SBM + r;
-    const float4 v = b < P.n_batch ? ldg4(P.U + (long long)P.users[b] * P.ldu + c4 * 4) : make_float4(0.f, 0.f, 0.f, 0.f);
+    float4 v;
+    if constexpr (GROUP) {
+      const int p = __ldg(P.slot_pos + utile * SBM + r);
+      v = p >= 0 ? ldg4(P.U + (long long)__ldg(P.users + p) * P.ldu + c4 * 4) : make_float4(0.f, 0.f, 0.f, 0.f);
+    } else {
+      const int b = utile * SBM + r;
+      v = b < P.n_batch ? ldg4(P.U + (long long)P.users[b] * P.ldu + c4 * 4) : make_float4(0.f, 0.f, 0.f, 0.f);
+    }
     float4 h, l;
     split4(v, h, l);
     const uint32_t off = (uint32_t)(c4 >> 3) * kTileU + sw128_off(r, c4 & 7);
@@ -95,12 +115,20 @@ __global__ void __launch_bounds__(128, 1) score_topk_tc_kernel(const __grid_cons
   fence_proxy_async_smem();
   __syncthreads();
 
-  // ===== selection state: thread t < 64 owns user row t of the tile =====
+  // ===== selection state: thread t < 64 owns user row t of the tile (GROUP: group t of the tile) =====
   const int b = utile * SBM + tid;
-  const bool live = tid < SBM && b < P.n_batch;
+  int grp = 0, r0 = tid;   // GROUP: the thread's group and the tile row of its first member
+  bool live;
+  if constexpr (GROUP) {
+    grp = __ldg(P.tile_g0 + utile) + tid;
+    live = tid < SBM && grp < __ldg(P.tile_g0 + utile + 1);
+    if (live) r0 = __ldg(P.gofs + grp);
+  } else {
+    live = tid < SBM && b < P.n_batch;
+  }
   int mp = 0, mend = 0, next_masked = 0x7fffffff;
   if (live && P.mask_rowptr) {
-    const int u = P.users[b];
+    const int u = GROUP ? grp : P.users[b];
     mp = P.mask_rowptr[u]; mend = P.mask_rowptr[u + 1];
     next_masked = mp < mend ? __ldg(P.mask_col + mp) : 0x7fffffff;
   }
@@ -197,8 +225,23 @@ __global__ void __launch_bounds__(128, 1) score_topk_tc_kernel(const __grid_cons
       tile_ids[tid] = col < P.n_items ? __ldg(P.among + col) : 0x7fffffff;
     }
     __syncthreads();
+    if constexpr (GROUP) {   // fold each group's member rows into its first row: all 128 threads, one (group, column) per step
+      const int g0 = __ldg(P.tile_g0 + utile), ng = __ldg(P.tile_g0 + utile + 1) - g0;
+#pragma unroll 1
+      for (int e = tid; e < ng * SBN; e += 128) {   // consecutive threads take consecutive columns of one group's rows
+        const int gg = g0 + e / SBN, c = e % SBN;
+        const int n = __ldg(P.grp_rowptr + gg + 1) - __ldg(P.grp_rowptr + gg);
+        if (n == 1) continue;
+        float* col = stg + __ldg(P.gofs + gg) * kStageLd + c;
+        float v = agg_start(P.agg);
+#pragma unroll 1
+        for (int m = 0; m < n; ++m) v = agg_fold(P.agg, v, col[m * kStageLd]);
+        col[0] = agg_end(P.agg, v, n);
+      }
+      __syncthreads();
+    }
     if (live) {
-      const float* srow = stg + tid * kStageLd;
+      const float* srow = stg + r0 * kStageLd;
 #pragma unroll 1
       for (int c0 = 0; c0 < SBN; c0 += 32) {
         // fast path: one compare per score builds the mask of columns that beat the current threshold
@@ -217,8 +260,9 @@ __global__ void __launch_bounds__(128, 1) score_topk_tc_kernel(const __grid_cons
     __syncthreads();   // staging free for the next tile
   }
   if (live) {
-    int* oi = P.cand_idx + ((long long)b * P.splits + split) * Kc;
-    float* ov = P.cand_val + ((long long)b * P.splits + split) * Kc;
+    const long long q = GROUP ? grp : b;
+    int* oi = P.cand_idx + (q * P.splits + split) * Kc;
+    float* ov = P.cand_val + (q * P.splits + split) * Kc;
     for (int k = 0; k < Kc; ++k) {
       const bool has = k < count;
       oi[k] = has ? HI(k) : -1;
@@ -240,6 +284,34 @@ __global__ void split_hi_lo_kernel(const float* __restrict__ X, long long ldx, c
 
 // exact fp32 rescoring of the candidates of one user + final (score desc, id asc) top-K: ONE WARP per user
 constexpr int kMaxCandPerLane = 20;   // 32 x 20 = 640 candidates (<= 6 slices x 96)
+
+// the final top-K of a warp's rescored candidates (lane-owned sc / id, id -1 = none; NaN and -inf never win): K rounds of a warp
+// arg-max by (score desc, id asc) -> out_idx[0 .. K) / out_val (may be NULL), padded with -1 / -inf
+__device__ __forceinline__ void warp_emit_topk(float (&sc)[kMaxCandPerLane], int (&id)[kMaxCandPerLane], int K, int lane, int* out_idx,
+                                               float* out_val) {
+  for (int r = 0; r < K; ++r) {
+    float best = -INFINITY; int besti = 0x7fffffff, bestq = -1;
+#pragma unroll
+    for (int q = 0; q < kMaxCandPerLane; ++q) {
+      if (id[q] >= 0 && sc[q] != -INFINITY && (sc[q] > best || (sc[q] == best && id[q] < besti))) { best = sc[q]; besti = id[q]; bestq = q; }
+    }
+    float wb = best; int wi = besti;
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      const float ov = __shfl_xor_sync(0xffffffffu, wb, o); const int oi = __shfl_xor_sync(0xffffffffu, wi, o);
+      if (ov > wb || (ov == wb && oi < wi)) { wb = ov; wi = oi; }
+    }
+    const bool ok = wi != 0x7fffffff;
+    if (lane == 0) {
+      out_idx[r] = ok ? wi : -1;
+      if (out_val) out_val[r] = ok ? wb : -INFINITY;
+    }
+    if (ok && bestq >= 0 && besti == wi) {   // the owning lane retires the winner (ids are unique per user)
+#pragma unroll
+      for (int q = 0; q < kMaxCandPerLane; ++q) if (q == bestq) id[q] = -1;
+    }
+  }
+}
 __global__ void __launch_bounds__(256) rescore_topk_kernel(const float* __restrict__ U, long long ldu, const float* __restrict__ I, long long ldi,
                                                            const int* __restrict__ users, int n_batch, int d, const int* __restrict__ cand_idx,
                                                            int n_cand, int K, int* __restrict__ out_idx, float* __restrict__ out_val) {
@@ -265,28 +337,40 @@ __global__ void __launch_bounds__(256) rescore_topk_kernel(const float* __restri
     }
     sc[q] = a; id[q] = item;
   }
-  for (int r = 0; r < K; ++r) {
-    float best = -INFINITY; int besti = 0x7fffffff, bestq = -1;
+  warp_emit_topk(sc, id, K, lane, out_idx + (long long)b * K, out_val ? out_val + (long long)b * K : nullptr);
+}
+
+// exact rescoring for groups: ONE WARP per group; each candidate's group score is every member's fmaf chain (the order of
+// score_rows_kernel) in member order, folded by the exact rule (agg_*).  Member rows are warp-uniform loads from L1 / L2.
+__global__ void __launch_bounds__(256) rescore_topk_group_kernel(const float* __restrict__ U, long long ldu, const float* __restrict__ I,
+                                                                 long long ldi, const int* __restrict__ grp_rowptr, const int* __restrict__ members,
+                                                                 int n_groups, int d, int agg, const int* __restrict__ cand_idx, int n_cand, int K,
+                                                                 int* __restrict__ out_idx, float* __restrict__ out_val) {
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  const int g = blockIdx.x * 8 + w;
+  if (g >= n_groups) return;
+  const int m0 = __ldg(grp_rowptr + g), m1 = __ldg(grp_rowptr + g + 1);
+  const int* ci = cand_idx + (long long)g * n_cand;
+  float sc[kMaxCandPerLane]; int id[kMaxCandPerLane];
 #pragma unroll
-    for (int q = 0; q < kMaxCandPerLane; ++q) {
-      if (id[q] >= 0 && sc[q] != -INFINITY && (sc[q] > best || (sc[q] == best && id[q] < besti))) { best = sc[q]; besti = id[q]; bestq = q; }
+  for (int q = 0; q < kMaxCandPerLane; ++q) {
+    const int c = q * 32 + lane;
+    const int item = c < n_cand ? ci[c] : -1;
+    float v = -INFINITY;
+    if (item >= 0) {
+      const float* it = I + (long long)item * ldi;
+      v = agg_start(agg);
+      for (int m = m0; m < m1; ++m) {
+        const float* u = U + (long long)__ldg(members + m) * ldu;
+        float a = 0.f;
+        for (int j = 0; j < d; ++j) a = fmaf(__ldg(u + j), __ldg(it + j), a);
+        v = agg_fold(agg, v, a);
+      }
+      v = agg_end(agg, v, m1 - m0);
     }
-    float wb = best; int wi = besti;
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-      const float ov = __shfl_xor_sync(0xffffffffu, wb, o); const int oi = __shfl_xor_sync(0xffffffffu, wi, o);
-      if (ov > wb || (ov == wb && oi < wi)) { wb = ov; wi = oi; }
-    }
-    const bool ok = wi != 0x7fffffff;
-    if (lane == 0) {
-      out_idx[(long long)b * K + r] = ok ? wi : -1;
-      if (out_val) out_val[(long long)b * K + r] = ok ? wb : -INFINITY;
-    }
-    if (ok && bestq >= 0 && besti == wi) {   // the owning lane retires the winner (ids are unique per user)
-#pragma unroll
-      for (int q = 0; q < kMaxCandPerLane; ++q) if (q == bestq) id[q] = -1;
-    }
+    sc[q] = v; id[q] = item;
   }
+  warp_emit_topk(sc, id, K, lane, out_idx + (long long)g * K, out_val ? out_val + (long long)g * K : nullptr);
 }
 
 bool score_tc_supported(int d, int K, long long ldu, long long ldi, const void* U, const void* I) {
@@ -314,6 +398,40 @@ long long score_tc_scratch(int n_batch, int n_items, int d, int K) {
   return 2LL * n_items * d + 2LL * n_batch * splits * score_kc(K) + 64;
 }
 
+// The hi / lo copies of the catalog, the tensor maps, the pipeline depth and the launch of score_topk_tc_kernel<D, GROUP> over
+// row_tiles x P.splits CTAs; P's plan, operands and candidate buffers are set by the caller.
+template <bool GROUP>
+static int launch_select(ScoreParams& P, const float* I, long long ldi, const int* among, int n_items, int d, int row_tiles, float* Ihi,
+                         float* Ilo, cudaStream_t st) {
+  {
+    const long long n = (long long)n_items * d;
+    split_hi_lo_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(I, ldi, among, n_items, d, Ihi, Ilo);
+    LLMREC_CHECK_LAUNCH("split_hi_lo");
+  }
+  if (!make_tmap_2d_f32(&P.tmIhi, Ihi, (uint64_t)d, (uint64_t)n_items, (uint64_t)d * 4, SBK, SBN)) return 4;
+  if (!make_tmap_2d_f32(&P.tmIlo, Ilo, (uint64_t)d, (uint64_t)n_items, (uint64_t)d * 4, SBK, SBN)) return 4;
+  const size_t fixed = (size_t)2 * d * SBM * 4 /*A hi, lo*/ + (size_t)SBM * kStageLd * 4 + (size_t)P.Kc * SBM * 8 /*heaps*/ + 64 /*barriers*/ +
+                       (among ? SBN * 4 : 0) /*tile ids*/ + 1024 /*align*/;
+  int stages = (int)((227 * 1024 - fixed) / (2 * kTileI));
+  if (stages > 4) stages = 4;
+  LLMREC_CHECK_ARG(stages >= 2, "score_topk: not enough shared memory for the pipeline");
+  P.stages = stages;
+  const size_t smem = fixed + (size_t)stages * 2 * kTileI;
+  dim3 grid(row_tiles, P.splits);
+  switch (d) {
+#define LLMREC_CASE(W)                                                                                                               \
+  case W:                                                                                                                            \
+    LLMREC_CHECK_CUDA(cudaFuncSetAttribute(score_topk_tc_kernel<W, GROUP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
+    score_topk_tc_kernel<W, GROUP><<<grid, 128, smem, st>>>(P);                                                                      \
+    break;
+    LLMREC_CASE(32) LLMREC_CASE(64) LLMREC_CASE(96) LLMREC_CASE(128)
+#undef LLMREC_CASE
+    default: LLMREC_CHECK_ARG(false, "score_topk: no tensor-core kernel for d=%d", d);
+  }
+  LLMREC_CHECK_LAUNCH("score_topk_tc");
+  return 0;
+}
+
 // among: NULL (the catalog is I), or n_items ascending ids of rows of I (the catalog is those rows)
 int score_topk_tc(const float* U, long long ldu, const float* I, long long ldi, const int* users, int n_batch, const int* among, int n_items, int d,
                   const int* mask_rowptr, const int* mask_col, int K, int* out_idx, float* out_val, float* scratch, long long scratch_elems,
@@ -326,38 +444,81 @@ int score_topk_tc(const float* U, long long ldu, const float* I, long long ldi, 
   float* Ihi = scratch; float* Ilo = scratch + (long long)n_items * d;
   float* cval = Ilo + (long long)n_items * d;
   int* cidx = reinterpret_cast<int*>(cval + (long long)n_batch * P.splits * P.Kc);
-  {
-    const long long n = (long long)n_items * d;
-    split_hi_lo_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(I, ldi, among, n_items, d, Ihi, Ilo);
-    LLMREC_CHECK_LAUNCH("split_hi_lo");
-  }
-  if (!make_tmap_2d_f32(&P.tmIhi, Ihi, (uint64_t)d, (uint64_t)n_items, (uint64_t)d * 4, SBK, SBN)) return 4;
-  if (!make_tmap_2d_f32(&P.tmIlo, Ilo, (uint64_t)d, (uint64_t)n_items, (uint64_t)d * 4, SBK, SBN)) return 4;
   P.U = U; P.ldu = ldu; P.users = users; P.n_batch = n_batch; P.n_items = n_items; P.d = d; P.among = among;
   P.mask_rowptr = mask_rowptr; P.mask_col = mask_col; P.cand_idx = cidx; P.cand_val = cval;
-  const size_t fixed = (size_t)2 * d * SBM * 4 /*A hi, lo*/ + (size_t)SBM * kStageLd * 4 + (size_t)P.Kc * SBM * 8 /*heaps*/ + 64 /*barriers*/ +
-                       (among ? SBN * 4 : 0) /*tile ids*/ + 1024 /*align*/;
-  int stages = (int)((227 * 1024 - fixed) / (2 * kTileI));
-  if (stages > 4) stages = 4;
-  LLMREC_CHECK_ARG(stages >= 2, "score_topk: not enough shared memory for the pipeline");
-  P.stages = stages;
-  const size_t smem = fixed + (size_t)stages * 2 * kTileI;
-  dim3 grid((n_batch + SBM - 1) / SBM, P.splits);
-  switch (d) {
-#define LLMREC_CASE(W)                                                                                                    \
-  case W:                                                                                                                 \
-    LLMREC_CHECK_CUDA(cudaFuncSetAttribute(score_topk_tc_kernel<W>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
-    score_topk_tc_kernel<W><<<grid, 128, smem, st>>>(P);                                                                  \
-    break;
-    LLMREC_CASE(32) LLMREC_CASE(64) LLMREC_CASE(96) LLMREC_CASE(128)
-#undef LLMREC_CASE
-    default: LLMREC_CHECK_ARG(false, "score_topk: no tensor-core kernel for d=%d", d);
-  }
-  LLMREC_CHECK_LAUNCH("score_topk_tc");
+  if (int rc = launch_select<false>(P, I, ldi, among, n_items, d, (n_batch + SBM - 1) / SBM, Ihi, Ilo, st)) return rc;
   const int n_cand = P.splits * P.Kc;
   LLMREC_CHECK_ARG(n_cand <= 32 * kMaxCandPerLane, "score_topk: %d candidates per user exceed the rescoring capacity", n_cand);
   rescore_topk_kernel<<<(n_batch + 7) / 8, 256, (size_t)8 * d * sizeof(float), st>>>(U, ldu, I, ldi, users, n_batch, d, cidx, n_cand, K, out_idx, out_val);
   LLMREC_CHECK_LAUNCH("rescore_topk");
+  return 0;
+}
+
+// ---- groups ----------------------------------------------------------------------------------------------------------------
+// The tile plan of llmrec_score_topk_group_f32 from the host member CSR: groups in the order given, a new tile whenever the next
+// group does not fit the current one.  -> the plan's ints in one array: grp_rowptr [n_groups+1], gofs [n_groups],
+// tile_g0 [n_tiles+1], slot_pos [n_tiles * 64]; returns n_tiles.
+int group_tile_plan(const int* rp, int n_groups, std::vector<int>* plan) {
+  std::vector<int> gofs(n_groups), g0(1, 0), slots;
+  int fill = 0;
+  for (int g = 0; g < n_groups; ++g) {
+    const int n = rp[g + 1] - rp[g];
+    if (fill + n > SBM) {   // close the tile
+      slots.resize(slots.size() + (SBM - fill), -1);
+      g0.push_back(g);
+      fill = 0;
+    }
+    gofs[g] = fill;
+    for (int j = 0; j < n; ++j) slots.push_back(rp[g] + j);
+    fill += n;
+  }
+  if (fill > 0) { slots.resize(slots.size() + (SBM - fill), -1); g0.push_back(n_groups); }
+  const int n_tiles = (int)g0.size() - 1;
+  if (plan) {
+    plan->assign(rp, rp + n_groups + 1);
+    plan->insert(plan->end(), gofs.begin(), gofs.end());
+    plan->insert(plan->end(), g0.begin(), g0.end());
+    plan->insert(plan->end(), slots.begin(), slots.end());
+  }
+  return n_tiles;
+}
+
+static long long plan_elems(int n_groups, int n_tiles) { return ((2LL * n_groups + 2 + n_tiles + 1 + (long long)n_tiles * SBM) + 3) / 4 * 4; }
+
+long long score_tc_group_scratch(const int* rp, int n_groups, int n_items, int d, int K) {
+  const int n_tiles = group_tile_plan(rp, n_groups, nullptr);
+  int splits, tps;
+  score_plan(n_tiles * SBM, n_items, K, &splits, &tps);
+  return 2LL * n_items * d + 2LL * n_groups * splits * score_kc(K) + plan_elems(n_groups, n_tiles) + 64;
+}
+
+// rp: the HOST member CSR; members: device rows of U
+int score_topk_group_tc(const float* U, long long ldu, const float* I, long long ldi, const int* rp, const int* members, int n_groups,
+                        const int* among, int n_items, int d, const int* mask_rowptr, const int* mask_col, int K, int agg, int* out_idx,
+                        float* out_val, float* scratch, long long scratch_elems, cudaStream_t st) {
+  LLMREC_CHECK_ARG(scratch && scratch_elems >= score_tc_group_scratch(rp, n_groups, n_items, d, K), "score_topk_group: scratch too small");
+  std::vector<int> plan;
+  const int n_tiles = group_tile_plan(rp, n_groups, &plan);
+  ScoreParams P;
+  memset(&P, 0, sizeof(P));
+  score_plan(n_tiles * SBM, n_items, K, &P.splits, &P.tiles_per_split);
+  P.Kc = score_kc(K);
+  float* Ihi = scratch; float* Ilo = scratch + (long long)n_items * d;
+  float* cval = Ilo + (long long)n_items * d;
+  int* cidx = reinterpret_cast<int*>(cval + (long long)n_groups * P.splits * P.Kc);
+  int* dplan = cidx + (long long)n_groups * P.splits * P.Kc;
+  // pageable source: the copy is staged before this returns, so `plan` may go when it does
+  LLMREC_CHECK_CUDA(cudaMemcpyAsync(dplan, plan.data(), plan.size() * sizeof(int), cudaMemcpyHostToDevice, st));
+  P.grp_rowptr = dplan; P.gofs = dplan + n_groups + 1; P.tile_g0 = P.gofs + n_groups; P.slot_pos = P.tile_g0 + n_tiles + 1;
+  P.agg = agg;
+  P.U = U; P.ldu = ldu; P.users = members; P.n_batch = n_tiles * SBM; P.n_items = n_items; P.d = d; P.among = among;
+  P.mask_rowptr = mask_rowptr; P.mask_col = mask_col; P.cand_idx = cidx; P.cand_val = cval;
+  if (int rc = launch_select<true>(P, I, ldi, among, n_items, d, n_tiles, Ihi, Ilo, st)) return rc;
+  const int n_cand = P.splits * P.Kc;
+  LLMREC_CHECK_ARG(n_cand <= 32 * kMaxCandPerLane, "score_topk_group: %d candidates per group exceed the rescoring capacity", n_cand);
+  rescore_topk_group_kernel<<<(n_groups + 7) / 8, 256, 0, st>>>(U, ldu, I, ldi, P.grp_rowptr, members, n_groups, d, agg, cidx, n_cand, K, out_idx,
+                                                               out_val);
+  LLMREC_CHECK_LAUNCH("rescore_topk_group");
   return 0;
 }
 

@@ -518,6 +518,26 @@ class Trainer(object):
         mode = ops.SCORE_MODE.get(getattr(self.args, "proj_mode", "3xtf32"), 0)
         return recommend.run_top_k(hot, job, mode)
 
+    def recommend_groups(self, groups, K=10, agg="mean", exclude="train", new_items=None, among=None, exclude_items=None):
+        """-> (ids int64 [g x K], scores fp32 [g x K]) on the device: one list per group of trained users who choose together, ties to
+        the lowest item id, padded with -1 / -inf when fewer than K items are left.
+        groups: user-id lists or a (rowptr, col) pair, one row per group; repeats collapse and order does not matter; 1..64 distinct
+        members per group.  A group's score of an item, with s(u, i) the bits `score` returns: agg="mean" the fp32 sum of s(u, i) over
+        the members in ascending id, then one division by their number; "min" the least misery, "max" the most pleasure (exact; a NaN
+        member score makes the group's NaN).  An item whose group score is NaN or -inf is never returned.
+        exclude: "train" masks every member's training items and every new item whose list names a member; "none" masks nothing.
+        new_items / among: as for `recommend`.  exclude_items: per group, item ids to leave out on top of `exclude` (one row per group,
+        in the forms `recommend` takes).  K: 1..64, at most the catalog size and at most the number of distinct ids in `among`.
+        A group of one member [u] gets exactly `recommend(users=[u])`'s row, and a group's row does not depend on the other groups of
+        the call -- in --proj_mode 3xtf32 unless group scores closer than the tensor-core rounding straddle the selection's slack (the
+        slack follows the size of the call, as for `recommend`).  Every argument is checked before anything runs.  --proj_mode picks the
+        scoring mode; both give the same ids and bits under the same proviso."""
+        job = recommend.prepare_group_top_k(self.hot, self.graph.rowptr_u, self.graph.col_u, groups, K=K, agg=agg, exclude=exclude,
+                                            new_items=new_items, among=among, exclude_items=exclude_items)
+        hot = self._current_model()
+        mode = ops.SCORE_MODE.get(getattr(self.args, "proj_mode", "3xtf32"), 0)
+        return recommend.run_group_top_k(hot, job, mode)
+
     def fold_in(self, histories, known=None):
         """-> U_new [m x d]: the fused user representations of item-id histories (lists or a (rowptr, col) pair) under the current
         parameters; known: each history's trained user id or -1 (layer 0 = that user's ID embedding, or zero)."""
@@ -590,6 +610,12 @@ class Trainer(object):
         """--rerank_out: every user's candidate row (`candidate_indices` layout [n_users x C]) re-ranked by this model, nothing excluded,
         top K, pickled as a CPU int64 tensor [n_users x K] to `path` (atomically, as `write_candidates`)."""
         ids, _ = self.rerank(candidates, K=K)
+        return recommend.write_candidates(path, ids)
+
+    def write_groups(self, path, groups, K=10, agg="mean"):
+        """--groups_out: the top-K of every group of `groups` (--groups_in) under `agg`, each group's training items excluded, pickled
+        as a CPU int64 tensor [n_groups x K] to `path` (atomically, as `write_candidates`)."""
+        ids, _ = self.recommend_groups(groups, K=K, agg=agg, exclude="train")
         return recommend.write_candidates(path, ids)
 
     def write_candidates(self, path, K=10, among=None, diversity=None, pool=None):
@@ -686,6 +712,7 @@ def main(argv=None):
     if args.candidates_out and trainer.masked_mode:
         raise ValueError("--candidates_out needs a fixed model: not with --mask / --mask_rate > 0 / --drop_rate > 0")
     rerank_in, rerank_k = check_rerank_flags(args, trainer)
+    groups_in = check_groups_flags(args, trainer)
     ret = trainer.evaluate() if args.eval_only else trainer.train()
     if args.candidates_out:                                           # from the model in memory when the run ends
         trainer.write_candidates(args.candidates_out, args.candidates_k, among=cand_among, diversity=args.candidates_diversity,
@@ -695,6 +722,10 @@ def main(argv=None):
         trainer.write_rerank(args.rerank_out, rerank_in, rerank_k)
         trainer.logger.logging("rerank: %d users' candidates from %s, top-%d written to %s" % (trainer.n_users, args.rerank_in, rerank_k,
                                                                                               args.rerank_out))
+    if groups_in is not None:
+        trainer.write_groups(args.groups_out, groups_in, args.groups_k, args.groups_agg)
+        trainer.logger.logging("groups: top-%d (%s) of %d groups from %s written to %s" % (args.groups_k, args.groups_agg, groups_in[0].numel() - 1,
+                                                                                           args.groups_in, args.groups_out))
     return ret
 
 
@@ -735,6 +766,22 @@ def check_rerank_flags(args, trainer):
     K = int(cand.shape[1]) if args.rerank_k is None else args.rerank_k
     recommend.check_rerank_k(K)
     return cand, K
+
+
+def check_groups_flags(args, trainer):
+    """--groups_in / --groups_out / --groups_k / --groups_agg, checked before the first training step -> the groups ((rowptr, col) of
+    recommend.groups_csr), or None."""
+    g_in, g_out = getattr(args, "groups_in", None), getattr(args, "groups_out", None)
+    if not g_in and not g_out:
+        return None
+    if not (g_in and g_out):
+        raise ValueError("--groups_in and --groups_out go together: the file of groups and the file to write")
+    if trainer.masked_mode:
+        raise ValueError("--groups_in needs a fixed model: not with --mask / --mask_rate > 0 / --drop_rate > 0")
+    recommend.check_engine(trainer.hot)
+    recommend.check_k(getattr(args, "groups_k", 10), trainer.n_items)
+    recommend.check_agg(getattr(args, "groups_agg", "mean"))
+    return recommend.read_groups(g_in, trainer.n_users)
 
 
 if __name__ == "__main__":

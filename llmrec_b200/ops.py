@@ -592,6 +592,33 @@ def score_topk_among(U, I, users, among, mask_rowptr, mask_col, K, mode=0, want_
     return (idx, val) if want_vals else idx
 
 
+GROUP_AGG = {"mean": 0, "min": 1, "max": 2}     # LLMREC_AGG_MEAN / _MIN / _MAX
+GROUP_MAX_MEMBERS = 64     # one wgmma M tile: a group never straddles a tile of llmrec_score_topk_group_f32
+
+
+def score_topk_group(U, I, member_rowptr, members, among, mask_rowptr, mask_col, K, agg="mean", mode=0, want_vals=False):
+    """Top-K per group of users (llmrec_score_topk_group_f32): group g's members are rows members[member_rowptr[g] ..
+    member_rowptr[g+1]) of U (1..64, ascending, distinct; member_rowptr is read on the host), its score of an item the mean (fp32 sum
+    in member order, then one division), min or max of the members' exact chains (a NaN member makes it NaN).  among: None (the
+    catalog is I) or int32 device ids, strictly ascending; mask rows are indexed by group and hold global ids.  Ties -> lowest id;
+    NaN / -inf group scores never returned; padded with -1 / -inf."""
+    _mat(U); _mat(I)
+    if agg not in GROUP_AGG:
+        raise ValueError(f"agg = {agg!r}: one of {tuple(GROUP_AGG)}")
+    rp = member_rowptr.detach().to("cpu", torch.int32).contiguous()
+    ng, d = int(rp.numel()) - 1, int(I.shape[1])
+    ni = int(I.shape[0]) if among is None else int(among.numel())
+    idx = torch.empty((ng, K), dtype=torch.int32, device=U.device)
+    val = torch.empty((ng, K), dtype=torch.float32, device=U.device) if want_vals else None
+    scratch = _score_topk_scratch(int(N.lib().llmrec_score_topk_group_scratch(_p(rp), ng, ni, d, K, mode)), U.device)
+    N.check(N.lib().llmrec_score_topk_group_f32(_p(U), _ld(U), _p(I), _ld(I), _p(rp), _p(_i32(members, "members")), ng,
+                                                 _p(None if among is None else _i32(among, "among")), ni, d, _p(mask_rowptr), _p(mask_col),
+                                                 K, GROUP_AGG[agg], _p(idx), _p(val), mode, _p(scratch),
+                                                 scratch.numel() if scratch is not None else 0, _stream()), "score_topk_group")
+    _count(3)
+    return (idx, val) if want_vals else idx
+
+
 RERANK_MAX_K = 1024        # LLMREC_RERANK_MAX_K: the selection width of llmrec_rerank_f32
 
 

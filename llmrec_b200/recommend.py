@@ -22,6 +22,10 @@ of it by maximal marginal relevance with `ops.diversify` (llmrec_diversify_f32),
 Scores of given (user, item) pairs are `ops.score_pairs` (llmrec_score_pairs_f32) and re-ranking of given candidate lists is
 `ops.rerank` (llmrec_rerank_f32, K <= 1024): the same sequential fp32 chain as score_topk's returned scores, so the bits agree, and the
 same mask rows (`exclusion_mask`) for exclude="train".
+
+Group lists (`top_k_groups`) rank the catalog for sets of trained users who choose together, by the mean, minimum or maximum of the
+members' scores, with `ops.score_topk_group` (llmrec_score_topk_group_f32): every member is scored, the group scores are aggregated
+inside the scoring kernel and no score matrix is stored.  A group's mask row is the union of its members' rows (`group_rows`).
 """
 from __future__ import annotations
 
@@ -648,3 +652,127 @@ def explain(engine, train_rowptr, train_col, items, users=None, histories=None, 
     are folded in (repeats collapse; an unknown user has no ID layer, so own = 0) and new item j is target n_items + j.  top: None, or
     N in 1..64 to also select each target's N most helpful history items on the device.  -> Explanation."""
     return run_explain(engine, prepare_explain(engine, train_rowptr, train_col, items, users, histories, new_items, top))
+
+
+# ---- group recommendations ------------------------------------------------------------------------------------------------------
+GROUP_AGGS = tuple(ops.GROUP_AGG)
+
+
+def check_agg(agg):
+    if not isinstance(agg, str) or agg not in GROUP_AGGS:
+        raise ValueError(f"agg = {agg!r}: one of {GROUP_AGGS} (the mean of the members' scores, the least misery, the most pleasure)")
+    return agg
+
+
+def groups_csr(groups, n_users, what="groups"):
+    """Groups of trained users -- a sequence of user-id lists or a (rowptr, col) pair -- checked and made canonical: ids are integers in
+    [0, n_users), repeats collapse and members come in ascending id, each group has 1..64 distinct members (64 = one tile of the
+    scoring kernel).  -> (rowptr int64 CPU tensor [g+1], col int64 CPU tensor)."""
+    if isinstance(groups, tuple) and len(groups) == 2 and all(hasattr(a, "shape") for a in groups):
+        rp, col = _ids(groups[0], f"{what} rowptr"), _ids(groups[1], what)
+    else:
+        if isinstance(groups, (str, bytes)) or not hasattr(groups, "__iter__"):
+            raise ValueError(f"{what}: a sequence of user-id lists or a (rowptr, col) pair, got {type(groups).__name__}")
+        rows = []
+        for r in groups:
+            if isinstance(r, (str, bytes)) or not (hasattr(r, "shape") or hasattr(r, "__iter__")):
+                raise ValueError(f"{what}: each group is a list of user ids, got {type(r).__name__}")
+            rows.append(_ids(r if hasattr(r, "shape") else list(r), what))
+        rp = torch.zeros(len(rows) + 1, dtype=torch.int64)
+        rp[1:] = torch.cumsum(torch.tensor([r.numel() for r in rows], dtype=torch.int64), 0)
+        col = torch.cat(rows) if rows else torch.zeros(0, dtype=torch.int64)
+    R = history_matrix(rp, col, n_users, what=what, unit="user id")
+    sizes = np.diff(R.indptr)
+    if sizes.size and sizes.min() < 1:
+        raise ValueError(f"{what}: group {int(np.argmin(sizes))} is empty; a group has 1..{ops.GROUP_MAX_MEMBERS} members")
+    if sizes.size and sizes.max() > ops.GROUP_MAX_MEMBERS:
+        g = int(np.argmax(sizes))
+        raise ValueError(f"{what}: group {g} has {int(sizes[g])} distinct members; at most {ops.GROUP_MAX_MEMBERS} (one tile of the "
+                         "scoring kernel)")
+    return torch.from_numpy(R.indptr.astype(np.int64)), torch.from_numpy(R.indices.astype(np.int64))
+
+
+def group_rows(rowptr, col, members, member_rowptr, n_catalog):
+    """Row g = the sorted union of rows members[member_rowptr[g] .. member_rowptr[g+1]) of an int32 CSR (int64 CPU member_rowptr)
+    -> (rowptr, col) int32 on the CSR's device."""
+    dev = col.device
+    mrp, mcol = select_rows(rowptr, col, members.long())
+    mrp = mrp.long()
+    ng, nm = member_rowptr.numel() - 1, members.numel()
+    group_of = torch.repeat_interleave(torch.arange(ng, device=dev), (member_rowptr[1:] - member_rowptr[:-1]).to(dev))
+    owner = torch.repeat_interleave(torch.arange(nm, device=dev), mrp[1:] - mrp[:-1])
+    keys = torch.unique(group_of[owner] * n_catalog + mcol.long())                        # sorted: by group, then id
+    rp = torch.zeros(ng + 1, dtype=torch.long, device=dev)
+    rp[1:] = torch.cumsum(torch.bincount(keys // n_catalog, minlength=ng), 0)
+    return rp.to(torch.int32), (keys % n_catalog).to(torch.int32)
+
+
+def prepare_group_top_k(engine, train_rowptr, train_col, groups, K=10, agg="mean", exclude="train", new_items=None, among=None,
+                        exclude_items=None):
+    """Every check of `top_k_groups`, and its host-side inputs, before anything is launched: -> a dict for `run_group_top_k`."""
+    check_engine(engine)
+    Rn = new_items_csr(new_items, engine.nu)
+    n = engine.ni + (0 if Rn is None else Rn.shape[0])
+    dev = engine.E_u.device
+    S = None if among is None else catalog_ids(among, n, dev)
+    K = check_k(K, n) if S is None else check_k(K, S.numel(), "|among|")
+    check_agg(agg)
+    check_exclude(exclude)
+    extra = None if exclude_items is None else candidates_csr(exclude_items, n)
+    grp_rp, grp_col = groups_csr(groups, engine.nu)
+    ng = grp_rp.numel() - 1
+    if extra is not None and extra[0].numel() - 1 != ng:
+        raise ValueError(f"exclude_items: {extra[0].numel() - 1} rows for {ng} groups")
+    members = _i32(grp_col.numpy(), dev)
+    if exclude == "train":                                   # each member's training row and the new items naming it, united
+        urp, ucol = exclusion_mask(engine, train_rowptr, train_col, "train", Rn)
+        rp, col = group_rows(urp, ucol, members, grp_rp, n)
+    else:
+        rp, col = torch.zeros(ng + 1, dtype=torch.int32, device=dev), torch.zeros(0, dtype=torch.int32, device=dev)
+    if extra is not None:
+        rp, col = merge_rows(rp, col, extra[0], extra[1], n)
+    return dict(Rn=Rn, member_rowptr=grp_rp, members=members, mask_rowptr=rp, mask_col=col, K=K, agg=agg, among=S)
+
+
+def run_group_top_k(engine, job, mode=0):
+    """The launches of `top_k_groups` for a `prepare_group_top_k` job: the new items' fold-in, then one group launch per block of
+    groups holding at most USER_BLOCK members."""
+    I = _catalog(engine, job["Rn"])
+    grp_rp, members, mrp, K = job["member_rowptr"], job["members"], job["mask_rowptr"], job["K"]
+    ng, dev = grp_rp.numel() - 1, members.device
+    ids = torch.empty((ng, K), dtype=torch.int64, device=dev)
+    vals = torch.empty((ng, K), dtype=torch.float32, device=dev)
+    for s, e in _blocks(grp_rp, USER_BLOCK):
+        a, b = int(grp_rp[s]), int(grp_rp[e])
+        idx, v = ops.score_topk_group(engine.U, I, grp_rp[s:e + 1] - a, members[a:b], job["among"], mrp[s:e + 1], job["mask_col"], K,
+                                      agg=job["agg"], mode=mode, want_vals=True)
+        ids[s:e].copy_(idx)
+        vals[s:e].copy_(v)
+    return ids, vals
+
+
+def top_k_groups(engine, train_rowptr, train_col, groups, K=10, agg="mean", exclude="train", mode=0, new_items=None, among=None,
+                 exclude_items=None):
+    """Top-K for groups of trained users of a model whose last full `forward()` is current.  groups: user-id lists or a (rowptr, col)
+    pair (`groups_csr`: repeats collapse, members taken in ascending id, 1..64 per group).  A group's score of item i, with s(u, i) the
+    exact fp32 chain of `score_pairs`: agg="mean" the fp32 sum of s(u, i) over the members in ascending id, then one division by their
+    number; "min" / "max" the exact minimum / maximum (a NaN member score makes it NaN).  exclude: "train" masks every member's
+    training row and every new item whose list names a member; "none" masks nothing.  new_items / among / exclude_items (one row per
+    group) as in `top_k`.  -> (ids int64 [g x K], scores fp32 [g x K]) on the engine's device by (score desc, id asc); NaN and -inf
+    group scores are never returned; padded with -1 / -inf."""
+    job = prepare_group_top_k(engine, train_rowptr, train_col, groups, K, agg, exclude, new_items, among, exclude_items)
+    return run_group_top_k(engine, job, mode)
+
+
+def read_groups(path, n_users):
+    """The --groups_in file (a pickled sequence of trained-user-id lists, one per group) -> (rowptr, col) of `groups_csr`, checked: the
+    file loads, and every group holds 1..64 distinct ids in [0, n_users)."""
+    flag = f"--groups_in {path}"
+    try:
+        with open(os.fspath(path), "rb") as f:
+            groups = pickle.load(f)
+    except Exception as e:                                                  # noqa: BLE001 -- any unreadable file is a flag error
+        raise ValueError(f"{flag}: cannot read a pickled sequence of user-id lists ({type(e).__name__}: {e})") from e
+    if isinstance(groups, tuple) or not isinstance(groups, (list, np.ndarray, torch.Tensor)):
+        raise ValueError(f"{flag}: need a list (or 2-D array) of user-id lists, one per group, got {type(groups).__name__}")
+    return groups_csr(groups, n_users, flag)

@@ -114,6 +114,15 @@ _EXTRA = [
     ("rerank_out", dict(default=None, help="where --rerank_in's rows go, re-ranked by (score desc, id asc), nothing excluded, repeats kept "
                                            "once: the pickled CPU int64 tensor [n_users x --rerank_k], padded with -1, written atomically")),
     ("rerank_k", dict(type=int, default=None, help="list length of --rerank_out (1..1024; default: the width C of --rerank_in)")),
+    ("groups_in", dict(default=None, help="when the run ends, recommend for groups of users who choose together: a pickled list of "
+                                          "trained-user-id lists, one per group (1..64 distinct members each; repeats and order do not "
+                                          "matter). Needs --groups_out. Not with the mask / dropout branch")),
+    ("groups_out", dict(default=None, help="where --groups_in's lists go: each group's top --groups_k items under --groups_agg, every "
+                                           "member's training items excluded, as the pickled CPU int64 tensor [n_groups x K], padded "
+                                           "with -1, written atomically")),
+    ("groups_k", dict(type=int, default=10, help="list length of --groups_out (1..64, at most n_items)")),
+    ("groups_agg", dict(default="mean", choices=["mean", "min", "max"], help="group score of --groups_out: the mean of the members' "
+                                                                             "scores, the least misery (min) or the most pleasure (max)")),
 ]
 
 DATASET_ALIASES = {"netflix": "netflix_valid_item", "movielens": "preprocessed_raw_MovieLens", "movieLens": "preprocessed_raw_MovieLens"}
