@@ -5,7 +5,7 @@
       the grouped projections at the training step's own shapes: the item tables on the live items, their weight gradient paired
       with column blocks of GPi through the sorted live-row map, the user table in full (netflix d = 64, movielens d = 128), for
       fp32 and bf16 tables and modes 0 and 1.  Each group is replayed from its own CUDA graph between CUDA events (median of
-      5 x 50 replays).  --dump writes dW / db of every set, --compare checks them bit for bit against a dump; --lib-root imports
+      5 x 50 replays).  --dump writes Y, dW and db of every set, --compare checks them bit for bit against a dump; --lib-root imports
       the package from another tree (e.g. a worktree of an earlier commit, built) so that two builds see the same inputs.
 """
 import argparse, os, subprocess, sys
@@ -148,8 +148,9 @@ if which == "step":
                 d_, fw, wg, grads, gradb = step_problems(name, dtype)
                 t_fwd = graph_ms(lambda: ops.proj_fwd_group(fw, d_, m))
                 t_wg = graph_ms(lambda: ops.proj_wgrad_group(wg, d_, m))
-                ops.proj_wgrad_group(wg, d_, m); torch.cuda.synchronize()
+                ops.proj_fwd_group(fw, d_, m); ops.proj_wgrad_group(wg, d_, m); torch.cuda.synchronize()
                 res = {f"dW_{k}": v.cpu() for k, v in grads.items()} | {f"db_{k}": v.cpu() for k, v in gradb.items()}
+                res |= {f"Y_{j}": f[3].cpu() for j, f in enumerate(fw)}
                 line = f"{tag}: proj_fwd {t_fwd:.4f} ms  proj_wgrad {t_wg:.4f} ms"
                 if args.dump:
                     os.makedirs(args.dump, exist_ok=True)
@@ -158,7 +159,7 @@ if which == "step":
                     ref = torch.load(os.path.join(args.compare, tag + ".pt"))
                     diff = [k for k in ref if not torch.equal(ref[k].view(torch.int32), res[k].view(torch.int32))]
                     bad += len(diff)
-                    line += "  dW/db bit-identical" if not diff else f"  DIFFERENT: {diff}"
+                    line += "  Y/dW/db bit-identical" if not diff else f"  DIFFERENT: {diff}"
                 print(line, flush=True)
     if bad:
         sys.exit(1)
