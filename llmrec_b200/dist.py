@@ -387,6 +387,18 @@ class ShardedHotPath:
         self.opt.step_tensor(1, self.g_Ei)
         return self.loss
 
+    def step_grads(self):
+        """The gradients the last train_step handed to AdamW -> (this rank's user rows [nu x d], item rows, first item row).
+        The demand step's user gradient is row-sparse: AdamW reads g_Eu on the batch rows only, so every other row reads zero here.
+        With the item table's optimizer sharded (item_sharded, item_opt_sharded) the item gradient holds this rank's rows [ilo, ihi).
+        For tests; it launches nothing inside a step."""
+        g_u = self.g_Eu
+        if self.demand:
+            bits = (self.batchU.mask.to(torch.int64) & 0xffffffff)[:, None] >> torch.arange(32, device=g_u.device)
+            keep = (bits & 1).reshape(-1)[:self.nu].bool()
+            g_u = torch.where(keep[:, None], g_u, torch.zeros_like(g_u))
+        return g_u, self.g_Ei, (self.ilo if (self.item_sharded or self.item_opt_sharded) else 0)
+
     def train_step(self, users, pos, neg):
         if self.demand:
             return self._train_step_demand(users, pos, neg)

@@ -13,8 +13,11 @@ Exchanges per step (L layers, S = 2 + #attribute tables feature blocks of d colu
 Item-side gradients that come straight from the loss (heads, feat_reg, fusion) are identical on every rank and are added ONCE,
 after the cross-rank sum.  The schedule mirrors engine.HotPath line by line; world size 1 reproduces it.
 
-Status: the orchestration is verified on CPU (tests/test_dist_feat_emulated.py: world-size-1/2 gloo, torch stand-ins for the
-kernels, against the oracle); it has not run on GPUs yet and no benchmark uses it.
+Status: runs on the H100 at world 1 (tests/test_dist_gpu.py against engine.HotPath; tests/test_dist_fp64_gpu.py holds every
+gradient, loss head and AdamW update of five-step runs to the fp64 step model in proj_mode 0 and 2).  World 2 over NCCL is in the
+same tests and needs two visible GPUs; on CPU the orchestration runs at world 1/2/3 under gloo with torch stand-ins for the kernels
+(tests/test_dist_feat_emulated.py against the oracle, tests/test_dist_fp64_cpu.py against the fp64 step model, even and uneven item
+ranges).  No benchmark uses it.
 """
 from __future__ import annotations
 

@@ -8,7 +8,8 @@ project's float64 normalisation.  Feature tables enter at their exact values (fp
 
 Heads: "mf" and "emb" of the ID head (main.py:232-235), "img" and "txt" (x mm_mf_rate), one "aug:<key>" per attribute key
 (x aug_mf_rate), "feat" (feat_reg, main.py:151-156) and, in the mask branch, "restore" (x att_re_rate, main.py:258-271).  Each
-head's gradient is its own `autograd.grad`, so the bound below can weigh each head by its own size.
+head's gradient is its own `autograd.grad`, so the bound below can weigh each head by its own size.  With feats=None the step is
+the ID-only configuration of dist.ShardedHotPath (no feature tables, params = the two ID tables): `id_forward`, heads "mf" / "emb".
 
 Kept sets: each BPR head keeps the n_keep = int((1 - rate) * B') smallest maxi (stable argsort, ties to the lower position, as the
 kernel).  `StepRef.cuts[head]` = (gap, need): the fp64 gap of x = <u, p> - <u, n> + 1e-8 between the largest kept and the
@@ -112,6 +113,22 @@ def engine_inputs(hp, device=None):
     return p, feats, sparse64(hp.ui, dev), sparse64(hp.iu, dev)
 
 
+def id_forward(params, ui, iu, cfg: O.OracleConfig) -> dict:
+    """The ID-only forward: the propagation and layer mean of `oracle.llmrec_oracle.forward` (Models.py:172-186) with no side term."""
+    e_u, e_i = params["user_id_embedding.weight"], params["item_id_embedding.weight"]
+    us, its = [e_u], [e_i]
+    L = cfg.n_ui_layers
+    for l in range(L):
+        e_u = torch.mm(ui, e_i)
+        if l == L - 1:
+            e_u = torch.softmax(e_u, dim=-1)
+        e_i = torch.mm(iu, e_u)
+        if l == L - 1:
+            e_i = torch.softmax(e_i, dim=-1)
+        us.append(e_u); its.append(e_i)
+    return dict(U=torch.mean(torch.stack(us), dim=0), I=torch.mean(torch.stack(its), dim=0))
+
+
 @dataclass
 class StepRef:
     loss: float                     # total
@@ -157,6 +174,8 @@ def reference(params, feats, ui, iu, cfg: O.OracleConfig, users, pos, neg, n_ite
     u_mask, alpha, kind) for the restoration head.  dtype=float32 gives the fp32 oracle (calibration); proj="3xtf32" / "tf32" gives it
     the projection arithmetic of those tensor-core modes.
 
+    feats=None: the ID-only step (`id_forward`, the "mf" and "emb" heads only).
+
     The remaining keywords are mutations of the step, for the tests that show the bound can see them: drop_heads (head names
     left out), n_keep (instead of int((1 - rate) * B')), reg_div (instead of cfg.batch_size), feat_div (instead of n_items),
     detach_last (the last triplet's rows get no gradient from any BPR head), softmax_identity (the last layer's softmax Jacobian
@@ -164,7 +183,8 @@ def reference(params, feats, ui, iu, cfg: O.OracleConfig, users, pos, neg, n_ite
     dev = next(iter(params.values())).device
     cast = lambda t: t.to(dev, dtype)
     P = {k: cast(v).detach().requires_grad_(True) for k, v in params.items()}
-    X = dict(image=cast(feats["image"]), text=cast(feats["text"]), user=cast(feats["user"]), item={k: cast(v) for k, v in feats["item"].items()})
+    X = None if feats is None else \
+        dict(image=cast(feats["image"]), text=cast(feats["text"]), user=cast(feats["user"]), item={k: cast(v) for k, v in feats["item"].items()})
     ui_, iu_ = cast(ui), cast(iu)
     dr = None if drop is None else [cast(m) for m in drop]
     idx = lambda a: torch.as_tensor(a, dtype=torch.long).to(dev)
@@ -176,13 +196,14 @@ def reference(params, feats, ui, iu, cfg: O.OracleConfig, users, pos, neg, n_ite
                              reg_div, feat_div, detach_last, softmax_identity)
     B = int(u.numel())
     keep_n = int((1 - cfg.prune_loss_drop_rate) * B) if n_keep is None else int(n_keep)
+    fwd = (lambda: id_forward(P, ui_, iu_, cfg)) if X is None else (lambda: O.forward(P, X, ui_, iu_, cfg, drop=dr))
     if softmax_identity:                 # softmax's value, the identity as its Jacobian (O.forward calls torch.softmax on layer L only)
         sm = torch.softmax
         fake = lambda x, dim=-1: x + (sm(x, dim=dim) - x).detach()
         with unittest.mock.patch.object(torch, "softmax", fake):
-            out = O.forward(P, X, ui_, iu_, cfg, drop=dr)
+            out = fwd()
     else:
-        out = O.forward(P, X, ui_, iu_, cfg, drop=dr)
+        out = fwd()
 
     def rows(T, ix):
         G = T[ix]
@@ -208,6 +229,19 @@ def reference(params, feats, ui, iu, cfg: O.OracleConfig, users, pos, neg, n_ite
     mf, emb = bpr("mf", out["U"], out["I"])
     losses["mf"], losses["emb"] = mf, emb
     head_out["mf"] = (float(mf), float(emb))
+    if X is None:                        # the ID-only step: no side heads, no projections
+        for h in drop_heads:
+            losses.pop(h)
+        names = list(P)
+        grads = {k: torch.zeros_like(P[k]) for k in names}
+        per_head, mag = {}, {k: torch.zeros_like(P[k]) for k in names}
+        for h, L in losses.items():
+            g = torch.autograd.grad(L, [P[k] for k in names], retain_graph=True)
+            per_head[h] = {k: gg.detach() for k, gg in zip(names, g)}
+            for k in names:
+                grads[k] += per_head[h][k]; mag[k] += per_head[h][k].abs()
+        return StepRef(loss=sum(float(L) for L in losses.values()), parts={h: float(L) for h, L in losses.items()}, head_out=head_out,
+                       grads=grads, per_head=per_head, mag=mag, cuts=cuts, n_keep=keep_n, B=B)
     for name, su, si in (("img", "img_u", "img_i"), ("txt", "txt_u", "txt_i")):
         m, e = bpr(name, out[su], out[si])
         losses[name] = cfg.mm_mf_rate * m
